@@ -277,10 +277,6 @@ int sb_apply_time_channel(const float* d_x, const float* d_h, const float* d_no,
 int sb_tdl_sos(const float* d_doppler, const float* d_theta, const float* d_phi, const float* d_phi0,
                const float* d_powers, float los_power, float los_aoa, float* d_a, int64_t batch, int32_t num_ant_pairs,
                int32_t num_paths, int32_t num_sinusoids, int32_t num_time_steps, float sampling_frequency, void* stream);
-/* cir_to_ofdm_channel (channel/utils.py:180-253) for delays shared by all links: d_a [rows, paths, time_steps] complex,
- * d_e [paths, subcarriers] = exp(-j 2 pi f tau) -> d_h [rows, time_steps, subcarriers]. */
-int sb_cir_to_ofdm(const float* d_a, const float* d_e, float* d_h, int64_t rows, int32_t num_paths,
-                   int32_t num_time_steps, int32_t num_subcarriers, void* stream);
 /* CIR -> channel conversion without eager tensor expressions (channel/utils.py:180-350), csrc/channel.cu.
  * sb_phase_table: d_e [n_tab, paths, cols] complex; mode 0: exp(-j 2 pi x_j tau[tab, p]) (x = subcarrier frequencies,
  *   cir_to_ofdm_channel :232-244); mode 1: sinc(x_j - tau[tab, p] * scale) (x = tap lags l, scale = bandwidth,

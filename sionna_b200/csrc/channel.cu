@@ -1,12 +1,15 @@
-// channel.cu -- on-device channel generation helpers for sm_90a (SURVEY.md section 8 row f3), second part: everything
-// the CIR -> channel conversion needs so that no step of it runs as an eager tensor expression. Replaces (paths under
-// /root/reference/src/sionna/phy/):
-//   sb_phase_table     exp(-j 2 pi f tau) of cir_to_ofdm_channel   channel/utils.py:232-244
-//                      sinc(l - tau W)    of cir_to_time_channel   channel/utils.py:318-338
-//   sb_cir_gram        (no counterpart: Gram matrix of the table, used to normalise without a second pass over h)
-//   sb_cir_link_scale  normalisation factor of channel/utils.py:246-251 (OFDM) and :341-348 (time)
-//   sb_cir_apply       h = sum_p a_p e_p (channel/utils.py:240-244, 336-338), per-link tables and scaling folded in
-//   sb_spatial_corr    TDL._apply_correlation (channel/tr38901/tdl.py:466-490): v' = L v per (batch, path, time step)
+// channel.cu -- on-device channel generation and application for sm_90a (SURVEY.md section 8 row f3): the TDL taps,
+// everything the CIR -> channel conversion needs so that no step of it runs as an eager tensor expression, and the
+// channel applied to a signal. Replaces (paths under /root/reference/src/sionna/phy/):
+//   sb_tdl_sos            TDL.__call__ sum of sinusoids      channel/tr38901/tdl.py:372-456
+//   sb_phase_table        exp(-j 2 pi f tau) of cir_to_ofdm_channel   channel/utils.py:232-244
+//                         sinc(l - tau W)    of cir_to_time_channel   channel/utils.py:318-338
+//   sb_cir_gram           (no counterpart: Gram matrix of the table, used to normalise without a second pass over h)
+//   sb_cir_link_scale     normalisation factor of channel/utils.py:246-251 (OFDM) and :341-348 (time)
+//   sb_cir_apply          h = sum_p a_p e_p (channel/utils.py:240-244, 336-338), per-link tables and scaling folded in
+//   sb_spatial_corr       TDL._apply_correlation (channel/tr38901/tdl.py:466-490): v' = L v per (batch, path, time step)
+//   sb_apply_ofdm_channel ApplyOFDMChannel.call   channel/apply_ofdm_channel.py:70-80
+//   sb_apply_time_channel ApplyTimeChannel.call   channel/apply_time_channel.py:115-137
 //
 // Normalisation without touching h twice. The reference computes c = sqrt(mean |h|^2) over (rx ant, tx ant, time,
 // frequency) per link from the finished tensor and divides. Because h[f] = sum_p a_p e[p, f],
@@ -15,16 +18,10 @@
 // model): sb_cir_link_scale evaluates that quadratic form (P^2 MACs per (antenna pair, time step) instead of reading
 // F * 8 bytes) and sb_cir_apply writes the already scaled h exactly once. Every reduction runs in a fixed order
 // (no atomics): results are reproducible bit for bit from run to run.
-#include <algorithm>
 #include "sb_common.h"
+#include "rng.cuh"
 
 namespace {
-
-__device__ __forceinline__ float2 cmul_(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-
-inline int grid_cap(long long blocks) {
-    return (int)std::max<long long>(1, std::min<long long>(blocks, (long long)sb_num_sms() * 16));
-}
 
 // e[tab, p, j]: mode 0: exp(-j 2 pi x_j tau[tab, p]); mode 1: sinc(x_j - tau[tab, p] * scale) (+ 0 j).
 // The phase is reduced in double precision (f tau reaches a few turns) and evaluated with sincospi.
@@ -111,7 +108,7 @@ __global__ void cir_link_scale_kernel(const float2* __restrict__ a, const float2
                     const float2 y = ap[(size_t)q * d.T];
                     const float2 gq = s_g[p * d.P + q];             // sum_f e_p conj(e_q)
                     // terms (p, q) and (q, p) together: 2 Re( a_p conj(a_q) G[p, q] )
-                    const float2 cy = cmul_(x, make_float2(y.x, -y.y));
+                    const float2 cy = cmul(x, make_float2(y.x, -y.y));
                     s.x += cy.x * gq.x - cy.y * gq.y;
                 }
                 e += 2.f * s.x;
@@ -209,7 +206,7 @@ int launch_cir_apply(const float2* a, const float2* e, long long e_link_stride, 
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int tiles_t = (d.T + TILE_T - 1) / TILE_T, tiles_f = (F + TILE_F - 1) / TILE_F;
     const long long R = d.B * d.RX * d.RA * d.TX * d.TA;
-    kern<<<grid_cap(R * tiles_t * tiles_f), (TILE_T / RT) * (TILE_F / RJ), smem, stream>>>(a, e, e_link_stride, scale, h, d, F,
+    kern<<<sb_grid(R * tiles_t * tiles_f, 1, 16), (TILE_T / RT) * (TILE_F / RJ), smem, stream>>>(a, e, e_link_stride, scale, h, d, F,
                                                                                          tiles_t, tiles_f);
     return SB_OK;
 }
@@ -228,7 +225,7 @@ __global__ void spatial_corr_kernel(const float2* __restrict__ in, const float2*
         for (int r = 0; r < n; ++r) {
             float2 acc = make_float2(0.f, 0.f);
             for (int j = 0; j <= r; ++j) {                         // L is lower triangular (Cholesky factor)
-                const float2 v = cmul_(s_l[r * n + j], ip[(size_t)j * cols]);
+                const float2 v = cmul(s_l[r * n + j], ip[(size_t)j * cols]);
                 acc.x += v.x;
                 acc.y += v.y;
             }
@@ -237,7 +234,137 @@ __global__ void spatial_corr_kernel(const float2* __restrict__ in, const float2*
     }
 }
 
+// TDL tap gains by the sum-of-sinusoids model: for link b, antenna pair a (rx-major), path p, time step t
+//   a = sqrt(P_p / Ns) sum_n exp(j (w_b t/fs cos(2 pi (n+1)/Ns + theta[b,p,n]) + phi[b,a,p,n]))
+//       (+ sqrt(P_los) exp(j (w_b t/fs cos(aoa) + phi0[b])) on path 0 of the LoS models)
+// One thread per (b, a, p) row. Time is processed in chunks of 16 steps held in registers: per sinusoid one cos for the
+// angular rate, one sincos for the phasor at the chunk start and one for the per-step rotation, then 16 complex
+// multiplications (the recurrence is re-anchored every chunk, so its rounding error stays below 1e-6).
+constexpr int kSosChunk = 16;
+__device__ __forceinline__ void sos_accumulate(float2* acc, float rate, float phase, int t0) {
+    float s0, c0, sd, cd;
+    sincosf(rate * (float)t0 + phase, &s0, &c0);
+    sincosf(rate, &sd, &cd);
+    float2 z = make_float2(c0, s0);
+    const float2 step = make_float2(cd, sd);
+#pragma unroll
+    for (int i = 0; i < kSosChunk; ++i) {
+        acc[i].x += z.x;
+        acc[i].y += z.y;
+        z = cmul(z, step);
+    }
+}
+__global__ void tdl_sos_kernel(const float* __restrict__ doppler, const float* __restrict__ theta,
+                               const float* __restrict__ phi, const float* __restrict__ phi0,
+                               const float* __restrict__ powers, float los_power, float los_aoa, float2* __restrict__ out,
+                               long long B, int A, int P, int Ns, int T, float fs) {
+    const long long rows = B * A * P;                            // (b, a, p)
+    for (long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x; row < rows; row += (long long)gridDim.x * blockDim.x) {
+        const int p = (int)(row % P);
+        const long long b = row / ((long long)P * A);
+        const float wd = doppler[b] / fs;                        // radians per time step at cos = 1
+        const float* th = theta + (b * P + p) * (long long)Ns;
+        const float* ph = phi + row * (long long)Ns;
+        const float amp = sqrtf(powers[p]) * (1.0f / sqrtf((float)Ns));
+        const bool los = phi0 != nullptr && p == 0;
+        const float la = los ? sqrtf(los_power) : 0.f;
+        for (int t0 = 0; t0 < T; t0 += kSosChunk) {
+            float2 acc[kSosChunk];
+#pragma unroll
+            for (int i = 0; i < kSosChunk; ++i) acc[i] = make_float2(0.f, 0.f);
+            for (int n = 0; n < Ns; ++n) {
+                const float alpha = 6.283185307179586f / (float)Ns * (float)(n + 1) + th[n];
+                sos_accumulate(acc, wd * cosf(alpha), ph[n], t0);
+            }
+            float2 spec[kSosChunk];
+#pragma unroll
+            for (int i = 0; i < kSosChunk; ++i) spec[i] = make_float2(0.f, 0.f);
+            if (los) sos_accumulate(spec, wd * cosf(los_aoa), phi0[b], t0);
+#pragma unroll
+            for (int i = 0; i < kSosChunk; ++i)
+                if (t0 + i < T) out[row * T + t0 + i] = make_float2(acc[i].x * amp + la * spec[i].x, acc[i].y * amp + la * spec[i].y);
+        }
+    }
+}
+
+// ApplyOFDMChannel: y[b, r, re] = sum_t h[b, r, t, re] * x[b, t, re] + sqrt(no) CN(0,1)   (r = rx*ant, t = tx*ant)
+__global__ void apply_ofdm_channel_kernel(const float2* __restrict__ x, const float2* __restrict__ h,
+                                          const float* __restrict__ no, long long no_inner, float2* __restrict__ y,
+                                          long long B, int R, int Tt, int RE, int add_noise, unsigned long long seed,
+                                          unsigned long long offset) {
+    const long long rows = B * R;
+    for (long long row = (long long)blockIdx.x * blockDim.y + threadIdx.y; row < rows; row += (long long)gridDim.x * blockDim.y) {
+        const long long b = row / R;
+        const float2* hp = h + row * (long long)Tt * RE;
+        const float2* xp = x + b * (long long)Tt * RE;
+        const long long obase = row * (long long)RE;
+        const bool row_no = add_noise && (no_inner % RE) == 0;      // one noise power per row (the usual case)
+        const float sd_row = row_no ? sqrtf(no[obase / no_inner]) * 0.70710678118654752f : 0.f;
+        for (int re = threadIdx.x; re < RE; re += blockDim.x) {
+            float2 acc = make_float2(0.f, 0.f);
+            for (int t = 0; t < Tt; ++t) acc = cadd(acc, cmul(hp[(size_t)t * RE + re], xp[(size_t)t * RE + re]));
+            if (add_noise) {
+                const unsigned long long i = (unsigned long long)(obase + re);    // same Philox counter as the flat index
+                uint4 rr = philox4x32_10(seed, offset, i);
+                float2 g = box_muller(rr.x, rr.y);
+                float sd = row_no ? sd_row : sqrtf(no[i / (unsigned long long)no_inner]) * 0.70710678118654752f;
+                acc.x += g.x * sd;
+                acc.y += g.y * sd;
+            }
+            y[obase + re] = acc;
+        }
+    }
+}
+
+// ApplyTimeChannel (channel/apply_time_channel.py:115-137): time-variant FIR filtering
+//   y[b, r, n] = sum_t sum_l h[b, r, t, n, l] x[b, t, n - l]   (x = 0 outside [0, N)),  n in [0, N + L - 1)
+// r = (rx, rx_ant), t = (tx, tx_ant). A CTA row is (b, r); threads walk the output samples.
+__global__ void apply_time_channel_kernel(const float2* __restrict__ x, const float2* __restrict__ h,
+                                          const float* __restrict__ no, long long no_inner, float2* __restrict__ y,
+                                          long long B, int R, int Tt, int N, int L, int add_noise, unsigned long long seed,
+                                          unsigned long long offset) {
+    const int NO = N + L - 1;
+    const long long rows = B * R;
+    for (long long row = (long long)blockIdx.x * blockDim.y + threadIdx.y; row < rows; row += (long long)gridDim.x * blockDim.y) {
+        const long long b = row / R;
+        const long long obase = row * (long long)NO;
+        for (int n = threadIdx.x; n < NO; n += blockDim.x) {
+            float2 acc = make_float2(0.f, 0.f);
+            for (int t = 0; t < Tt; ++t) {
+                const float2* hp = h + ((row * Tt + t) * (long long)NO + n) * L;
+                const float2* xp = x + (b * Tt + t) * (long long)N;
+                const int l0 = n - (N - 1) > 0 ? n - (N - 1) : 0;     // n - l <= N - 1
+                const int l1 = n < L - 1 ? n : L - 1;                  // n - l >= 0
+                for (int l = l0; l <= l1; ++l) acc = cadd(acc, cmul(hp[l], xp[n - l]));
+            }
+            if (add_noise) {
+                const unsigned long long i = (unsigned long long)(obase + n);
+                uint4 rr = philox4x32_10(seed, offset, i);
+                float2 g = box_muller(rr.x, rr.y);
+                float sd = sqrtf(no[i / (unsigned long long)no_inner]) * 0.70710678118654752f;
+                acc.x += g.x * sd;
+                acc.y += g.y * sd;
+            }
+            y[obase + n] = acc;
+        }
+    }
+}
+
 }  // namespace
+
+extern "C" int sb_tdl_sos(const float* d_doppler, const float* d_theta, const float* d_phi, const float* d_phi0,
+                          const float* d_powers, float los_power, float los_aoa, float* d_a, int64_t batch,
+                          int32_t num_ant_pairs, int32_t num_paths, int32_t num_sinusoids, int32_t num_time_steps,
+                          float sampling_frequency, void* stream) {
+    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    SB_CHECK_ARG(d_doppler && d_theta && d_phi && d_powers && d_a && num_ant_pairs > 0 && num_paths > 0 &&
+                     num_sinusoids > 0 && num_time_steps > 0 && sampling_frequency > 0.f, "sb_tdl_sos: bad arguments");
+    tdl_sos_kernel<<<sb_grid(batch * num_ant_pairs * num_paths, 128, 16), 128, 0, (cudaStream_t)stream>>>(
+        d_doppler, d_theta, d_phi, d_phi0, d_powers, los_power, los_aoa, (float2*)d_a, batch, num_ant_pairs, num_paths,
+        num_sinusoids, num_time_steps, sampling_frequency);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
 
 extern "C" int sb_phase_table(const float* d_tau, const float* d_x, float scale, int32_t mode, float* d_e, int64_t n_tab,
                               int32_t num_paths, int32_t num_cols, void* stream) {
@@ -245,7 +372,7 @@ extern "C" int sb_phase_table(const float* d_tau, const float* d_x, float scale,
     SB_CHECK_ARG(d_tau && d_x && d_e && n_tab > 0 && num_paths > 0 && num_cols > 0 && (mode == 0 || mode == 1),
                  "sb_phase_table: bad arguments");
     const long long total = n_tab * num_paths * (long long)num_cols;
-    phase_table_kernel<<<grid_cap((total + 255) / 256), 256, 0, (cudaStream_t)stream>>>(d_tau, d_x, (float2*)d_e, n_tab,
+    phase_table_kernel<<<sb_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(d_tau, d_x, (float2*)d_e, n_tab,
                                                                                        num_paths, num_cols, scale, mode);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -255,7 +382,7 @@ extern "C" int sb_cir_gram(const float* d_e, float* d_g, int64_t n_tab, int32_t 
     if (n_tab == 0) return SB_OK;
     SB_CHECK_ARG(d_e && d_g && n_tab > 0 && num_paths > 0 && num_cols > 0, "sb_cir_gram: bad arguments");
     const long long warps = n_tab * num_paths * (long long)num_paths;
-    cir_gram_kernel<<<grid_cap((warps + 7) / 8), 256, 0, (cudaStream_t)stream>>>((const float2*)d_e, (float2*)d_g, n_tab,
+    cir_gram_kernel<<<sb_grid(warps, 8, 16), 256, 0, (cudaStream_t)stream>>>((const float2*)d_e, (float2*)d_g, n_tab,
                                                                                 num_paths, num_cols);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -274,7 +401,7 @@ extern "C" int sb_cir_link_scale(const float* d_a, const float* d_g, int64_t g_l
     CirDims d{batch, num_rx, num_rx_ant, num_tx, num_tx_ant, num_paths, num_time_steps};
     const long long links = batch * num_rx * (long long)num_tx;
     const size_t smem = sizeof(float2) * (size_t)num_paths * num_paths;
-    cir_link_scale_kernel<<<grid_cap(links), 256, smem, (cudaStream_t)stream>>>((const float2*)d_a, (const float2*)d_g,
+    cir_link_scale_kernel<<<sb_grid(links, 1, 16), 256, smem, (cudaStream_t)stream>>>((const float2*)d_a, (const float2*)d_g,
                                                                                 g_link_stride, d_scale, d, denom);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -308,8 +435,39 @@ extern "C" int sb_spatial_corr(const float* d_in, const float* d_l, float* d_out
     const long long total = batch * cols;
     const size_t smem = sizeof(float2) * (size_t)n * n;
     if (smem > 48 * 1024) SB_CUDA(cudaFuncSetAttribute(spatial_corr_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    spatial_corr_kernel<<<grid_cap((total + 127) / 128), 128, smem, (cudaStream_t)stream>>>((const float2*)d_in, (const float2*)d_l,
+    spatial_corr_kernel<<<sb_grid(total, 128, 16), 128, smem, (cudaStream_t)stream>>>((const float2*)d_in, (const float2*)d_l,
                                                                                           (float2*)d_out, batch, n, cols);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+extern "C" int sb_apply_ofdm_channel(const float* d_x, const float* d_h, const float* d_no, int64_t no_inner, float* d_y,
+                                     int64_t batch, int32_t num_rx_ant_total, int32_t num_tx_ant_total, int32_t num_re,
+                                     int32_t add_noise, uint64_t seed, uint64_t offset, void* stream) {
+    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    SB_CHECK_ARG(d_x && d_h && d_y && batch >= 0 && num_rx_ant_total > 0 && num_tx_ant_total > 0 && num_re > 0 &&
+                     (!add_noise || (d_no && no_inner >= 1)), "sb_apply_ofdm_channel: bad arguments");
+    long long total = batch * num_rx_ant_total * (long long)num_re;
+    if (total == 0) return SB_OK;
+    const RowLaunch rl = row_launch(batch * num_rx_ant_total, num_re);
+    apply_ofdm_channel_kernel<<<rl.grid, rl.block, 0, (cudaStream_t)stream>>>(
+        (const float2*)d_x, (const float2*)d_h, d_no, no_inner > 0 ? no_inner : 1, (float2*)d_y, batch, num_rx_ant_total,
+        num_tx_ant_total, num_re, add_noise, seed, offset);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+extern "C" int sb_apply_time_channel(const float* d_x, const float* d_h, const float* d_no, int64_t no_inner, float* d_y,
+                                     int64_t batch, int32_t num_rx_ant_total, int32_t num_tx_ant_total,
+                                     int32_t num_time_samples, int32_t l_tot, int32_t add_noise, uint64_t seed,
+                                     uint64_t offset, void* stream) {
+    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    SB_CHECK_ARG(d_x && d_h && d_y && num_rx_ant_total > 0 && num_tx_ant_total > 0 && num_time_samples > 0 && l_tot > 0 &&
+                     (!add_noise || (d_no && no_inner >= 1)), "sb_apply_time_channel: bad arguments");
+    const RowLaunch rl = row_launch(batch * num_rx_ant_total, num_time_samples + l_tot - 1);
+    apply_time_channel_kernel<<<rl.grid, rl.block, 0, (cudaStream_t)stream>>>(
+        (const float2*)d_x, (const float2*)d_h, d_no, no_inner > 0 ? no_inner : 1, (float2*)d_y, batch, num_rx_ant_total,
+        num_tx_ant_total, num_time_samples, l_tot, add_noise, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }

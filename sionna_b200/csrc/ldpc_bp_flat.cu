@@ -18,10 +18,6 @@
 
 namespace {
 
-inline int grid_cap(long long blocks) {
-    return (int)std::max<long long>(1, std::min<long long>(blocks, (long long)sb_num_sms() * 16));
-}
-
 // llr[v, b] = -x[b, v] (decoding.py:565), 32 x 32 tiles through shared memory
 __global__ void flat_transpose_neg_kernel(const float* __restrict__ x, float* __restrict__ llr, long long B, int N) {
     __shared__ float tile[32][33];
@@ -129,10 +125,10 @@ extern "C" int sb_ldpc_flat_init(const float* d_x, const int32_t* d_vn_of_edge, 
     SB_CHECK_ARG(d_x && d_vn_of_edge && d_llr && d_v2c && batch > 0 && num_vn > 0 && num_edges >= 0, "sb_ldpc_flat_init: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
     const long long tiles = ((batch + 31) / 32) * ((num_vn + 31) / 32);
-    flat_transpose_neg_kernel<<<grid_cap(tiles), dim3(32, 8, 1), 0, st>>>(d_x, d_llr, batch, num_vn);
+    flat_transpose_neg_kernel<<<sb_grid(tiles, 1, 16), dim3(32, 8, 1), 0, st>>>(d_x, d_llr, batch, num_vn);
     SB_LAUNCH_CHECK();
     if (num_edges > 0) {
-        flat_init_v2c_kernel<<<grid_cap(((long long)num_edges * batch + 255) / 256), 256, 0, st>>>(d_llr, d_vn_of_edge, d_state_in,
+        flat_init_v2c_kernel<<<sb_grid((long long)num_edges * batch, 256, 16), 256, 0, st>>>(d_llr, d_vn_of_edge, d_state_in,
                                                                                                 d_v2c, batch, num_edges);
         SB_LAUNCH_CHECK();
     }
@@ -147,7 +143,7 @@ extern "C" int sb_ldpc_flat_cn(const float* d_v2c, float* d_c2v, const int32_t* 
                  "sb_ldpc_flat_cn: bad arguments");
     SB_CHECK_ARG(cn_rule >= SB_CN_BOXPLUS_PHI && cn_rule <= SB_CN_IDENTITY, "sb_ldpc_flat_cn: unknown cn_rule %d", cn_rule);
     cudaStream_t st = (cudaStream_t)stream;
-    const int grid = grid_cap(((long long)num_nodes * batch + 127) / 128);
+    const int grid = sb_grid((long long)num_nodes * batch, 128, 16);
 #define SB_FLAT_CASE(R)                                                                                                  \
     case R:                                                                                                              \
         flat_cn_kernel<R><<<grid, 128, 0, st>>>(d_v2c, d_c2v, d_cn_ptr, d_v2c_perm, d_cn_list, num_nodes, batch, llr_max, offset); \
@@ -170,7 +166,7 @@ extern "C" int sb_ldpc_flat_vn(const float* d_c2v, const float* d_llr, const int
     if (batch == 0) return SB_OK;
     SB_CHECK_ARG(d_c2v && d_llr && d_vn_ptr && d_c2v_perm && d_v2c && d_xhat && num_vn > 0 && batch > 0 && llr_max >= 0.f &&
                      (vn_rule == SB_VN_SUM || vn_rule == SB_VN_IDENTITY), "sb_ldpc_flat_vn: bad arguments");
-    flat_vn_kernel<<<grid_cap(((long long)num_vn * batch + 127) / 128), 128, 0, (cudaStream_t)stream>>>(
+    flat_vn_kernel<<<sb_grid((long long)num_vn * batch, 128, 16), 128, 0, (cudaStream_t)stream>>>(
         d_c2v, d_llr, d_vn_ptr, d_c2v_perm, d_v2c, d_xhat, num_vn, batch, vn_rule, llr_max);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -182,11 +178,11 @@ extern "C" int sb_ldpc_flat_out(const float* d_xhat, const int32_t* d_out_vn, fl
     if (batch == 0) return SB_OK;
     SB_CHECK_ARG(d_xhat && d_out_vn && d_out && batch > 0 && n_out > 0, "sb_ldpc_flat_out: bad arguments");
     cudaStream_t st = (cudaStream_t)stream;
-    flat_out_kernel<<<grid_cap((batch * n_out + 255) / 256), 256, 0, st>>>(d_xhat, d_out_vn, d_out, batch, n_out, hard_out);
+    flat_out_kernel<<<sb_grid(batch * n_out, 256, 16), 256, 0, st>>>(d_xhat, d_out_vn, d_out, batch, n_out, hard_out);
     SB_LAUNCH_CHECK();
     if (d_state_out && d_v2c && num_edges > 0) {
         const long long n = (long long)num_edges * batch;
-        flat_negate_kernel<<<grid_cap((n + 255) / 256), 256, 0, st>>>(d_v2c, d_state_out, n);       // :636
+        flat_negate_kernel<<<sb_grid(n, 256, 16), 256, 0, st>>>(d_v2c, d_state_out, n);       // :636
         SB_LAUNCH_CHECK();
     }
     return SB_OK;

@@ -6,18 +6,9 @@
 //   A = B + I = C C^H, A^-1 = C^-H C^-1;  G y_w = A^-1 z;  diag(G H_w)_k = sum_j (A^-1)_kj B_jk
 //   output: x_hat_k = (G y_w)_k / diag_k, no_eff_k = Re(1 / diag_k - 1)     (mimo/equalization.py:217-231)
 #pragma once
-#include <cuda_runtime.h>
+#include "sb_common.h"
 
 namespace sb_lmmse {
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-__device__ __forceinline__ float2 cmulc(float2 a, float2 b) { return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y); }
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
-__device__ __forceinline__ float2 cdiv(float2 a, float2 b) {
-    float d = b.x * b.x + b.y * b.y;
-    return make_float2((a.x * b.x + a.y * b.y) / d, (a.y * b.x - a.x * b.y) / d);
-}
-
 template <int K>
 __device__ __forceinline__ void lmmse_diag_solve(const float2* Bm, const float2* z, float2* xh, float* ne) {
     // A = B + I = C C^H (lower, in registers)

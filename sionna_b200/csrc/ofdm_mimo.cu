@@ -7,7 +7,6 @@
 //   sb_rg_map             ResourceGridMapper.call  ofdm/resource_grid.py:394-412
 //   sb_ls_at_pilots       BaseChannelEstimator.call pilot gather :138-150 + LSChannelEstimator :257-285
 //   sb_interp_lin         LinearInterpolator._interpolate ofdm/channel_estimation.py:657-734
-//   sb_apply_ofdm_channel ApplyOFDMChannel.call    channel/apply_ofdm_channel.py:70-80
 //   sb_pusch_precode      PUSCHPrecoder.call       nr/pusch_precoder.py:75-95
 //   sb_pusch_ls_combine   PUSCHLSChannelEstimator.estimate_at_pilot_locations   nr/pusch_channel_estimation.py:117-169
 //   sb_lmmse_equalize     lmmse_equalizer mimo/equalization.py:101-233 (+ whiten_channel mimo/utils.py:292-357,
@@ -18,43 +17,10 @@
 //                         [.., M, M] tensor, 2 KB per RE for M = 16).
 // All kernels are one pass over HBM; FFT twiddles come from sincospif (<= 1 ulp), parity bar 1e-5 (the reference's own
 // round-trip test tolerance, test/unit/ofdm/test_ofdm.py:85-96).
-#include <algorithm>
-#include <cstdlib>
-#include <vector>
 #include "sb_common.h"
-#include "rng.cuh"
 #include "lmmse_diag.cuh"
 
 namespace {
-
-__device__ __forceinline__ float2 cmul(float2 a, float2 b) { return make_float2(a.x * b.x - a.y * b.y, a.x * b.y + a.y * b.x); }
-__device__ __forceinline__ float2 cmulc(float2 a, float2 b) {   // a * conj(b)
-    return make_float2(a.x * b.x + a.y * b.y, a.y * b.x - a.x * b.y);
-}
-__device__ __forceinline__ float2 cadd(float2 a, float2 b) { return make_float2(a.x + b.x, a.y + b.y); }
-__device__ __forceinline__ float2 csub(float2 a, float2 b) { return make_float2(a.x - b.x, a.y - b.y); }
-__device__ __forceinline__ float2 cscale(float2 a, float s) { return make_float2(a.x * s, a.y * s); }
-__device__ __forceinline__ float2 cdiv(float2 a, float2 b) {
-    float d = b.x * b.x + b.y * b.y;
-    return make_float2((a.x * b.x + a.y * b.y) / d, (a.y * b.x - a.x * b.y) / d);
-}
-
-// Row-wise element kernels: blockDim = (tx, ty) with tx = row length rounded up to a warp (<= 256) and ty rows per CTA;
-// a CTA walks rows (64-bit row index once per row), threads walk columns with 32-bit arithmetic only.
-struct RowLaunch { dim3 block; int grid; };
-inline RowLaunch row_launch(long long rows, int cols) {
-    int tx = std::min(256, std::max(32, (cols + 31) / 32 * 32));
-    int ty = std::max(1, 256 / tx);
-    long long ctas = (rows + ty - 1) / ty;
-    int grid = (int)std::max<long long>(1, std::min<long long>(ctas, (long long)sb_num_sms() * 16));
-    return RowLaunch{dim3((unsigned)tx, (unsigned)ty, 1), grid};
-}
-
-inline int grid_for(long long work_items, int threads) {
-    long long blocks = (work_items + threads - 1) / threads;
-    long long cap = (long long)sb_num_sms() * 16;
-    return (int)std::max<long long>(1, std::min(blocks, cap));
-}
 
 // ---------------------------------------------------------------------------------------------------------------
 // Mixed-radix Stockham FFT in shared memory: one CTA transforms one length-N vector (ping-pong buffers, twiddle table
@@ -108,70 +74,59 @@ __device__ void fft_inplace_smem(float2* buf0, float2* buf1, const float2* W, co
     *result = x;
 }
 
-// OFDMModulator: x [rows, nsym, N] (frequency domain, DC in the centre) -> out [rows, sum_l (N + cp[l])]
-// ifftshift -> ifft * sqrt(N) -> cyclic prefix (modulator.py:100-124, signal/utils.py:240-249).
-__global__ void ofdm_mod_kernel(const float2* __restrict__ x, float2* __restrict__ out, FftPlan plan, int nsym,
-                                const int* __restrict__ cp, const int* __restrict__ out_off, int out_len, long long rows,
-                                int shift) {
+// Generic path, one CTA per transform. off / len: offsets of the OFDM symbols in a time-domain row and the row length.
+//   DEMOD = 0, OFDMModulator: x [rows, nsym, N] (frequency domain, DC in the centre) -> out [rows, sum_l (N + cp[l])]
+//     ifftshift -> ifft * sqrt(N) -> cyclic prefix (modulator.py:100-124, signal/utils.py:240-249).
+//   DEMOD = 1, OFDMDemodulator: x [rows, >= sum_l (N + cp[l])] -> out [rows, nsym, N]: strip CP, fft / sqrt(N), phase
+//     compensation exp(-j 2 pi k l_min / N) (fp32 table, demodulator.py:131-134, 196-198), fftshift (:201).
+template <int DEMOD>
+__global__ void ofdm_fft_kernel(const float2* __restrict__ x, float2* __restrict__ out, FftPlan plan, int nsym,
+                                const int* __restrict__ cp, const int* __restrict__ off, int len, int l_min,
+                                long long rows, int shift) {
     extern __shared__ float2 sm[];
     const int N = plan.n, tid = threadIdx.x, T = blockDim.x;
     float2* b0 = sm; float2* b1 = sm + N; float2* W = sm + 2 * N;
+    float2* PC = sm + 3 * N;                                       // phase compensation (demodulator only)
     for (int k = tid; k < N; k += T) {
         float sn, cs;
         sincospif(-2.0f * (float)k / (float)N, &sn, &cs);
         W[k] = make_float2(cs, sn);
+        if (DEMOD) {
+            // tmp = -2 pi l_min / N * k in fp32 as the reference computes it, then exp(j tmp)
+            float tmp = -2.0f * 3.14159265358979323846f * (float)l_min / (float)N * (float)k;
+            PC[k] = make_float2(cosf(tmp), sinf(tmp));
+        }
     }
-    const float scale = 1.0f / sqrtf((float)N);     // ifft = conj(fft(conj))/N, then * sqrt(N)
+    const float scale = 1.0f / sqrtf((float)N);     // modulator: ifft = conj(fft(conj))/N, then * sqrt(N)
     for (long long job = blockIdx.x; job < rows * nsym; job += gridDim.x) {
         const int l = (int)(job % nsym);
-        const float2* src = x + job * N;
+        const float2* src = DEMOD ? x + (job / nsym) * len + off[l] + cp[l] : x + job * N;
         __syncthreads();
-        for (int k = tid; k < N; k += T) {
-            float2 v = src[shift ? (k + N / 2) % N : k];   // ifftshift: out[k] = in[(k + floor(N/2)) mod N]
-            b0[k] = make_float2(v.x, -v.y);
+        if (DEMOD) {
+            for (int k = tid; k < N; k += T) b0[k] = src[k];
+        } else {
+            for (int k = tid; k < N; k += T) {
+                float2 v = src[shift ? (k + N / 2) % N : k];   // ifftshift: out[k] = in[(k + floor(N/2)) mod N]
+                b0[k] = make_float2(v.x, -v.y);
+            }
         }
         __syncthreads();
         float2* res;
         fft_inplace_smem(b0, b1, W, plan, &res);
-        const int c = cp[l];
-        float2* dst = out + (job / nsym) * out_len + out_off[l];
-        for (int i = tid; i < N + c; i += T) {
-            float2 v = res[(i - c + N) % N];
-            dst[i] = make_float2(v.x * scale, -v.y * scale);
-        }
-    }
-}
-
-// OFDMDemodulator: x [rows, >= sum_l (N + cp[l])] -> out [rows, nsym, N]: strip CP, fft / sqrt(N), phase compensation
-// exp(-j 2 pi k l_min / N) (fp32 table, demodulator.py:131-134, 196-198), fftshift (:201).
-__global__ void ofdm_demod_kernel(const float2* __restrict__ x, float2* __restrict__ out, FftPlan plan, int nsym,
-                                  const int* __restrict__ cp, const int* __restrict__ in_off, int in_len, int l_min,
-                                  long long rows, int shift) {
-    extern __shared__ float2 sm[];
-    const int N = plan.n, tid = threadIdx.x, T = blockDim.x;
-    float2* b0 = sm; float2* b1 = sm + N; float2* W = sm + 2 * N; float2* PC = sm + 3 * N;
-    for (int k = tid; k < N; k += T) {
-        float sn, cs;
-        sincospif(-2.0f * (float)k / (float)N, &sn, &cs);
-        W[k] = make_float2(cs, sn);
-        // tmp = -2 pi l_min / N * k in fp32 as the reference computes it, then exp(j tmp)
-        float tmp = -2.0f * 3.14159265358979323846f * (float)l_min / (float)N * (float)k;
-        PC[k] = make_float2(cosf(tmp), sinf(tmp));
-    }
-    const float scale = 1.0f / sqrtf((float)N);
-    for (long long job = blockIdx.x; job < rows * nsym; job += gridDim.x) {
-        const int l = (int)(job % nsym);
-        const float2* src = x + (job / nsym) * in_len + in_off[l] + cp[l];
-        __syncthreads();
-        for (int k = tid; k < N; k += T) b0[k] = src[k];
-        __syncthreads();
-        float2* res;
-        fft_inplace_smem(b0, b1, W, plan, &res);
-        float2* dst = out + job * N;
-        for (int k = tid; k < N; k += T) {
-            int ks = shift ? (k + N / 2) % N : k;   // fftshift: out[k'] with k' = (k + floor(N/2)) mod N takes bin k
-            float2 v = cmul(cscale(res[k], scale), PC[k]);
-            dst[ks] = v;
+        if (DEMOD) {
+            float2* dst = out + job * N;
+            for (int k = tid; k < N; k += T) {
+                int ks = shift ? (k + N / 2) % N : k;   // fftshift: out[k'] with k' = (k + floor(N/2)) mod N takes bin k
+                float2 v = cmul(cscale(res[k], scale), PC[k]);
+                dst[ks] = v;
+            }
+        } else {
+            const int c = cp[l];
+            float2* dst = out + (job / nsym) * len + off[l];
+            for (int i = tid; i < N + c; i += T) {
+                float2 v = res[(i - c + N) % N];
+                dst[i] = make_float2(v.x * scale, -v.y * scale);
+            }
         }
     }
 }
@@ -599,9 +554,7 @@ int launch_fft_r16(const float2* x, float2* out, int nsym, const int* cp, const 
     const size_t smem = sizeof(float2) * ((size_t)N + 256 + 2 * PAD);
     auto kern = ofdm_fft_r16_kernel<DEMOD, R0>;
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    const long long jobs = rows * nsym;
-    const int grid = (int)std::min<long long>(jobs, (long long)sb_num_sms() * (R0 == 16 ? 2 : 4));
-    kern<<<grid, 256, smem, stream>>>(x, out, nsym, cp, off, len, l_min, rows, shift);
+    kern<<<sb_grid(rows * nsym, 1, R0 == 16 ? 2 : 4), 256, smem, stream>>>(x, out, nsym, cp, off, len, l_min, rows, shift);
     return SB_OK;
 }
 
@@ -755,41 +708,14 @@ __global__ void interp_lin_kernel(const T* __restrict__ h, const int* __restrict
     }
 }
 
-// ApplyOFDMChannel: y[b, r, re] = sum_t h[b, r, t, re] * x[b, t, re] + sqrt(no) CN(0,1)   (r = rx*ant, t = tx*ant)
-__global__ void apply_ofdm_channel_kernel(const float2* __restrict__ x, const float2* __restrict__ h,
-                                          const float* __restrict__ no, long long no_inner, float2* __restrict__ y,
-                                          long long B, int R, int Tt, int RE, int add_noise, unsigned long long seed,
-                                          unsigned long long offset) {
-    const long long rows = B * R;
-    for (long long row = (long long)blockIdx.x * blockDim.y + threadIdx.y; row < rows; row += (long long)gridDim.x * blockDim.y) {
-        const long long b = row / R;
-        const float2* hp = h + row * (long long)Tt * RE;
-        const float2* xp = x + b * (long long)Tt * RE;
-        const long long obase = row * (long long)RE;
-        const bool row_no = add_noise && (no_inner % RE) == 0;      // one noise power per row (the usual case)
-        const float sd_row = row_no ? sqrtf(no[obase / no_inner]) * 0.70710678118654752f : 0.f;
-        for (int re = threadIdx.x; re < RE; re += blockDim.x) {
-            float2 acc = make_float2(0.f, 0.f);
-            for (int t = 0; t < Tt; ++t) acc = cadd(acc, cmul(hp[(size_t)t * RE + re], xp[(size_t)t * RE + re]));
-            if (add_noise) {
-                const unsigned long long i = (unsigned long long)(obase + re);    // same Philox counter as the flat index
-                uint4 rr = philox4x32_10(seed, offset, i);
-                float2 g = box_muller(rr.x, rr.y);
-                float sd = row_no ? sd_row : sqrtf(no[i / (unsigned long long)no_inner]) * 0.70710678118654752f;
-                acc.x += g.x * sd;
-                acc.y += g.y * sd;
-            }
-            y[obase + re] = acc;
-        }
-    }
-}
-
 // ---------------------------------------------------------------------------------------------------------------
-// LMMSE equalisation of one received vector, complex64, thread per resource element; scratch matrices live in shared
-// memory interleaved by thread (element e of thread t at [e * T + t]: conflict-free).
-//   whitening: L = chol(S), y_w = L^-1 y, H_w = L^-1 H              (mimo/utils.py:343-347, utils/linalg.py:28-32)
-//   G = (H_w^H H_w + I)^-1 H_w^H via chol + cholesky_solve          (mimo/equalization.py:95-97)
-//   x_hat = G y_w / diag(G H_w),  no_eff = Re(1 / diag(G H_w) - 1)  (mimo/equalization.py:217-231)
+// Dense per-vector linear algebra, complex64, one thread per received vector; matrices live in shared memory interleaved
+// by thread (element e of thread t at [e * T + t]: conflict-free). The LMMSE kernels and the mimo_linalg modes are
+// compositions of these steps:
+//   chol_lower       L = chol(S), in place                                   (utils/linalg.py:28-32)
+//   whiten           y_w = L^-1 y, H_w = L^-1 H                              (mimo/utils.py:343-347)
+//   tx_lmmse_matrix  G = (H^H H + I)^-1 H^H via chol + cholesky_solve        (mimo/equalization.py:95-97)
+//   lmmse_epilogue   x_hat = G y / diag(G H), no_eff = Re(1 / diag(G H) - 1)  (mimo/equalization.py:217-231)
 // ---------------------------------------------------------------------------------------------------------------
 struct Scratch {
     float2* p;
@@ -797,104 +723,7 @@ struct Scratch {
     __device__ __forceinline__ float2& operator()(int e) const { return p[(size_t)e * T + t]; }
 };
 
-// in: S (M x M, row-major, lower triangle read), H (M x K), y (M). out: xh[K], ne[K] written through the callback arrays.
-__device__ void lmmse_core(const Scratch& S, const Scratch& H, const Scratch& Y, const Scratch& A, const Scratch& G,
-                           int M, int K, float2* xh, float* ne) {
-    // Cholesky S = L L^H (lower), in place
-    for (int j = 0; j < M; ++j) {
-        float d = S(j * M + j).x;
-        for (int k = 0; k < j; ++k) { float2 l = S(j * M + k); d -= l.x * l.x + l.y * l.y; }
-        d = sqrtf(d);
-        S(j * M + j) = make_float2(d, 0.f);
-        for (int i = j + 1; i < M; ++i) {
-            float2 v = S(i * M + j);
-            for (int k = 0; k < j; ++k) v = csub(v, cmulc(S(i * M + k), S(j * M + k)));
-            S(i * M + j) = make_float2(v.x / d, v.y / d);
-        }
-    }
-    // forward substitution: y_w = L^-1 y, H_w = L^-1 H
-    for (int i = 0; i < M; ++i) {
-        float d = S(i * M + i).x;
-        float2 v = Y(i);
-        for (int k = 0; k < i; ++k) v = csub(v, cmul(S(i * M + k), Y(k)));
-        Y(i) = make_float2(v.x / d, v.y / d);
-        for (int c = 0; c < K; ++c) {
-            float2 w = H(i * K + c);
-            for (int k = 0; k < i; ++k) w = csub(w, cmul(S(i * M + k), H(k * K + c)));
-            H(i * K + c) = make_float2(w.x / d, w.y / d);
-        }
-    }
-    // A = H_w^H H_w + I  (K x K)
-    for (int a = 0; a < K; ++a)
-        for (int b = 0; b <= a; ++b) {
-            float2 acc = make_float2(a == b ? 1.f : 0.f, 0.f);
-            for (int m = 0; m < M; ++m) acc = cadd(acc, cmulc(H(m * K + b), H(m * K + a)));   // conj(H[m,a]) * H[m,b]
-            A(a * K + b) = acc;
-        }
-    // Cholesky A = C C^H in place (lower)
-    for (int j = 0; j < K; ++j) {
-        float d = A(j * K + j).x;
-        for (int k = 0; k < j; ++k) { float2 l = A(j * K + k); d -= l.x * l.x + l.y * l.y; }
-        d = sqrtf(d);
-        A(j * K + j) = make_float2(d, 0.f);
-        for (int i = j + 1; i < K; ++i) {
-            float2 v = A(i * K + j);
-            for (int k = 0; k < j; ++k) v = csub(v, cmulc(A(i * K + k), A(j * K + k)));
-            A(i * K + j) = make_float2(v.x / d, v.y / d);
-        }
-    }
-    // G = A^-1 H_w^H (K x M): solve C Z = H_w^H, then C^H G = Z, column by column
-    for (int m = 0; m < M; ++m) {
-        for (int i = 0; i < K; ++i) {
-            float2 v = H(m * K + i);
-            v.y = -v.y;                                            // (H_w^H)[i, m]
-            for (int k = 0; k < i; ++k) v = csub(v, cmul(A(i * K + k), G(k * M + m)));
-            float d = A(i * K + i).x;
-            G(i * M + m) = make_float2(v.x / d, v.y / d);
-        }
-        for (int i = K - 1; i >= 0; --i) {
-            float2 v = G(i * M + m);
-            for (int k = i + 1; k < K; ++k) { float2 c = A(k * K + i); c.y = -c.y; v = csub(v, cmul(c, G(k * M + m))); }
-            float d = A(i * K + i).x;
-            G(i * M + m) = make_float2(v.x / d, v.y / d);
-        }
-    }
-    for (int k = 0; k < K; ++k) {
-        float2 gy = make_float2(0.f, 0.f), dd = make_float2(0.f, 0.f);
-        for (int m = 0; m < M; ++m) {
-            gy = cadd(gy, cmul(G(k * M + m), Y(m)));
-            dd = cadd(dd, cmul(G(k * M + m), H(m * K + k)));
-        }
-        xh[k] = cdiv(gy, dd);
-        float2 inv = cdiv(make_float2(1.f, 0.f), dd);
-        ne[k] = inv.x - 1.f;
-    }
-}
-
-// lmmse_equalizer(y [R, M], h [R, M, K], s [R, M, M]) -> x_hat [R, K], no_eff [R, K]
-__global__ void lmmse_kernel(const float2* __restrict__ y, const float2* __restrict__ h, const float2* __restrict__ s,
-                             float2* __restrict__ xh, float* __restrict__ ne, long long R, int M, int K) {
-    extern __shared__ float2 smem[];
-    const int T = blockDim.x, t = threadIdx.x;
-    Scratch S{smem, T, t}, H{smem + (size_t)M * M * T, T, t}, Y{smem + (size_t)(M * M + M * K) * T, T, t},
-        A{smem + (size_t)(M * M + M * K + M) * T, T, t}, G{smem + (size_t)(M * M + M * K + M + K * K) * T, T, t};
-    float2 xo[16];
-    float no[16];
-    for (long long r = (long long)blockIdx.x * T + t; r < R; r += (long long)gridDim.x * T) {
-        for (int e = 0; e < M * M; ++e) S(e) = s[r * M * M + e];
-        for (int e = 0; e < M * K; ++e) H(e) = h[r * M * K + e];
-        for (int e = 0; e < M; ++e) Y(e) = y[r * M + e];
-        lmmse_core(S, H, Y, A, G, M, K, xo, no);
-        for (int k = 0; k < K; ++k) { xh[r * K + k] = xo[k]; ne[r * K + k] = no[k]; }
-    }
-}
-
-// ---- the reference's small dense helpers as callable kernels (thread per matrix, scratch interleaved in shared memory) ---
-//   mode 0  inv_cholesky(s)            utils/linalg.py:8-32          out0 = L^-1 [R, M, M] (lower triangular)
-//   mode 1  whiten_channel(y, h, s)    mimo/utils.py:292-357         out0 = L^-1 y [R, M], out1 = L^-1 H [R, M, K]
-//   mode 2  lmmse_matrix(h, s)         mimo/equalization.py:11-99    out0 = G = H^H (H H^H + S)^-1 [R, K, M]; s == nullptr:
-//                                                                    G = (H^H H + I)^-1 H^H
-//   mode 3  lmmse_equalizer(whiten_interference=False)  :183-233     out0 = x_hat [R, K], out1 = no_eff [R, K] (float)
+// A = L L^H (lower, n x n), in place
 __device__ void chol_lower(const Scratch& A, int n) {
     for (int j = 0; j < n; ++j) {
         float d = A(j * n + j).x;
@@ -908,10 +737,27 @@ __device__ void chol_lower(const Scratch& A, int n) {
         }
     }
 }
-// solve (C C^H) x = b in place for one column held in X(i * ldx + col), C lower triangular n x n
-__device__ void chol_solve_col(const Scratch& C, int n, const Scratch& X, int ldx, int col) {
+
+// forward substitution with the Cholesky factor L (M x M), in place: Y = L^-1 Y (M), H = L^-1 H (M x K)
+__device__ void whiten(const Scratch& L, const Scratch& Y, const Scratch& H, int M, int K) {
+    for (int i = 0; i < M; ++i) {
+        float d = L(i * M + i).x;
+        float2 v = Y(i);
+        for (int k = 0; k < i; ++k) v = csub(v, cmul(L(i * M + k), Y(k)));
+        Y(i) = make_float2(v.x / d, v.y / d);
+        for (int c = 0; c < K; ++c) {
+            float2 w = H(i * K + c);
+            for (int k = 0; k < i; ++k) w = csub(w, cmul(L(i * M + k), H(k * K + c)));
+            H(i * K + c) = make_float2(w.x / d, w.y / d);
+        }
+    }
+}
+
+// solve (C C^H) x = b for one column, b_i = b(i), x_i in X(i * ldx + col); C lower triangular n x n
+template <typename BF>
+__device__ void chol_solve_col(const Scratch& C, int n, const BF& b, const Scratch& X, int ldx, int col) {
     for (int i = 0; i < n; ++i) {
-        float2 v = X(i * ldx + col);
+        float2 v = b(i);
         for (int k = 0; k < i; ++k) v = csub(v, cmul(C(i * n + k), X(k * ldx + col)));
         float d = C(i * n + i).x;
         X(i * ldx + col) = make_float2(v.x / d, v.y / d);
@@ -924,6 +770,77 @@ __device__ void chol_solve_col(const Scratch& C, int n, const Scratch& X, int ld
     }
 }
 
+// G = (H^H H + I)^-1 H^H (K x M) for H (M x K): A = H^H H + I = C C^H (K x K, A is overwritten by C), then
+// C C^H G = H^H column by column
+__device__ void tx_lmmse_matrix(const Scratch& H, const Scratch& A, const Scratch& G, int M, int K) {
+    for (int a = 0; a < K; ++a)
+        for (int b = 0; b <= a; ++b) {
+            float2 acc = make_float2(a == b ? 1.f : 0.f, 0.f);
+            for (int m = 0; m < M; ++m) acc = cadd(acc, cmulc(H(m * K + b), H(m * K + a)));   // conj(H[m,a]) * H[m,b]
+            A(a * K + b) = acc;
+        }
+    chol_lower(A, K);
+    for (int m = 0; m < M; ++m)
+        chol_solve_col(A, K, [&](int k) { float2 v = H(m * K + k); v.y = -v.y; return v; }, G, M, m);
+}
+
+// xh[k] = (G y)_k / (G H)_kk, ne[k] = Re(1 / (G H)_kk - 1) for k < K, with G[k, m] = g(k, m), y[m] = y(m), H (M x K)
+template <typename GF, typename YF>
+__device__ __forceinline__ void lmmse_epilogue(const GF& g, const YF& y, const Scratch& H, int M, int K, float2* xh, float* ne) {
+    for (int k = 0; k < K; ++k) {
+        float2 gy = make_float2(0.f, 0.f), dd = make_float2(0.f, 0.f);
+        for (int m = 0; m < M; ++m) {
+            const float2 gkm = g(k, m);
+            gy = cadd(gy, cmul(gkm, y(m)));
+            dd = cadd(dd, cmul(gkm, H(m * K + k)));
+        }
+        xh[k] = cdiv(gy, dd);
+        float2 inv = cdiv(make_float2(1.f, 0.f), dd);
+        ne[k] = inv.x - 1.f;
+    }
+}
+
+// LMMSE equalisation of one received vector with noise covariance S (mimo/equalization.py:101-233, whitening
+// mimo/utils.py:292-357). Per-thread scratch: S [M, M], H [M, K], y [M], A [K, K], G [K, M].
+struct LmmseScratch {
+    Scratch S, H, Y, A, G;
+    __device__ __forceinline__ LmmseScratch(float2* smem, int T, int t, int M, int K)
+        : S{smem, T, t}, H{smem + (size_t)M * M * T, T, t}, Y{smem + (size_t)(M * M + M * K) * T, T, t},
+          A{smem + (size_t)(M * M + M * K + M) * T, T, t}, G{smem + (size_t)(M * M + M * K + M + K * K) * T, T, t} {}
+    static size_t elems(int M, int K) { return (size_t)(M * M + M * K + M + K * K + K * M); }   // per thread
+};
+
+// in: S (M x M, row-major, lower triangle read), H (M x K), y (M). out: xh[K], ne[K].
+__device__ void lmmse_core(const LmmseScratch& w, int M, int K, float2* xh, float* ne) {
+    chol_lower(w.S, M);
+    whiten(w.S, w.Y, w.H, M, K);
+    tx_lmmse_matrix(w.H, w.A, w.G, M, K);
+    lmmse_epilogue([&](int k, int m) { return w.G(k * M + m); }, w.Y, w.H, M, K, xh, ne);
+}
+
+// lmmse_equalizer(y [R, M], h [R, M, K], s [R, M, M]) -> x_hat [R, K], no_eff [R, K]
+__global__ void lmmse_kernel(const float2* __restrict__ y, const float2* __restrict__ h, const float2* __restrict__ s,
+                             float2* __restrict__ xh, float* __restrict__ ne, long long R, int M, int K) {
+    extern __shared__ float2 smem[];
+    const int T = blockDim.x, t = threadIdx.x;
+    const LmmseScratch w(smem, T, t, M, K);
+    float2 xo[16];
+    float no[16];
+    for (long long r = (long long)blockIdx.x * T + t; r < R; r += (long long)gridDim.x * T) {
+        for (int e = 0; e < M * M; ++e) w.S(e) = s[r * M * M + e];
+        for (int e = 0; e < M * K; ++e) w.H(e) = h[r * M * K + e];
+        for (int e = 0; e < M; ++e) w.Y(e) = y[r * M + e];
+        lmmse_core(w, M, K, xo, no);
+        for (int k = 0; k < K; ++k) { xh[r * K + k] = xo[k]; ne[r * K + k] = no[k]; }
+    }
+}
+
+// ---- the reference's small dense helpers as callable kernels (thread per matrix, scratch interleaved in shared memory) ---
+//   mode 0  inv_cholesky(s)            utils/linalg.py:8-32          out0 = L^-1 [R, M, M] (lower triangular)
+//   mode 1  whiten_channel(y, h, s)    mimo/utils.py:292-357         out0 = L^-1 y [R, M], out1 = L^-1 H [R, M, K]
+//   mode 2  lmmse_matrix(h, s)         mimo/equalization.py:11-99    out0 = G = H^H (H H^H + S)^-1 [R, K, M]; s == nullptr:
+//                                                                    G = (H^H H + I)^-1 H^H
+//   mode 3  lmmse_equalizer(whiten_interference=False)  :183-233     out0 = x_hat [R, K], out1 = no_eff [R, K] (float)
 __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const float2* __restrict__ h,
                                    const float2* __restrict__ s, float2* __restrict__ out0, void* __restrict__ out1v,
                                    long long R, int M, int K) {
@@ -947,17 +864,8 @@ __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const
                 for (int e = 0; e < M * M; ++e) out0[r * M * M + e] = X(e);
             } else {
                 float2* hw = reinterpret_cast<float2*>(out1v);
-                for (int i = 0; i < M; ++i) {
-                    float d = A(i * M + i).x;
-                    float2 v = y[r * M + i];
-                    for (int k = 0; k < i; ++k) v = csub(v, cmul(A(i * M + k), X(k)));
-                    X(i) = make_float2(v.x / d, v.y / d);
-                    for (int c = 0; c < K; ++c) {
-                        float2 w = H(i * K + c);
-                        for (int k = 0; k < i; ++k) w = csub(w, cmul(A(i * M + k), H(k * K + c)));
-                        H(i * K + c) = make_float2(w.x / d, w.y / d);
-                    }
-                }
+                for (int i = 0; i < M; ++i) X(i) = y[r * M + i];
+                whiten(A, X, H, M, K);
                 for (int i = 0; i < M; ++i) out0[r * M + i] = X(i);
                 for (int e = 0; e < M * K; ++e) hw[r * M * K + e] = H(e);
             }
@@ -972,20 +880,9 @@ __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const
                     A(a * M + b) = acc;
                 }
             chol_lower(A, M);
-            for (int e = 0; e < M * K; ++e) X(e) = H(e);
-            for (int c = 0; c < K; ++c) chol_solve_col(A, M, X, K, c);     // X = G^H [M, K]
-        } else {                                                    // G = (H^H H + I)^-1 H^H, X = G [K, M]
-            for (int a = 0; a < K; ++a)
-                for (int b = 0; b <= a; ++b) {
-                    float2 acc = make_float2(a == b ? 1.f : 0.f, 0.f);
-                    for (int m = 0; m < M; ++m) acc = cadd(acc, cmulc(H(m * K + b), H(m * K + a)));
-                    A(a * K + b) = acc;
-                }
-            chol_lower(A, K);
-            for (int m = 0; m < M; ++m) {
-                for (int k = 0; k < K; ++k) { float2 v = H(m * K + k); v.y = -v.y; X(k * M + m) = v; }
-                chol_solve_col(A, K, X, M, m);
-            }
+            for (int c = 0; c < K; ++c) chol_solve_col(A, M, [&](int i) { return H(i * K + c); }, X, K, c);   // X = G^H [M, K]
+        } else {
+            tx_lmmse_matrix(H, A, X, M, K);                                // X = G [K, M]
         }
         if (mode == 2) {
             for (int k = 0; k < K; ++k)
@@ -994,20 +891,10 @@ __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const
                     if (rx_side) { g = X(m * K + k); g.y = -g.y; }                 // G = (G^H)^H
                     out0[(r * K + k) * M + m] = g;
                 }
-        } else {
+        } else {                                                    // mode 3 has s: X = G^H
             float* ne = reinterpret_cast<float*>(out1v);
-            for (int k = 0; k < K; ++k) {
-                float2 gy = make_float2(0.f, 0.f), dd = make_float2(0.f, 0.f);
-                for (int m = 0; m < M; ++m) {
-                    float2 g = X(m * K + k);
-                    g.y = -g.y;
-                    gy = cadd(gy, cmul(g, y[r * M + m]));
-                    dd = cadd(dd, cmul(g, H(m * K + k)));
-                }
-                out0[r * K + k] = cdiv(gy, dd);
-                float2 inv = cdiv(make_float2(1.f, 0.f), dd);
-                ne[r * K + k] = inv.x - 1.f;
-            }
+            lmmse_epilogue([&](int k, int m) { float2 g = X(m * K + k); g.y = -g.y; return g; },
+                           [&](int m) { return y[r * M + m]; }, H, M, K, out0 + r * K, ne + r * K);
         }
     }
 }
@@ -1030,8 +917,7 @@ struct OfdmEqParams {
 __global__ void ofdm_lmmse_kernel(const OfdmEqParams p) {
     extern __shared__ float2 smem[];
     const int T = blockDim.x, t = threadIdx.x, M = p.ANT, K = p.K;
-    Scratch Sm{smem, T, t}, H{smem + (size_t)M * M * T, T, t}, Y{smem + (size_t)(M * M + M * K) * T, T, t},
-        A{smem + (size_t)(M * M + M * K + M) * T, T, t}, G{smem + (size_t)(M * M + M * K + M + K * K) * T, T, t};
+    const LmmseScratch w(smem, T, t, M, K);
     float2 xo[16];
     float no_e[16];
     const long long SF = (long long)p.S * p.F;
@@ -1047,9 +933,9 @@ __global__ void ofdm_lmmse_kernel(const OfdmEqParams p) {
         if (!any) continue;
         for (int m = 0; m < M; ++m) {
             long long ybase = ((b * p.RX + rx) * M + m) * SF + re;
-            Y(m) = p.y[ybase];
+            w.Y(m) = p.y[ybase];
             long long hb = ((b * p.RX + rx) * M + m) * (long long)p.TXS;
-            for (int k = 0; k < K; ++k) H(m * K + k) = p.hhat[(hb + p.des[rx * K + k]) * SF + re];
+            for (int k = 0; k < K; ++k) w.H(m * K + k) = p.hhat[(hb + p.des[rx * K + k]) * SF + re];
             // S = H_u H_u^H + diag(no) + diag(sum_txs err_var)   (equalization.py:205-218)
             float evs = 0.f;
             for (int q = 0; q < p.TXS; ++q)
@@ -1063,10 +949,10 @@ __global__ void ofdm_lmmse_kernel(const OfdmEqParams p) {
                     acc = cadd(acc, cmulc(p.hhat[(hb + p.und[rx * p.KU + u]) * SF + re],
                                           p.hhat[(hb2 + p.und[rx * p.KU + u]) * SF + re]));
                 if (m2 == m) acc.x += nn + evs;
-                Sm(m * M + m2) = acc;
+                w.S(m * M + m2) = acc;
             }
         }
-        lmmse_core(Sm, H, Y, A, G, M, K, xo, no_e);
+        lmmse_core(w, M, K, xo, no_e);
         for (int k = 0; k < K; ++k) {
             int ts = p.out_ts[rx * K + k];
             int dp = p.data_pos[(size_t)ts * SF + re];
@@ -1185,7 +1071,7 @@ __global__ void __launch_bounds__(128, 4) ofdm_lmmse_diag_kernel(const OfdmEqPar
 
 template <int K>
 void launch_lmmse_diag(const OfdmEqParams& p, long long total, cudaStream_t stream) {
-    ofdm_lmmse_diag_kernel<K><<<grid_for(total, 128), 128, 0, stream>>>(p);
+    ofdm_lmmse_diag_kernel<K><<<sb_grid(total, 128, 16), 128, 0, stream>>>(p);
 }
 
 int make_plan(int n, FftPlan* plan) {
@@ -1208,9 +1094,6 @@ int make_plan(int n, FftPlan* plan) {
     return 0;
 }
 
-}  // namespace
-
-namespace {
 // Host side of the small-FFT path: the stage radices (the plan travels as a kernel parameter).
 int get_small_plan(int n, SmallFftPlan* out) {
     FftPlan fp;
@@ -1247,9 +1130,7 @@ int launch_fft_small_fpw(const SmallFftPlan& sp, const float2* x, float2* out, i
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 1;
     SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, warps * 32, smem));
-    long long jobs = rows * nsym;
-    long long want = (jobs + (long long)warps * FPW - 1) / ((long long)warps * FPW);
-    int grid = (int)std::max<long long>(1, std::min<long long>(want, (long long)sb_num_sms() * std::max(1, occ)));
+    const int grid = sb_grid(rows * nsym, warps * FPW, std::max(1, occ));
     kern<<<grid, warps * 32, smem, stream>>>(x, out, sp, nsym, cp, off, len, l_min, rows, shift);
     return SB_OK;
 }
@@ -1260,104 +1141,62 @@ int launch_fft_small(const float2* x, float2* out, int n, int nsym, const int* c
     SmallFftPlan sp;
     int rc = get_small_plan(n, &sp);
     if (rc) return rc;
-    // transforms per warp (SB_FFT_FPW overrides, for experiments). Measured at N = 76, modulator / demodulator ms per
-    // 458 k transforms: 2 -> 0.39 / 0.37, 4 -> 0.277 / 0.254, 8 -> 0.34 / 0.29 (8 halves the resident warps per SM).
-    int fpw = n <= 128 ? 4 : (n <= 256 ? 2 : 1);               // three buffers of fpw transforms per warp, 2 CTAs per SM
-    if (const char* e = getenv("SB_FFT_FPW")) {
-        int v = atoi(e);
-        if ((v == 1 || v == 2 || v == 4 || v == 8) && (size_t)n * 8 * (2 + 24 * v) <= 200 * 1024) fpw = v;
-    }
-    if (fpw == 8) return launch_fft_small_fpw<DEMOD, 8>(sp, x, out, nsym, cp, off, len, l_min, rows, shift, stream);
+    // transforms per warp. Measured at N = 76, modulator / demodulator ms per 458 k transforms: 2 -> 0.39 / 0.37,
+    // 4 -> 0.277 / 0.254, 8 -> 0.34 / 0.29 (8 halves the resident warps per SM).
+    const int fpw = n <= 128 ? 4 : (n <= 256 ? 2 : 1);         // three buffers of fpw transforms per warp, 2 CTAs per SM
     if (fpw == 4) return launch_fft_small_fpw<DEMOD, 4>(sp, x, out, nsym, cp, off, len, l_min, rows, shift, stream);
     if (fpw == 2) return launch_fft_small_fpw<DEMOD, 2>(sp, x, out, nsym, cp, off, len, l_min, rows, shift, stream);
     return launch_fft_small_fpw<DEMOD, 1>(sp, x, out, nsym, cp, off, len, l_min, rows, shift, stream);
+}
+
+// Body of sb_ofdm_modulate (DEMOD = 0) and sb_ofdm_demodulate (DEMOD = 1), `name` is the entry point named in errors.
+// N <= 1024: warp-per-transform kernel; N = 2048, 4096: radix-16 kernel; any other N <= 8192: one CTA per transform.
+template <int DEMOD>
+int ofdm_fft(const char* name, const float* d_x, float* d_out, int64_t rows, int32_t nsym, int32_t n, const int32_t* d_cp,
+             const int32_t* d_off, int32_t len, int32_t l_min, int32_t shift, cudaStream_t stream) {
+    if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    SB_CHECK_ARG(d_x && d_out && d_cp && d_off && rows >= 0 && nsym > 0 && n > 0 && n <= 8192, "%s: bad arguments", name);
+    const float2* x = (const float2*)d_x;
+    float2* out = (float2*)d_out;
+    int rc = SB_OK;
+    if (n <= kSmallFftMax) {
+        rc = launch_fft_small<DEMOD>(x, out, n, nsym, d_cp, d_off, len, l_min, rows, shift, stream);
+    } else if (n == 4096 || n == 2048) {
+        rc = launch_fft_pow2<DEMOD>(n, x, out, nsym, d_cp, d_off, len, l_min, rows, shift, stream);
+    } else {
+        FftPlan plan;
+        SB_CHECK_ARG(make_plan(n, &plan) == 0, "%s: fft_size has too many factors", name);
+        const int threads = std::min(256, std::max(32, (n / 2 + 31) / 32 * 32));
+        const size_t smem = sizeof(float2) * (DEMOD ? 4 : 3) * (size_t)n;
+        int dev = 0, optin = 0;
+        SB_CUDA(cudaGetDevice(&dev));
+        SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+        if (smem > (size_t)optin) {
+            sb_set_error("%s: fft_size %d needs %zu bytes of shared memory per CTA, the device offers %d", name, n, smem, optin);
+            return SB_EUNSUPPORTED;
+        }
+        auto kern = ofdm_fft_kernel<DEMOD>;
+        SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<sb_grid(rows * nsym, 1, 8), threads, smem, stream>>>(x, out, plan, nsym, d_cp, d_off, len, l_min, rows, shift);
+    }
+    if (rc) return rc;
+    SB_LAUNCH_CHECK();
+    return SB_OK;
 }
 
 }  // namespace
 
 extern "C" int sb_ofdm_modulate(const float* d_x, float* d_out, int64_t rows, int32_t num_symbols, int32_t fft_size,
                                 const int32_t* d_cp, const int32_t* d_out_off, int32_t out_len, int32_t shift, void* stream) {
-    if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_x && d_out && d_cp && d_out_off && rows >= 0 && num_symbols > 0 && fft_size > 0 && fft_size <= 8192,
-                 "sb_ofdm_modulate: bad arguments");
-    if (rows == 0) return SB_OK;
-    if (fft_size <= kSmallFftMax) {
-        int rc = launch_fft_small<0>((const float2*)d_x, (float2*)d_out, fft_size, num_symbols, d_cp, d_out_off, out_len, 0,
-                                     rows, shift, (cudaStream_t)stream);
-        if (rc) return rc;
-        SB_LAUNCH_CHECK();
-        return SB_OK;
-    }
-    if (fft_size == 4096 || fft_size == 2048) {
-        int rc = launch_fft_pow2<0>(fft_size, (const float2*)d_x, (float2*)d_out, num_symbols, d_cp, d_out_off, out_len, 0, rows,
-                                    shift, (cudaStream_t)stream);
-        if (rc) return rc;
-        SB_LAUNCH_CHECK();
-        return SB_OK;
-    }
-    FftPlan plan;
-    SB_CHECK_ARG(make_plan(fft_size, &plan) == 0, "sb_ofdm_modulate: fft_size has too many factors");
-    int threads = std::min(256, std::max(32, (fft_size / 2 + 31) / 32 * 32));
-    size_t smem = sizeof(float2) * 3 * (size_t)fft_size;
-    {
-        int dev = 0, optin = 0;
-        SB_CUDA(cudaGetDevice(&dev));
-        SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        if (smem > (size_t)optin) {
-            sb_set_error("sb_ofdm_modulate: fft_size %d needs %zu bytes of shared memory per CTA, the device offers %d", fft_size, smem, optin);
-            return SB_EUNSUPPORTED;
-        }
-    }
-    SB_CUDA(cudaFuncSetAttribute(ofdm_mod_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    long long jobs = rows * num_symbols;
-    int grid = (int)std::min<long long>(jobs, (long long)sb_num_sms() * 8);
-    ofdm_mod_kernel<<<grid, threads, smem, (cudaStream_t)stream>>>((const float2*)d_x, (float2*)d_out, plan, num_symbols,
-                                                                   d_cp, d_out_off, out_len, rows, shift);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
+    return ofdm_fft<0>("sb_ofdm_modulate", d_x, d_out, rows, num_symbols, fft_size, d_cp, d_out_off, out_len, 0, shift,
+                       (cudaStream_t)stream);
 }
 
 extern "C" int sb_ofdm_demodulate(const float* d_x, float* d_out, int64_t rows, int32_t num_symbols, int32_t fft_size,
                                   const int32_t* d_cp, const int32_t* d_in_off, int32_t in_len, int32_t l_min,
                                   int32_t shift, void* stream) {
-    if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_x && d_out && d_cp && d_in_off && rows >= 0 && num_symbols > 0 && fft_size > 0 && fft_size <= 8192,
-                 "sb_ofdm_demodulate: bad arguments");
-    if (rows == 0) return SB_OK;
-    if (fft_size <= kSmallFftMax) {
-        int rc = launch_fft_small<1>((const float2*)d_x, (float2*)d_out, fft_size, num_symbols, d_cp, d_in_off, in_len,
-                                     l_min, rows, shift, (cudaStream_t)stream);
-        if (rc) return rc;
-        SB_LAUNCH_CHECK();
-        return SB_OK;
-    }
-    if (fft_size == 4096 || fft_size == 2048) {
-        int rc = launch_fft_pow2<1>(fft_size, (const float2*)d_x, (float2*)d_out, num_symbols, d_cp, d_in_off, in_len, l_min, rows,
-                                    shift, (cudaStream_t)stream);
-        if (rc) return rc;
-        SB_LAUNCH_CHECK();
-        return SB_OK;
-    }
-    FftPlan plan;
-    SB_CHECK_ARG(make_plan(fft_size, &plan) == 0, "sb_ofdm_demodulate: fft_size has too many factors");
-    int threads = std::min(256, std::max(32, (fft_size / 2 + 31) / 32 * 32));
-    size_t smem = sizeof(float2) * 4 * (size_t)fft_size;
-    {
-        int dev = 0, optin = 0;
-        SB_CUDA(cudaGetDevice(&dev));
-        SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-        if (smem > (size_t)optin) {
-            sb_set_error("sb_ofdm_demodulate: fft_size %d needs %zu bytes of shared memory per CTA, the device offers %d", fft_size, smem, optin);
-            return SB_EUNSUPPORTED;
-        }
-    }
-    SB_CUDA(cudaFuncSetAttribute(ofdm_demod_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    long long jobs = rows * num_symbols;
-    int grid = (int)std::min<long long>(jobs, (long long)sb_num_sms() * 8);
-    ofdm_demod_kernel<<<grid, threads, smem, (cudaStream_t)stream>>>((const float2*)d_x, (float2*)d_out, plan,
-                                                                     num_symbols, d_cp, d_in_off, in_len, l_min, rows, shift);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
+    return ofdm_fft<1>("sb_ofdm_demodulate", d_x, d_out, rows, num_symbols, fft_size, d_cp, d_in_off, in_len, l_min, shift,
+                       (cudaStream_t)stream);
 }
 
 extern "C" int sb_gather_rows(const float* d_in, const int32_t* d_idx, float* d_out, int64_t batch, int32_t rows,
@@ -1418,7 +1257,7 @@ extern "C" int sb_interp_lin(const float* d_h, const int32_t* d_fx0, const int32
                      (words == 1 || words == 2), "sb_interp_lin: bad arguments (words: 1 = real, 2 = complex)");
     const long long rows = batch * num_streams;
     if (rows == 0 || num_symbols * num_subcarriers == 0) return SB_OK;
-    const int grid = (int)std::min<long long>(rows, (long long)sb_num_sms() * 16);
+    const int grid = sb_grid(rows, 1, 16);
     const int threads = std::min(256, std::max(32, (num_subcarriers + 31) / 32 * 32));
     if (words == 2)
         interp_lin_kernel<float2><<<grid, threads, 0, (cudaStream_t)stream>>>(
@@ -1432,178 +1271,12 @@ extern "C" int sb_interp_lin(const float* d_h, const int32_t* d_fx0, const int32
     return SB_OK;
 }
 
-extern "C" int sb_apply_ofdm_channel(const float* d_x, const float* d_h, const float* d_no, int64_t no_inner, float* d_y,
-                                     int64_t batch, int32_t num_rx_ant_total, int32_t num_tx_ant_total, int32_t num_re,
-                                     int32_t add_noise, uint64_t seed, uint64_t offset, void* stream) {
-    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_x && d_h && d_y && batch >= 0 && num_rx_ant_total > 0 && num_tx_ant_total > 0 && num_re > 0 &&
-                     (!add_noise || (d_no && no_inner >= 1)), "sb_apply_ofdm_channel: bad arguments");
-    long long total = batch * num_rx_ant_total * (long long)num_re;
-    if (total == 0) return SB_OK;
-    const RowLaunch rl = row_launch(batch * num_rx_ant_total, num_re);
-    apply_ofdm_channel_kernel<<<rl.grid, rl.block, 0, (cudaStream_t)stream>>>(
-        (const float2*)d_x, (const float2*)d_h, d_no, no_inner > 0 ? no_inner : 1, (float2*)d_y, batch, num_rx_ant_total,
-        num_tx_ant_total, num_re, add_noise, seed, offset);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
-}
-
-// ---- On-device channel generation (channel/tr38901/tdl.py:372-502, channel/utils.py:180-253) --------------------------
-namespace {
-// TDL tap gains by the sum-of-sinusoids model: for link b, antenna pair a (rx-major), path p, time step t
-//   a = sqrt(P_p / Ns) sum_n exp(j (w_b t/fs cos(2 pi (n+1)/Ns + theta[b,p,n]) + phi[b,a,p,n]))
-//       (+ sqrt(P_los) exp(j (w_b t/fs cos(aoa) + phi0[b])) on path 0 of the LoS models)
-// One thread per (b, a, p) row. Time is processed in chunks of 16 steps held in registers: per sinusoid one cos for the
-// angular rate, one sincos for the phasor at the chunk start and one for the per-step rotation, then 16 complex
-// multiplications (the recurrence is re-anchored every chunk, so its rounding error stays below 1e-6).
-constexpr int kSosChunk = 16;
-__device__ __forceinline__ void sos_accumulate(float2* acc, float rate, float phase, int t0) {
-    float s0, c0, sd, cd;
-    sincosf(rate * (float)t0 + phase, &s0, &c0);
-    sincosf(rate, &sd, &cd);
-    float2 z = make_float2(c0, s0);
-    const float2 step = make_float2(cd, sd);
-#pragma unroll
-    for (int i = 0; i < kSosChunk; ++i) {
-        acc[i].x += z.x;
-        acc[i].y += z.y;
-        z = cmul(z, step);
-    }
-}
-__global__ void tdl_sos_kernel(const float* __restrict__ doppler, const float* __restrict__ theta,
-                               const float* __restrict__ phi, const float* __restrict__ phi0,
-                               const float* __restrict__ powers, float los_power, float los_aoa, float2* __restrict__ out,
-                               long long B, int A, int P, int Ns, int T, float fs) {
-    const long long rows = B * A * P;                            // (b, a, p)
-    for (long long row = (long long)blockIdx.x * blockDim.x + threadIdx.x; row < rows; row += (long long)gridDim.x * blockDim.x) {
-        const int p = (int)(row % P);
-        const long long b = row / ((long long)P * A);
-        const float wd = doppler[b] / fs;                        // radians per time step at cos = 1
-        const float* th = theta + (b * P + p) * (long long)Ns;
-        const float* ph = phi + row * (long long)Ns;
-        const float amp = sqrtf(powers[p]) * (1.0f / sqrtf((float)Ns));
-        const bool los = phi0 != nullptr && p == 0;
-        const float la = los ? sqrtf(los_power) : 0.f;
-        for (int t0 = 0; t0 < T; t0 += kSosChunk) {
-            float2 acc[kSosChunk];
-#pragma unroll
-            for (int i = 0; i < kSosChunk; ++i) acc[i] = make_float2(0.f, 0.f);
-            for (int n = 0; n < Ns; ++n) {
-                const float alpha = 6.283185307179586f / (float)Ns * (float)(n + 1) + th[n];
-                sos_accumulate(acc, wd * cosf(alpha), ph[n], t0);
-            }
-            float2 spec[kSosChunk];
-#pragma unroll
-            for (int i = 0; i < kSosChunk; ++i) spec[i] = make_float2(0.f, 0.f);
-            if (los) sos_accumulate(spec, wd * cosf(los_aoa), phi0[b], t0);
-#pragma unroll
-            for (int i = 0; i < kSosChunk; ++i)
-                if (t0 + i < T) out[row * T + t0 + i] = make_float2(acc[i].x * amp + la * spec[i].x, acc[i].y * amp + la * spec[i].y);
-        }
-    }
-}
-
-// h[r, t, f] = sum_p a[r, p, t] e[p, f],  e[p, f] = exp(-j 2 pi f_k tau_p) shared by all links (TDL: fixed delays).
-// A CTA owns rows r = (b, rx ant, tx ant); threads walk the subcarriers: e is read coalesced, a[r, p, t] is a broadcast.
-__global__ void cir_to_ofdm_kernel(const float2* __restrict__ a, const float2* __restrict__ e, float2* __restrict__ h,
-                                   long long R, int P, int T, int F) {
-    for (long long rt = (long long)blockIdx.x * blockDim.y + threadIdx.y; rt < R * T; rt += (long long)gridDim.x * blockDim.y) {
-        const long long r = rt / T;
-        const int t = (int)(rt - r * T);
-        const float2* ap = a + r * (long long)P * T + t;
-        float2* hp = h + rt * (long long)F;
-        for (int f = threadIdx.x; f < F; f += blockDim.x) {
-            float2 acc = make_float2(0.f, 0.f);
-            for (int p = 0; p < P; ++p) acc = cadd(acc, cmul(ap[(size_t)p * T], e[(size_t)p * F + f]));
-            hp[f] = acc;
-        }
-    }
-}
-}  // namespace
-
-namespace {
-// ApplyTimeChannel (channel/apply_time_channel.py:115-137): time-variant FIR filtering
-//   y[b, r, n] = sum_t sum_l h[b, r, t, n, l] x[b, t, n - l]   (x = 0 outside [0, N)),  n in [0, N + L - 1)
-// r = (rx, rx_ant), t = (tx, tx_ant). A CTA row is (b, r); threads walk the output samples.
-__global__ void apply_time_channel_kernel(const float2* __restrict__ x, const float2* __restrict__ h,
-                                          const float* __restrict__ no, long long no_inner, float2* __restrict__ y,
-                                          long long B, int R, int Tt, int N, int L, int add_noise, unsigned long long seed,
-                                          unsigned long long offset) {
-    const int NO = N + L - 1;
-    const long long rows = B * R;
-    for (long long row = (long long)blockIdx.x * blockDim.y + threadIdx.y; row < rows; row += (long long)gridDim.x * blockDim.y) {
-        const long long b = row / R;
-        const long long obase = row * (long long)NO;
-        for (int n = threadIdx.x; n < NO; n += blockDim.x) {
-            float2 acc = make_float2(0.f, 0.f);
-            for (int t = 0; t < Tt; ++t) {
-                const float2* hp = h + ((row * Tt + t) * (long long)NO + n) * L;
-                const float2* xp = x + (b * Tt + t) * (long long)N;
-                const int l0 = n - (N - 1) > 0 ? n - (N - 1) : 0;     // n - l <= N - 1
-                const int l1 = n < L - 1 ? n : L - 1;                  // n - l >= 0
-                for (int l = l0; l <= l1; ++l) acc = cadd(acc, cmul(hp[l], xp[n - l]));
-            }
-            if (add_noise) {
-                const unsigned long long i = (unsigned long long)(obase + n);
-                uint4 rr = philox4x32_10(seed, offset, i);
-                float2 g = box_muller(rr.x, rr.y);
-                float sd = sqrtf(no[i / (unsigned long long)no_inner]) * 0.70710678118654752f;
-                acc.x += g.x * sd;
-                acc.y += g.y * sd;
-            }
-            y[obase + n] = acc;
-        }
-    }
-}
-}  // namespace
-
-extern "C" int sb_apply_time_channel(const float* d_x, const float* d_h, const float* d_no, int64_t no_inner, float* d_y,
-                                     int64_t batch, int32_t num_rx_ant_total, int32_t num_tx_ant_total,
-                                     int32_t num_time_samples, int32_t l_tot, int32_t add_noise, uint64_t seed,
-                                     uint64_t offset, void* stream) {
-    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_x && d_h && d_y && num_rx_ant_total > 0 && num_tx_ant_total > 0 && num_time_samples > 0 && l_tot > 0 &&
-                     (!add_noise || (d_no && no_inner >= 1)), "sb_apply_time_channel: bad arguments");
-    const RowLaunch rl = row_launch(batch * num_rx_ant_total, num_time_samples + l_tot - 1);
-    apply_time_channel_kernel<<<rl.grid, rl.block, 0, (cudaStream_t)stream>>>(
-        (const float2*)d_x, (const float2*)d_h, d_no, no_inner > 0 ? no_inner : 1, (float2*)d_y, batch, num_rx_ant_total,
-        num_tx_ant_total, num_time_samples, l_tot, add_noise, seed, offset);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
-}
-
-extern "C" int sb_tdl_sos(const float* d_doppler, const float* d_theta, const float* d_phi, const float* d_phi0,
-                          const float* d_powers, float los_power, float los_aoa, float* d_a, int64_t batch,
-                          int32_t num_ant_pairs, int32_t num_paths, int32_t num_sinusoids, int32_t num_time_steps,
-                          float sampling_frequency, void* stream) {
-    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_doppler && d_theta && d_phi && d_powers && d_a && num_ant_pairs > 0 && num_paths > 0 &&
-                     num_sinusoids > 0 && num_time_steps > 0 && sampling_frequency > 0.f, "sb_tdl_sos: bad arguments");
-    tdl_sos_kernel<<<grid_for(batch * num_ant_pairs * num_paths, 128), 128, 0, (cudaStream_t)stream>>>(d_doppler, d_theta, d_phi, d_phi0, d_powers, los_power,
-                                                                  los_aoa, (float2*)d_a, batch, num_ant_pairs, num_paths,
-                                                                  num_sinusoids, num_time_steps, sampling_frequency);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
-}
-
-extern "C" int sb_cir_to_ofdm(const float* d_a, const float* d_e, float* d_h, int64_t rows, int32_t num_paths,
-                              int32_t num_time_steps, int32_t num_subcarriers, void* stream) {
-    if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_a && d_e && d_h && num_paths > 0 && num_time_steps > 0 && num_subcarriers > 0,
-                 "sb_cir_to_ofdm: bad arguments");
-    const RowLaunch rl = row_launch(rows * num_time_steps, num_subcarriers);
-    cir_to_ofdm_kernel<<<rl.grid, rl.block, 0, (cudaStream_t)stream>>>((const float2*)d_a, (const float2*)d_e, (float2*)d_h,
-                                                                      rows, num_paths, num_time_steps, num_subcarriers);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
-}
-
 // ---- PUSCH (nr/pusch_precoder.py, nr/pusch_channel_estimation.py) ---------------------------------------------------
 namespace {
 // y[b, t, p, re] = sum_l W[t, p, l] x[b, t, l, re]: codebook precoding of the layer grids onto the antenna ports
 __global__ void pusch_precode_kernel(const float2* __restrict__ x, const float2* __restrict__ w, float2* __restrict__ y,
                                      long long total, int num_tx, int L, int P, long long re) {
-    // grid-stride: grid_for() caps the grid at 16 CTAs per SM
+    // grid-stride: sb_grid() caps the grid at 16 CTAs per SM
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long long)gridDim.x * blockDim.x) {
         long long r = i % re;
         long long bp = i / re;
@@ -1672,7 +1345,7 @@ extern "C" int sb_pusch_precode(const float* d_x, const float* d_w, float* d_y, 
                  "sb_pusch_precode: bad arguments");
     long long total = batch * num_tx * (long long)num_ports * num_re;
     if (total == 0) return SB_OK;
-    pusch_precode_kernel<<<grid_for(total, 256), 256, 0, (cudaStream_t)stream>>>(
+    pusch_precode_kernel<<<sb_grid(total, 256, 16), 256, 0, (cudaStream_t)stream>>>(
         (const float2*)d_x, (const float2*)d_w, (float2*)d_y, total, num_tx, num_layers, num_ports, num_re);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -1688,37 +1361,36 @@ extern "C" int sb_pusch_ls_combine(float* d_h, float* d_err_var, int64_t rows, i
     if (rows == 0) return SB_OK;
     long long units = (long long)rows * (num_pilots / pilots_per_dmrs_symbol / dmrs_length) *
                       (pilots_per_dmrs_symbol / group_size);
-    pusch_ls_combine_kernel<<<grid_for(units, 256), 256, 0, (cudaStream_t)stream>>>(
+    pusch_ls_combine_kernel<<<sb_grid(units, 256, 16), 256, 0, (cudaStream_t)stream>>>(
         (float2*)d_h, rows, num_pilots, pilots_per_dmrs_symbol, dmrs_length, group_size);
     SB_LAUNCH_CHECK();
     long long n = (long long)rows * num_pilots;
-    scale_real_kernel<<<grid_for(n, 256), 256, 0, (cudaStream_t)stream>>>(d_err_var, n, dmrs_length == 2 ? 0.25f : 0.5f);
+    scale_real_kernel<<<sb_grid(n, 256, 16), 256, 0, (cudaStream_t)stream>>>(d_err_var, n, dmrs_length == 2 ? 0.25f : 0.5f);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
 
-static int lmmse_threads(int M, int K, size_t* smem) {
-    size_t per_thread = sizeof(float2) * (size_t)(M * M + M * K + M + K * K + K * M);
-    int t = (int)std::min<size_t>(128, (200 * 1024) / per_thread);
-    t = t / 32 * 32;
+// Threads per CTA of a thread-per-vector scratch kernel: at most 128, a multiple of 32, per_thread bytes of shared memory
+// each and at most cap bytes in all; 0 if not even one warp fits.
+static int scratch_threads(size_t per_thread, size_t cap, size_t* smem) {
+    int t = (int)std::min<size_t>(128, cap / per_thread) / 32 * 32;
     if (t < 32) return 0;
     *smem = per_thread * t;
     return t;
 }
+constexpr size_t kLmmseSmemCap = 200 * 1024;
 
 extern "C" int sb_lmmse_equalize(const float* d_y, const float* d_h, const float* d_s, float* d_x_hat, float* d_no_eff,
                                  int64_t num, int32_t M, int32_t K, void* stream) {
     if (num == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_y && d_h && d_s && d_x_hat && d_no_eff && num >= 0 && M >= 1 && K >= 1 && K <= 16 && K <= M,
                  "sb_lmmse_equalize: bad arguments (need 1 <= K <= 16, K <= M)");
-    if (num == 0) return SB_OK;
     size_t smem = 0;
-    int threads = lmmse_threads(M, K, &smem);
+    int threads = scratch_threads(sizeof(float2) * LmmseScratch::elems(M, K), kLmmseSmemCap, &smem);
     if (!threads) { sb_set_error("sb_lmmse_equalize: M = %d too large for the per-thread shared-memory path", M); return SB_EUNSUPPORTED; }
     SB_CUDA(cudaFuncSetAttribute(lmmse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int grid = grid_for(num, threads);
-    lmmse_kernel<<<grid, threads, smem, (cudaStream_t)stream>>>((const float2*)d_y, (const float2*)d_h, (const float2*)d_s,
-                                                               (float2*)d_x_hat, d_no_eff, num, M, K);
+    lmmse_kernel<<<sb_grid(num, threads, 16), threads, smem, (cudaStream_t)stream>>>(
+        (const float2*)d_y, (const float2*)d_h, (const float2*)d_s, (float2*)d_x_hat, d_no_eff, num, M, K);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -1731,15 +1403,14 @@ extern "C" int sb_mimo_linalg(int32_t mode, const float* d_y, const float* d_h, 
     SB_CHECK_ARG(mode != 1 || (d_y && d_s && d_out1), "sb_mimo_linalg: whiten_channel needs y, h, s and two outputs");
     SB_CHECK_ARG(mode != 3 || (d_y && d_s && d_out1), "sb_mimo_linalg: the equaliser needs y, h, s and two outputs");
     if (mode == 0) K = M;
-    const size_t per_thread = sizeof(float2) * ((size_t)M * M + 2 * (size_t)M * K);
     int dev = 0, optin = 0;
     SB_CUDA(cudaGetDevice(&dev));
     SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    int threads = (int)std::min<size_t>(128, (size_t)optin / per_thread) / 32 * 32;
-    if (threads < 32) { sb_set_error("sb_mimo_linalg: M = %d too large for the per-thread shared-memory path", M); return SB_EUNSUPPORTED; }
-    const size_t smem = per_thread * threads;
+    size_t smem = 0;
+    int threads = scratch_threads(sizeof(float2) * ((size_t)M * M + 2 * (size_t)M * K), (size_t)optin, &smem);
+    if (!threads) { sb_set_error("sb_mimo_linalg: M = %d too large for the per-thread shared-memory path", M); return SB_EUNSUPPORTED; }
     SB_CUDA(cudaFuncSetAttribute(mimo_linalg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    mimo_linalg_kernel<<<grid_for(num, threads), threads, smem, (cudaStream_t)stream>>>(
+    mimo_linalg_kernel<<<sb_grid(num, threads, 16), threads, smem, (cudaStream_t)stream>>>(
         mode, (const float2*)d_y, (const float2*)d_h, (const float2*)d_s, (float2*)d_out0, d_out1, num, M, K);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -1776,11 +1447,10 @@ extern "C" int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float
         return SB_OK;
     }
     size_t smem = 0;
-    int threads = lmmse_threads(num_rx_ant, streams_per_rx, &smem);
+    int threads = scratch_threads(sizeof(float2) * LmmseScratch::elems(num_rx_ant, streams_per_rx), kLmmseSmemCap, &smem);
     if (!threads) { sb_set_error("sb_ofdm_lmmse: %d receive antennas too many for the per-thread shared-memory path", num_rx_ant); return SB_EUNSUPPORTED; }
     SB_CUDA(cudaFuncSetAttribute(ofdm_lmmse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    long long total = batch * num_rx * (long long)num_symbols * num_subcarriers;
-    ofdm_lmmse_kernel<<<grid_for(total, threads), threads, smem, (cudaStream_t)stream>>>(p);
+    ofdm_lmmse_kernel<<<sb_grid(total_re, threads, 16), threads, smem, (cudaStream_t)stream>>>(p);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }

@@ -383,22 +383,13 @@ __global__ void scramble_kernel(const float* __restrict__ x, const float* __rest
     }
 }
 
-inline int grid_for(long long work_items, int threads) {
-    int sms = sb_num_sms();
-    long long blocks = (work_items + threads - 1) / threads;
-    long long cap = (long long)sms * 8;
-    if (blocks > cap) blocks = cap;                       // grid-stride beyond 8 CTAs per SM
-    if (blocks < 1) blocks = 1;
-    return (int)blocks;
-}
-
 }  // namespace
 
 extern "C" int sb_binary_source(float* d_out, int64_t n, uint64_t seed, uint64_t offset, void* stream) {
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_out && n >= 0, "sb_binary_source: bad arguments");
     if (n == 0) return SB_OK;
-    binary_source_kernel<<<grid_for((n + 127) / 128, 128), 128, 0, (cudaStream_t)stream>>>(d_out, n, seed, offset);
+    binary_source_kernel<<<sb_grid((n + 127) / 128, 128, 8), 128, 0, (cudaStream_t)stream>>>(d_out, n, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -409,7 +400,7 @@ extern "C" int sb_qam_map(const float* d_bits, const float* d_points, int32_t m,
     SB_CHECK_ARG(d_bits && d_points && d_out && m >= 1 && m <= 12 && n_sym >= 0, "sb_qam_map: bad arguments");
     if (n_sym == 0) return SB_OK;
     size_t smem = sizeof(float2) << m;
-    qam_map_kernel<<<grid_for(n_sym, 256), 256, smem, (cudaStream_t)stream>>>(
+    qam_map_kernel<<<sb_grid(n_sym, 256, 8), 256, smem, (cudaStream_t)stream>>>(
         d_bits, (const float2*)d_points, m, (float2*)d_out, d_idx_out, n_sym);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -425,7 +416,7 @@ extern "C" int sb_demap(const float* d_y, const float* d_no, int64_t no_inner, c
     SB_CHECK_ARG(!d_prior || prior_inner >= 1, "sb_demap: prior_inner must be >= 1");
     if (n_sym == 0) return SB_OK;
     size_t smem = (sizeof(float2) << m) + sizeof(float) * 128 * m;
-    int grid = grid_for(n_sym, 128);
+    int grid = sb_grid(n_sym, 128, 8);
     if (method == 0)
         launch_demap<0>(m, grid, smem, (cudaStream_t)stream, (const float2*)d_y, d_no, no_inner, (const float2*)d_points,
                         d_prior, prior_inner, d_llr, n_sym, hard_out);
@@ -442,7 +433,7 @@ extern "C" int sb_demap_qam(const float* d_y, const float* d_no, int64_t no_inne
     if (n_sym == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_y && d_no && d_levels_re && d_levels_im && d_llr && m >= 2 && m <= 10 && m % 2 == 0 && no_inner >= 1 &&
                      (method == 0 || method == 1), "sb_demap_qam: bad arguments (m even, 2..10; method 0 | 1)");
-    int grid = grid_for(n_sym, 128);
+    int grid = sb_grid(n_sym, 128, 8);
     if (method == 0)
         launch_demap_qam<0>(m / 2, grid, (cudaStream_t)stream, (const float2*)d_y, d_no, no_inner, d_levels_re, d_levels_im,
                             d_llr, n_sym, hard_out);
@@ -458,7 +449,7 @@ extern "C" int sb_awgn(const float* d_x, const float* d_no, int64_t no_inner, fl
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_x && d_no && d_y && n >= 0 && no_inner >= 1, "sb_awgn: bad arguments");
     if (n == 0) return SB_OK;
-    awgn_kernel<<<grid_for((n + 1) / 2, 256), 256, 0, (cudaStream_t)stream>>>((const float2*)d_x, d_no, no_inner,
+    awgn_kernel<<<sb_grid((n + 1) / 2, 256, 8), 256, 0, (cudaStream_t)stream>>>((const float2*)d_x, d_no, no_inner,
                                                                               (float2*)d_y, n, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -468,7 +459,7 @@ extern "C" int sb_normal(float* d_out, int64_t n, float mean, float stddev, uint
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_out && n >= 0, "sb_normal: bad arguments");
     if (n == 0) return SB_OK;
-    normal_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, (cudaStream_t)stream>>>(d_out, n, mean, stddev, seed, offset);
+    normal_kernel<<<sb_grid((n + 3) / 4, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_out, n, mean, stddev, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -476,7 +467,7 @@ extern "C" int sb_normal(float* d_out, int64_t n, float mean, float stddev, uint
 extern "C" int sb_uniform(float* d_out, int64_t n, float lo, float hi, uint64_t seed, uint64_t offset, void* stream) {
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_out && n >= 0 && hi >= lo, "sb_uniform: bad arguments");
-    uniform_kernel<<<grid_for((n + 3) / 4, 256), 256, 0, (cudaStream_t)stream>>>(d_out, n, lo, hi, seed, offset);
+    uniform_kernel<<<sb_grid((n + 3) / 4, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_out, n, lo, hi, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -486,7 +477,7 @@ extern "C" int sb_count_errors(const float* d_b, const float* d_b_hat, int64_t r
     if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_b && d_b_hat && d_counters && rows >= 0 && k >= 1, "sb_count_errors: bad arguments");
     if (rows == 0) return SB_OK;
-    count_errors_kernel<<<grid_for(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(
+    count_errors_kernel<<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(
         d_b, d_b_hat, rows, k, (unsigned long long*)d_counters);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -498,7 +489,7 @@ extern "C" int sb_crc_encode(const float* d_bits, const uint32_t* d_gen_rows, in
     SB_CHECK_ARG(d_bits && d_gen_rows && d_out && k >= 1 && crc_length >= 1 && crc_length <= 32 && rows >= 0,
                  "sb_crc_encode: bad arguments");
     if (rows == 0) return SB_OK;
-    crc_encode_kernel<<<grid_for(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(d_bits, d_gen_rows, k, crc_length, d_out, rows);
+    crc_encode_kernel<<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_bits, d_gen_rows, k, crc_length, d_out, rows);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -508,7 +499,7 @@ extern "C" int sb_crc_check(const float* d_x, const uint32_t* d_gen_rows, int32_
     if (rows == 0) return SB_OK;
     SB_CHECK_ARG(d_x && d_gen_rows && d_valid && crc_length >= 1 && crc_length <= 32 && n >= crc_length && rows >= 0,
                  "sb_crc_check: bad arguments");
-    crc_check_kernel<<<grid_for(rows * 32, 256), 256, 0, (cudaStream_t)stream>>>(d_x, d_gen_rows, n, crc_length, d_info, d_valid, rows);
+    crc_check_kernel<<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_x, d_gen_rows, n, crc_length, d_info, d_valid, rows);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -518,7 +509,7 @@ extern "C" int sb_scramble(const float* d_x, const float* d_seq, int32_t binary,
     if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_x && d_seq && d_out && rows >= 0 && n >= 1 && seq_rows >= 1, "sb_scramble: bad arguments");
     if (rows == 0) return SB_OK;
-    scramble_kernel<<<grid_for(rows * n, 256), 256, 0, (cudaStream_t)stream>>>(d_x, d_seq, binary, d_out, rows, n, seq_rows);
+    scramble_kernel<<<sb_grid(rows * n, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_x, d_seq, binary, d_out, rows, n, seq_rows);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }

@@ -2,7 +2,7 @@
 of SURVEY.md section 8(f3); mirror of /root/reference/src/sionna/phy/channel/tr38901/tdl.py:20-590 and of
 channel/utils.py:180-253, 1010-1060. Power delay profiles: TR 38.901 Tables 7.7.2-1..5 and TS 38.104 Annex G
 (``tdl_models.npz``, tools/make_code_tables.py). Random draws (``sb_uniform``), tap synthesis (``sb_tdl_sos``) and the
-frequency response (``sb_cir_to_ofdm``) are hand-written kernels."""
+frequency response (``sb_phase_table``, ``sb_cir_gram``, ``sb_cir_link_scale``, ``sb_cir_apply``) are hand-written kernels."""
 import os
 import numpy as np
 import torch

@@ -8,7 +8,7 @@ cap() {  # name kernel-regex
 cap demapper_app_64qam demap_qam_kernel
 cap demapper_maxlog_64qam demap_qam_kernel
 cap ofdm_demodulate_76 ofdm_fft_small_kernel
-cap ofdm_modulate_4096 ofdm_mod_kernel
+cap ofdm_modulate_4096 ofdm_fft_r16_kernel
 cap ofdm_lmmse_4x16 ofdm_lmmse_diag_kernel
 cap ls_estimator_lin_4x16 interp_lin_kernel
 cap ldpc5g_encode_4224_8448 ldpc5g_encode_kernel
