@@ -48,7 +48,7 @@ struct QcParams {
     int early;               // opt-in early termination by the syndrome of the hard decisions (see the kernel)
     int* iters_out;          // [B] iterations actually run per codeword, or nullptr
     const int2* row_edge;    // [nnz] per base entry (processing order): {column * Z, shift}  (syndrome pass only)
-    int tab_rep;             // copies of the phi log table in shared memory (32, 8 or 1; 0: rule does not use it)
+    int tab_rep;             // copies of the phi log table in shared memory (16, 8 or 1; 0: rule does not use it)
     float offset, llr_max;
 };
 
@@ -63,8 +63,8 @@ struct QcParams {
 //   (1) |x| >= 16.635532 (the phi clipping bound, :1113)  =>  phi(|x|) == 0 exactly              [saturated inputs]
 //   (2) p_e == 0  =>  P - p_e == P exactly  =>  phi(P - p_e) == phi(P), evaluated once per check
 //   (3) P - p_e <= 8.5e-8 (lower clipping bound)  =>  phi(P - p_e) == phi(8.5e-8) == phi_max
-// Once a codeword has converged every VN->CN message except those of degree-1 VNs sits at +-llr_max >= 16.64, and a
-// check costs ~3 phi evaluations instead of 2*deg; the per-iteration cost therefore depends on the channel SNR.
+// Once a codeword has converged most VN->CN messages except those of degree-1 VNs sit at +-llr_max >= 16.64, and a
+// check costs ~2 phi evaluations instead of 2*deg; the per-iteration cost therefore depends on the channel SNR.
 #ifndef SB_PHI_UNROLL
 // edge pairs per trip of the phi loops (an A/B variant is built with -DSB_PHI_UNROLL=n and selected with
 // SIONNA_B200_LIB)
@@ -75,7 +75,8 @@ struct QcParams {
 #define SB_PHI_HI 16.635532f
 #define SB_PHI_LO 8.5e-8f
 // SC = false: plain evaluation; one vote per check on its first edge pair probes for saturation and raises *sat_flag,
-// which makes the CTA use the SC = true variant (votes on every pair) from the next iteration on.
+// which makes the CTA use the SC = true variant (one vote per row for a saturated row, else votes on every pair) from
+// the next iteration on.
 // Out of line on purpose: the five degree classes then share ONE copy of each variant's loops (the kernel is bound by
 // instruction fetch as much as by issue: 12.35 -> 11.85 ms per 4096 codewords at 2 dB; making phi itself a call costs more
 // than it saves, 12.8 ms).
@@ -83,6 +84,32 @@ template <bool SC, class LT>
 __device__ __noinline__ void cn_phi_qc(float* pm, int Z, int deg, float clip, float phi_max, int* sat_flag,
                                        const LT& lt) {
     const unsigned am = __activemask();                   // lanes of this warp working on the same block row
+    if (SC) {
+        // Saturated row (one vote per row): every edge but the last has |x| >= 16.635532. Their phi are +0 (1), so
+        // P = p_last exactly; each of them gets phi(P) whichever of (2), (3) or a full evaluation the general code below
+        // would take, and the last edge gets phi(P - p_last) = phi(+0) = phi_max (3). Two phi per row, no per-pair votes
+        // and no stores between the two passes.
+        unsigned par = 0;
+        bool sat = true;
+        for (int k = 0; k + 1 < deg; ++k) {
+            const unsigned b = __float_as_uint(pm[k * Z]);
+            par ^= b;
+            sat = sat && fabsf(__uint_as_float(b)) >= SB_PHI_HI;
+        }
+        if (__all_sync(am, sat)) {
+            float* ql = pm + (deg - 1) * Z;
+            const unsigned bl = __float_as_uint(*ql);
+            par = (par ^ bl) & 0x80000000u;
+            const float pl = sb_phif_s(__uint_as_float(bl & 0x7fffffffu), lt);
+            const unsigned y = __float_as_uint(fminf(sb_phif_s(pl, lt), clip));
+            for (int k = 0; k + 1 < deg; ++k) {
+                float* q = pm + k * Z;
+                *q = __uint_as_float(y | ((__float_as_uint(*q) ^ par) & 0x80000000u));
+            }
+            *ql = __uint_as_float(__float_as_uint(fminf(phi_max, clip)) | ((bl ^ par) & 0x80000000u));
+            return;
+        }
+    }
     float P = 0.f;
     unsigned par = 0;
     int l = 0;
@@ -569,14 +596,15 @@ __device__ __forceinline__ void vn_all(const QcParams& p, const WarpCtx& w, uint
 #endif
 __host__ __device__ constexpr int qc_max_threads(int rule) { return rule == SB_CN_BOXPLUS_PHI ? SB_QC_PHI_THREADS : 768; }
 
-// REP: copies of the phi log table (32, 8 or 1). EARLY: the early-termination variant (hard-decision bytes + syndrome
+// REP: copies of the phi log table (16, 8 or 1). EARLY: the early-termination variant (hard-decision bytes + syndrome
 // pass); a separate instantiation so that the default kernel carries none of it (as a run-time flag it cost 2 %).
 template <int RULE, int REP, bool EARLY>
 __global__ void __launch_bounds__(qc_max_threads(RULE), 1) ldpc_bp_qc_kernel(const __grid_constant__ QcParams p) {
-    extern __shared__ __align__(16) unsigned char smem_raw[];
     const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, W = T >> 5;
     const int Z = p.Z, N = p.N, Zb = (Z + 31) >> 5;
-    // carve-up by byte offsets from the __shared__ base (keeps the shared address space visible to the compiler)
+    // carve-up by byte offsets from the __shared__ base (keeps the shared address space visible to the compiler): the
+    // phi log table at offset 0 (sb_math2.cuh), then the messages
+    unsigned char* const smem_raw = sb_smem + (RULE == SB_CN_BOXPLUS_PHI ? LogTab<REP>::bytes : 0);
     const int off_llr = p.E_alloc * 4;
     const int off_col = (off_llr + N * 4 + 15) & ~15;
     const int off_row = off_col + p.n_cols * 16;
@@ -590,9 +618,7 @@ __global__ void __launch_bounds__(qc_max_threads(RULE), 1) ldpc_bp_qc_kernel(con
     uint64_t* bar = reinterpret_cast<uint64_t*>(smem_raw + off_bar);
     int* sat_flag = reinterpret_cast<int*>(smem_raw + off_bar + 8);
     int* unsat = reinterpret_cast<int*>(smem_raw + off_bar + 12);
-    const int off_tab = off_bar + 16;                     // phi log table, tab_rep copies interleaved per entry
-    // early termination: one hard-decision byte per VN behind the table
-    unsigned char* hd = EARLY ? smem_raw + off_tab + (RULE == SB_CN_BOXPLUS_PHI ? REP * SB_LOGTAB_N * 8 : 0) : nullptr;
+    unsigned char* hd = EARLY ? smem_raw + off_bar + 16 : nullptr;   // early termination: one hard-decision byte per VN
     const uint32_t msgb = smem_u32(smem_raw);             // 32-bit shared-window addresses for the hot loops
     const uint32_t s_ce = msgb + off_ce;
     // a warp keeps one 32-lane slice `ib` of every block row/column it visits; G warp groups share the rows
@@ -604,18 +630,8 @@ __global__ void __launch_bounds__(qc_max_threads(RULE), 1) ldpc_bp_qc_kernel(con
     for (int i = tid; i < p.n_cols; i += T) s_col[i] = p.col_info[i];
     for (int i = tid; i < p.n_rows; i += T) s_row[i] = p.row_info[i];
     for (int i = tid; i < p.nnz; i += T) s_ce_p[i] = p.col_edge[i];
-    LogTab<REP> lt;
-    lt.inv = 0; lt.lane_off = 0;
-    if (RULE == SB_CN_BOXPLUS_PHI) {
-        // two arrays of SB_LOGTAB_N * REP floats; entry i, copy c at (i * REP + c) * 4: with REP = 32 lane l reads bank l
-        float* tab = reinterpret_cast<float*>(smem_raw + off_tab);
-        for (int i = tid; i < SB_LOGTAB_N * REP; i += T) {
-            tab[i] = sb_logtab_dev[2 * (i / REP)];
-            tab[SB_LOGTAB_N * REP + i] = sb_logtab_dev[2 * (i / REP) + 1];
-        }
-        lt.inv = msgb + off_tab;
-        lt.lane_off = 4 * (lane & (REP - 1));
-    }
+    const LogTab<REP> lt(lane);
+    if (RULE == SB_CN_BOXPLUS_PHI) LogTab<REP>::fill(tid, T);
     if (p.use_tma && tid == 0) {
         mbar_init(bar, 1);
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
@@ -730,7 +746,7 @@ int qc_ensure_uploaded(sb_ldpc_graph* g) {
 
 template <int RULE, bool EARLY>
 int launch_qc_e(const sb_ldpc_graph* g, const QcParams& p, int threads, size_t smem, cudaStream_t stream) {
-    auto kern = ldpc_bp_qc_kernel<RULE, 32, EARLY>;
+    auto kern = ldpc_bp_qc_kernel<RULE, 16, EARLY>;
     if constexpr (RULE == SB_CN_BOXPLUS_PHI) {
         if (p.tab_rep == 8) kern = ldpc_bp_qc_kernel<RULE, 8, EARLY>;
         if (p.tab_rep == 1) kern = ldpc_bp_qc_kernel<RULE, 1, EARLY>;
@@ -919,15 +935,9 @@ extern "C" int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entri
 // Test hook: evaluates phi on the device with the scalar (sb_math.h) and the packed (sb_math2.cuh) implementation.
 namespace {
 __global__ void debug_phi_kernel(const float* x, float* o1, float* o2, long long n) {
-    __shared__ float tab[2 * SB_LOGTAB_N * 32];           // the 32-copy layout of the decoder
-    for (int i = threadIdx.x; i < SB_LOGTAB_N * 32; i += blockDim.x) {
-        tab[i] = sb_logtab_dev[2 * (i / 32)];
-        tab[SB_LOGTAB_N * 32 + i] = sb_logtab_dev[2 * (i / 32) + 1];
-    }
+    LogTab<16>::fill(threadIdx.x, blockDim.x);            // the 16-copy layout of the decoder
     __syncthreads();
-    LogTab<32> lt;
-    lt.inv = smem_u32(tab);
-    lt.lane_off = 4 * (threadIdx.x & 31);
+    const LogTab<16> lt(threadIdx.x & 31);
     long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (2 * i + 1 < n) {
         float2 r = sb_phif2(make_float2(x[2 * i], x[2 * i + 1]), lt);
@@ -940,7 +950,8 @@ extern "C" int sb_debug_phi(const float* d_x, float* d_scalar, float* d_packed, 
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_x && d_scalar && d_packed && n >= 0 && n % 2 == 0, "sb_debug_phi: bad arguments");
     if (n == 0) return SB_OK;
-    debug_phi_kernel<<<(unsigned)((n / 2 + 255) / 256), 256, 0, (cudaStream_t)stream>>>(d_x, d_scalar, d_packed, n);
+    debug_phi_kernel<<<(unsigned)((n / 2 + 255) / 256), 256, LogTab<16>::bytes, (cudaStream_t)stream>>>(d_x, d_scalar,
+                                                                                                         d_packed, n);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -952,8 +963,8 @@ int sb_qc_try_decode(sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_
                      float* d_state_out, float* d_out, cudaStream_t stream, bool* handled, int32_t early, int32_t* d_iters) {
     *handled = false;
     if (!g->qc || !g->flooding || vn_rule != SB_VN_SUM || d_state_in || cn_rule > SB_CN_OFFSET_MINSUM) return SB_OK;
-    // boxplus-phi keeps the log table of phi in shared memory: one copy per bank pair if it fits, else a single copy
-    int tab_rep = cn_rule == SB_CN_BOXPLUS_PHI ? 32 : 0;
+    // boxplus-phi keeps the log table of phi in shared memory: one copy per bank pair if it fits, else 8 copies or one
+    int tab_rep = cn_rule == SB_CN_BOXPLUS_PHI ? 16 : 0;
     if (tab_rep && qc_smem_bytes(g, tab_rep, early) > (size_t)g->smem_optin) tab_rep = 8;
     if (tab_rep && qc_smem_bytes(g, tab_rep, early) > (size_t)g->smem_optin) tab_rep = 1;
     const size_t smem = qc_smem_bytes(g, tab_rep, early);

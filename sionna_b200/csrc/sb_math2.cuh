@@ -22,7 +22,6 @@ __device__ __forceinline__ float2 fmul2(float2 a, float2 b) { return make_float2
 __device__ __forceinline__ float2 sb_expf2_inrange(float2 x) {
     float2 t = ffma2(x, f2s(1.44269504088896341f), f2s(12582912.0f));
     float2 nf = fadd2(t, f2s(-12582912.0f));
-    int n0 = f2i_mov(t.x) - 0x4B400000, n1 = f2i_mov(t.y) - 0x4B400000;
     float2 r = ffma2(nf, f2s(-0.693145751953125f), x);
     r = ffma2(nf, f2s(-1.42860677e-06f), r);
     float2 g = ffma2(f2s(0x1.a124e4p-13f), r, f2s(0x1.6d4316p-10f));
@@ -33,7 +32,9 @@ __device__ __forceinline__ float2 sb_expf2_inrange(float2 x) {
     float2 r2 = fmul2(r, r);
     float2 s = ffma2(r2, g, r);
     float2 p = fadd2(f2s(1.0f), s);
-    return f2(i2f_mov(f2i_mov(p.x) + (n0 << 23)), i2f_mov(f2i_mov(p.y) + (n1 << 23)));
+    // bits(p) + (n << 23) with n = bits(t) - 0x4B400000: 0x4B400000 << 23 vanishes mod 2^32, so one LEA per element
+    return f2(i2f_mov((int)((unsigned)f2i_mov(p.x) + ((unsigned)f2i_mov(t.x) << 23))),
+              i2f_mov((int)((unsigned)f2i_mov(p.y) + ((unsigned)f2i_mov(t.y) << 23))));
 }
 
 // log(y) for positive normal y
@@ -60,18 +61,29 @@ __device__ __forceinline__ float2 sb_logf2(float2 y) {
     return ffma2(ef, f2s(0.693145751953125f), t2);
 }
 
-// Shared-memory copy of the sb_logf_tab table (sb_math.h), split into an inv_c array and a log c array so that the
-// packed code loads each operand straight into its register pair. Entry i of this lane's copy sits at offset
-// ((bits(y) >> rs) & mask) | lane_off of either array: the host picks the replication factor -- 32 copies (one per bank,
-// conflict-free LDS: rs 10, mask 0x1f80, lane_off 4*lane) when the table fits next to the messages, else a single copy
-// (rs 15, mask 0xfc, lane_off 0).
-template <int REP>                                        // REP = 32, 8 or 1 copies: compile-time shift, mask, distance
+// Dynamic shared memory of the kernels that use the table below; the table sits at its offset 0.
+extern __shared__ __align__(16) unsigned char sb_smem[];
+
+// Shared-memory copy of the sb_logf_tab table (sb_math.h) at offset 0 of the dynamic shared memory: entry i is the
+// pair {inv_c, log c}, read with one 64-bit LDS. REP copies are interleaved per entry (entry i, copy c at byte
+// (i * REP + c) * 8) and lane l reads copy l % REP, so the lookup offset is ((bits(y) >> rs) & mask) | lane_off. A 64-bit
+// warp access is served as two half-warps, so 16 copies (one per bank pair, 8 KB: rs 10, mask 0x1f80, lane_off
+// 8 * (lane % 16)) are conflict-free. The host falls back to 8 copies or a single one when the table does not fit next
+// to the messages.
+template <int REP>                                        // REP = 16, 8 or 1 copies: compile-time shift and mask
 struct LogTab {
-    uint32_t inv, lane_off;                               // `inv` is CTA-uniform; the log c array follows the inv_c array
-    static constexpr int log_stride = REP == 32 ? 7 : (REP == 8 ? 5 : 2);   // log2(REP * 4 bytes)
+    uint32_t lane_off;
+    static constexpr int bytes = SB_LOGTAB_N * REP * 8;
+    static constexpr int log_stride = REP == 16 ? 7 : (REP == 8 ? 6 : 3);   // log2(REP * 8 bytes)
     static constexpr int rs = SB_LOGTAB_SHIFT - log_stride;
     static constexpr int mask = (SB_LOGTAB_N - 1) << log_stride;
-    static constexpr int dist = SB_LOGTAB_N * REP * 4;
+    // every thread of the CTA stores a share of the table; a barrier must follow before the first lookup
+    __device__ static void fill(int tid, int T) {
+        float2* tab = reinterpret_cast<float2*>(sb_smem);
+        for (int i = tid; i < SB_LOGTAB_N * REP; i += T)
+            tab[i] = make_float2(sb_logtab_dev[2 * (i / REP)], sb_logtab_dev[2 * (i / REP) + 1]);
+    }
+    __device__ explicit LogTab(int lane) : lane_off(8 * (lane & (REP - 1))) {}
 };
 
 // (a & MASK) | c in one LOP3 (c in a register; nvcc otherwise emits two LOP3 when both constants are immediates)
@@ -82,22 +94,29 @@ __device__ __forceinline__ int and_or(int a, int c) {
     return d;
 }
 
-__device__ __forceinline__ float lds_ro(uint32_t a) {
-    float v;
-    asm("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a));     // read-only after the prologue barrier
+// {inv_c, log c} of bits(y) = ix from this lane's copy of the table. The base address of the dynamic shared memory is
+// CTA-uniform, so it folds into the LDS address operand.
+template <class LT>
+__device__ __forceinline__ float2 logtab_entry(int ix, const LT& lt) {
+    float2 v;
+    asm("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(v.x), "=f"(v.y)      // read-only after the prologue barrier
+        : "r"((uint32_t)__cvta_generic_to_shared(sb_smem) + and_or<LT::mask>(ix >> LT::rs, lt.lane_off)));
     return v;
 }
+
+// E - 127 of bits(y) = ix > 0 as 12582912 + E before the subtraction: float(0x4B400000 + E) is exact, and
+// (ix >> 23) + 0x4B400000 is one LEA.HI
+__device__ __forceinline__ float logtab_expf(int ix) { return i2f_mov((int)(((unsigned)ix >> 23) + 0x4B400000u)); }
 
 // sb_logf_tab, two at a time (same operation sequence per element)
 template <class LT>
 __device__ __forceinline__ float2 sb_logf2_tab(float2 y, const LT& lt) {
     int ix0 = f2i_mov(y.x), ix1 = f2i_mov(y.y);
-    uint32_t o0 = lt.inv + (((ix0 >> LT::rs) & LT::mask) | lt.lane_off);
-    uint32_t o1 = lt.inv + (((ix1 >> LT::rs) & LT::mask) | lt.lane_off);
-    float2 inv_c = f2(lds_ro(o0), lds_ro(o1));
-    float2 logc = f2(lds_ro(o0 + LT::dist), lds_ro(o1 + LT::dist));
+    float2 c0 = logtab_entry(ix0, lt), c1 = logtab_entry(ix1, lt);
+    float2 inv_c = f2(c0.x, c1.x);
+    float2 logc = f2(c0.y, c1.y);
     float2 m = f2(i2f_mov(and_or<0x007fffff>(ix0, 0x3f800000)), i2f_mov(and_or<0x007fffff>(ix1, 0x3f800000)));
-    float2 F = f2(i2f_mov((int)((unsigned)ix0 >> 23) | 0x4B400000), i2f_mov((int)((unsigned)ix1 >> 23) | 0x4B400000));
+    float2 F = f2(logtab_expf(ix0), logtab_expf(ix1));
     float2 ef = fadd2(F, f2s(-12583039.0f));
     float2 r = ffma2(m, inv_c, f2s(-1.0f));
     float2 q = ffma2(r, f2s(-0.25f), f2s(0x1.555556p-2f));
@@ -112,8 +131,8 @@ __device__ __forceinline__ float2 sb_logf2_tab(float2 y, const LT& lt) {
 template <class LT>
 __device__ __forceinline__ float sb_logf_tab_s(float y, const LT& lt) {
     int ix = __float_as_int(y);
-    uint32_t o = lt.inv + (((ix >> LT::rs) & LT::mask) | lt.lane_off);
-    return sb_logf_tab_core(ix, lds_ro(o), lds_ro(o + LT::dist));
+    float2 c = logtab_entry(ix, lt);
+    return sb_logf_tab_core(ix, c.x, c.y);
 }
 
 // phi(x) = log(e^x + 1) - log(e^x - 1) with the reference's fp32 clipping (see sb_phif)
