@@ -314,14 +314,20 @@ int sb_pusch_precode(const float* d_x, const float* d_w, float* d_y, int64_t bat
 int sb_pusch_ls_combine(float* d_h, float* d_err_var, int64_t rows, int32_t num_pilots, int32_t pilots_per_dmrs_symbol,
                         int32_t dmrs_length, int32_t group_size, void* stream);
 /* lmmse_equalizer (mimo/equalization.py:101-233, whiten_interference=True): d_y [num, M], d_h [num, M, K], d_s [num, M, M]
- * -> d_x_hat [num, K] complex, d_no_eff [num, K] real. 1 <= K <= 16, K <= M. */
+ * -> d_x_hat [num, K] complex, d_no_eff [num, K] real. 1 <= K <= 16, K <= M, and the per-vector scratch
+ * 8 (M^2 + 2 M K + M + K^2) bytes must fit 200 KB: M <= 158 for K = 1, M <= 143 for K = 16. Shapes whose scratch
+ * leaves room for fewer than 32 vectors per CTA run with 16 ... 1 threads per CTA (correct, not tuned for speed);
+ * larger ones return SB_EUNSUPPORTED. */
 int sb_lmmse_equalize(const float* d_y, const float* d_h, const float* d_s, float* d_x_hat, float* d_no_eff, int64_t num,
                       int32_t M, int32_t K, void* stream);
 /* The reference's small dense helpers as callable kernels (complex64, one thread per matrix):
  *   mode 0  inv_cholesky(s)          utils/linalg.py:8-32         d_s [num, M, M] -> d_out0 = L^-1 [num, M, M]
  *   mode 1  whiten_channel(y, h, s)  mimo/utils.py:292-357        -> d_out0 = L^-1 y [num, M], d_out1 = L^-1 H [num, M, K]
  *   mode 2  lmmse_matrix(h, s)       mimo/equalization.py:11-99   -> d_out0 = G [num, K, M]; d_s == NULL: (H^H H + I)^-1 H^H
- *   mode 3  lmmse_equalizer(y, h, s, whiten_interference=False) :183-233 -> d_out0 = x_hat [num, K], d_out1 = no_eff (fp32) */
+ *   mode 3  lmmse_equalizer(y, h, s, whiten_interference=False) :183-233 -> d_out0 = x_hat [num, K], d_out1 = no_eff (fp32)
+ * 1 <= K <= M (mode 0: K = M). The per-matrix scratch 8 (M^2 + 2 M K) bytes must fit the device's opt-in shared memory per
+ * block (227 KB on H100: inv_cholesky up to M = 98, M <= 155 for K = 16); below 32 matrices per CTA the kernel runs
+ * with 16 ... 1 threads per CTA (correct, not tuned for speed); larger shapes return SB_EUNSUPPORTED. */
 int sb_mimo_linalg(int32_t mode, const float* d_y, const float* d_h, const float* d_s, float* d_out0, void* d_out1,
                    int64_t num, int32_t M, int32_t K, void* stream);
 /* OFDMEqualizer.call with the LMMSE equaliser fused in (ofdm/equalization.py:109-275 + mimo/equalization.py:101-233):
@@ -331,7 +337,10 @@ int sb_mimo_linalg(int32_t mode, const float* d_y, const float* d_h, const float
  * d_desired [num_rx, streams_per_rx] / d_undesired [num_rx, interferers_per_rx]: tx-stream indices per receiver
  * (mimo/stream_management.py:200-246); d_out_stream [num_rx, streams_per_rx]: output stream row after the stream_ind
  * re-ordering; d_data_pos [num_tx_streams, num_symbols*num_subcarriers]: index among that stream's data symbols or -1.
- * Outputs d_x_hat / d_no_eff [batch, num_tx_streams, num_data]. */
+ * Outputs d_x_hat / d_no_eff [batch, num_tx_streams, num_data]. 1 <= streams_per_rx <= min(16, num_rx_ant). Receivers
+ * without interfering streams and streams_per_rx <= 4 run a register kernel with no limit on num_rx_ant; the others keep
+ * 8 (M^2 + 2 M K + M + K^2) bytes of scratch per resource element (M = num_rx_ant, K = streams_per_rx) in shared memory,
+ * which must fit 200 KB (M <= 143 for K = 16), with 16 ... 1 threads per CTA when fewer than 32 fit. */
 int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
                   const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired, const int32_t* d_undesired,
                   const int32_t* d_out_stream, const int32_t* d_data_pos, float* d_x_hat, float* d_no_eff, int64_t batch,

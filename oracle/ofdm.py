@@ -209,9 +209,62 @@ def lmmse_equalizer_f32(y, h, s):
     return (gy / d).astype(np.complex64), np.real(one / d - one).astype(np.float32)
 
 
+def _herm(a):
+    return np.conj(np.swapaxes(a, -1, -2))
+
+
+def _cholesky_solve(a, b):
+    """tf.linalg.cholesky_solve(tf.linalg.cholesky(a), b)."""
+    l = np.linalg.cholesky(a)
+    return np.linalg.solve(_herm(l), np.linalg.solve(l, b))
+
+
+def inv_cholesky(s):
+    """utils/linalg.py:28-32: L^-1 = triangular_solve(chol(s), I). Keeps the precision of s."""
+    return np.linalg.solve(np.linalg.cholesky(s), np.broadcast_to(np.eye(s.shape[-1], dtype=s.dtype), s.shape))
+
+
+def whiten_channel(y, h, s):
+    """mimo/utils.py:343-347: (L^-1 y, L^-1 H). Keeps the precision of the inputs."""
+    l_inv = inv_cholesky(s)
+    return (l_inv @ y[..., None])[..., 0], l_inv @ h
+
+
+def lmmse_matrix(h, s=None):
+    """mimo/equalization.py:76-97: G = (cholesky_solve(H H^H + S, H))^H, or with s None
+    G = cholesky_solve(H^H H + I, H^H). Keeps the precision of the inputs."""
+    if s is None:
+        return _cholesky_solve(_herm(h) @ h + np.eye(h.shape[-1], dtype=h.dtype), _herm(h))
+    return _herm(_cholesky_solve(h @ _herm(h) + s, h))
+
+
+def lmmse_equalizer_cholesky(y, h, s, whiten_interference=True):
+    """mimo/equalization.py:183-233 step by step as the reference evaluates it (whitening, then the Cholesky-based
+    lmmse_matrix), in the precision of the inputs: complex64 inputs give the reference's own fp32 error envelope."""
+    if whiten_interference:
+        y, h = whiten_channel(y, h, s)
+        g = lmmse_matrix(h)
+    else:
+        g = lmmse_matrix(h, s)
+    d = np.diagonal(g @ h, axis1=-2, axis2=-1)
+    one = np.ones((), y.real.dtype)
+    return (g @ y[..., None])[..., 0] / d, np.real(one / d - one)
+
+
 def ofdm_lmmse_equalize(y_eff, h_hat, err_var, no, mask, sm):
     """OFDMEqualizer.call + lmmse_equalizer (ofdm/equalization.py:126-275). y_eff [B, rx, ant, S, F] (effective
     subcarriers), h_hat [B, rx, ant, tx, st, S, F] -> x_hat, no_eff [B, tx, st, num_data]."""
+    return _ofdm_lmmse(y_eff, h_hat, err_var, no, mask, sm, np.complex128, np.float64, lmmse_equalizer)
+
+
+def ofdm_lmmse_equalize_f32(y_eff, h_hat, err_var, no, mask, sm):
+    """ofdm_lmmse_equalize with every step in complex64 / float32 (S assembled, then lmmse_equalizer_cholesky): the
+    reference's own single-precision error envelope."""
+    return _ofdm_lmmse(y_eff, h_hat, err_var, no, mask, sm, np.complex64, np.float32, lmmse_equalizer_cholesky)
+
+
+def _ofdm_lmmse(y_eff, h_hat, err_var, no, mask, sm, cdt, rdt, equalizer):
+    y_eff, h_hat, err_var = y_eff.astype(cdt), h_hat.astype(cdt), np.asarray(err_var).astype(rdt)
     b, rx, ant, s_, f_ = y_eff.shape
     tx, st = h_hat.shape[3:5]
     y_dt = np.transpose(y_eff, [0, 1, 3, 4, 2])
@@ -222,12 +275,12 @@ def ofdm_lmmse_equalize(y_eff, h_hat, err_var, no, mask, sm):
     hu = h_dt[sm["undesired"]].reshape(rx, -1, b, ant, s_, f_)
     hd = np.transpose(hd, [2, 0, 4, 5, 3, 1])
     hu = np.transpose(hu, [2, 0, 4, 5, 3, 1])
-    no_b = np.broadcast_to(np.asarray(no, np.float64).reshape(np.shape(no) + (1,) * (3 - np.ndim(no))), (b, rx, ant))
+    no_b = np.broadcast_to(np.asarray(no, rdt).reshape(np.shape(no) + (1,) * (3 - np.ndim(no))), (b, rx, ant))
     no_dt = np.transpose(np.broadcast_to(no_b[..., None, None], (b, rx, ant, s_, f_)), [0, 1, 3, 4, 2])
     s = hu @ np.conj(np.swapaxes(hu, -1, -2))
     idx = np.arange(ant)
     s[..., idx, idx] += no_dt + ev.sum(-1)
-    x_hat, no_eff = lmmse_equalizer(y_dt, hd, s)                       # [B, rx, S, F, K]
+    x_hat, no_eff = equalizer(y_dt, hd, s)                             # [B, rx, S, F, K]
     x_hat = np.transpose(x_hat, [1, 4, 2, 3, 0]).reshape(rx * sm["spr"], s_, f_, b)[sm["stream_ind"]]
     no_eff = np.transpose(no_eff, [1, 4, 2, 3, 0]).reshape(rx * sm["spr"], s_, f_, b)[sm["stream_ind"]]
     x_hat = x_hat.reshape(tx, st, s_ * f_, b)

@@ -78,7 +78,9 @@ __device__ void fft_inplace_smem(float2* buf0, float2* buf1, const float2* W, co
 //   DEMOD = 0, OFDMModulator: x [rows, nsym, N] (frequency domain, DC in the centre) -> out [rows, sum_l (N + cp[l])]
 //     ifftshift -> ifft * sqrt(N) -> cyclic prefix (modulator.py:100-124, signal/utils.py:240-249).
 //   DEMOD = 1, OFDMDemodulator: x [rows, >= sum_l (N + cp[l])] -> out [rows, nsym, N]: strip CP, fft / sqrt(N), phase
-//     compensation exp(-j 2 pi k l_min / N) (fp32 table, demodulator.py:131-134, 196-198), fftshift (:201).
+//     compensation exp(-j 2 pi k l_min / N) (fp32, demodulator.py:131-134, 196-198), fftshift (:201).
+// Shared memory: 3 N float2 (two data buffers and the twiddles), so N = 8192 fits the 227 KB opt-in limit. The phase
+// compensation is evaluated per output bin rather than tabulated: a fourth N-entry table would cap N at 7264.
 template <int DEMOD>
 __global__ void ofdm_fft_kernel(const float2* __restrict__ x, float2* __restrict__ out, FftPlan plan, int nsym,
                                 const int* __restrict__ cp, const int* __restrict__ off, int len, int l_min,
@@ -86,16 +88,10 @@ __global__ void ofdm_fft_kernel(const float2* __restrict__ x, float2* __restrict
     extern __shared__ float2 sm[];
     const int N = plan.n, tid = threadIdx.x, T = blockDim.x;
     float2* b0 = sm; float2* b1 = sm + N; float2* W = sm + 2 * N;
-    float2* PC = sm + 3 * N;                                       // phase compensation (demodulator only)
     for (int k = tid; k < N; k += T) {
         float sn, cs;
         sincospif(-2.0f * (float)k / (float)N, &sn, &cs);
         W[k] = make_float2(cs, sn);
-        if (DEMOD) {
-            // tmp = -2 pi l_min / N * k in fp32 as the reference computes it, then exp(j tmp)
-            float tmp = -2.0f * 3.14159265358979323846f * (float)l_min / (float)N * (float)k;
-            PC[k] = make_float2(cosf(tmp), sinf(tmp));
-        }
     }
     const float scale = 1.0f / sqrtf((float)N);     // modulator: ifft = conj(fft(conj))/N, then * sqrt(N)
     for (long long job = blockIdx.x; job < rows * nsym; job += gridDim.x) {
@@ -117,8 +113,12 @@ __global__ void ofdm_fft_kernel(const float2* __restrict__ x, float2* __restrict
             float2* dst = out + job * N;
             for (int k = tid; k < N; k += T) {
                 int ks = shift ? (k + N / 2) % N : k;   // fftshift: out[k'] with k' = (k + floor(N/2)) mod N takes bin k
-                float2 v = cmul(cscale(res[k], scale), PC[k]);
-                dst[ks] = v;
+                // tmp = -2 pi l_min / N * k in fp32 as the reference computes it, then exp(j tmp). The complex product
+                // is spelled out (a.y * pc rounded, a.x * pc fused) so that its rounding does not depend on how the
+                // compiler contracts cmul.
+                const float tmp = -2.0f * 3.14159265358979323846f * (float)l_min / (float)N * (float)k;
+                const float2 a = cscale(res[k], scale), pc = make_float2(cosf(tmp), sinf(tmp));
+                dst[ks] = make_float2(fmaf(a.x, pc.x, -__fmul_rn(a.y, pc.y)), fmaf(a.x, pc.y, __fmul_rn(a.y, pc.x)));
             }
         } else {
             const int c = cp[l];
@@ -807,7 +807,10 @@ struct LmmseScratch {
     __device__ __forceinline__ LmmseScratch(float2* smem, int T, int t, int M, int K)
         : S{smem, T, t}, H{smem + (size_t)M * M * T, T, t}, Y{smem + (size_t)(M * M + M * K) * T, T, t},
           A{smem + (size_t)(M * M + M * K + M) * T, T, t}, G{smem + (size_t)(M * M + M * K + M + K * K) * T, T, t} {}
-    static size_t elems(int M, int K) { return (size_t)(M * M + M * K + M + K * K + K * M); }   // per thread
+    static size_t elems(int M, int K) {                                                     // per thread
+        const size_t m = (size_t)M, k = (size_t)K;
+        return m * m + m * k + m + k * k + k * m;
+    }
 };
 
 // in: S (M x M, row-major, lower triangle read), H (M x K), y (M). out: xh[K], ne[K].
@@ -1155,7 +1158,8 @@ template <int DEMOD>
 int ofdm_fft(const char* name, const float* d_x, float* d_out, int64_t rows, int32_t nsym, int32_t n, const int32_t* d_cp,
              const int32_t* d_off, int32_t len, int32_t l_min, int32_t shift, cudaStream_t stream) {
     if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_x && d_out && d_cp && d_off && rows >= 0 && nsym > 0 && n > 0 && n <= 8192, "%s: bad arguments", name);
+    SB_CHECK_ARG(d_x && d_out && d_cp && d_off && rows >= 0 && nsym > 0 && n > 0 && n <= 8192,
+                 "%s: bad arguments (need 1 <= fft_size <= 8192, num_symbols >= 1)", name);
     const float2* x = (const float2*)d_x;
     float2* out = (float2*)d_out;
     int rc = SB_OK;
@@ -1167,7 +1171,7 @@ int ofdm_fft(const char* name, const float* d_x, float* d_out, int64_t rows, int
         FftPlan plan;
         SB_CHECK_ARG(make_plan(n, &plan) == 0, "%s: fft_size has too many factors", name);
         const int threads = std::min(256, std::max(32, (n / 2 + 31) / 32 * 32));
-        const size_t smem = sizeof(float2) * (DEMOD ? 4 : 3) * (size_t)n;
+        const size_t smem = sizeof(float2) * 3 * (size_t)n;
         int dev = 0, optin = 0;
         SB_CUDA(cudaGetDevice(&dev));
         SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
@@ -1370,11 +1374,15 @@ extern "C" int sb_pusch_ls_combine(float* d_h, float* d_err_var, int64_t rows, i
     return SB_OK;
 }
 
-// Threads per CTA of a thread-per-vector scratch kernel: at most 128, a multiple of 32, per_thread bytes of shared memory
-// each and at most cap bytes in all; 0 if not even one warp fits.
+// Threads per CTA of a thread-per-vector scratch kernel: per_thread bytes of shared memory each and at most cap bytes in
+// all. At most 128 and a multiple of 32 when a warp fits; otherwise the largest power of two that fits (16 ... 1), so
+// large matrices still run, at low occupancy. 0 if not even one thread fits.
 static int scratch_threads(size_t per_thread, size_t cap, size_t* smem) {
-    int t = (int)std::min<size_t>(128, cap / per_thread) / 32 * 32;
-    if (t < 32) return 0;
+    const int fit = (int)std::min<size_t>(128, cap / per_thread);
+    int t = fit / 32 * 32;
+    if (t == 0)
+        for (t = 16; t > fit; t /= 2) {}
+    if (t == 0) return 0;
     *smem = per_thread * t;
     return t;
 }
@@ -1386,8 +1394,13 @@ extern "C" int sb_lmmse_equalize(const float* d_y, const float* d_h, const float
     SB_CHECK_ARG(d_y && d_h && d_s && d_x_hat && d_no_eff && num >= 0 && M >= 1 && K >= 1 && K <= 16 && K <= M,
                  "sb_lmmse_equalize: bad arguments (need 1 <= K <= 16, K <= M)");
     size_t smem = 0;
-    int threads = scratch_threads(sizeof(float2) * LmmseScratch::elems(M, K), kLmmseSmemCap, &smem);
-    if (!threads) { sb_set_error("sb_lmmse_equalize: M = %d too large for the per-thread shared-memory path", M); return SB_EUNSUPPORTED; }
+    const size_t per_thread = sizeof(float2) * LmmseScratch::elems(M, K);
+    int threads = scratch_threads(per_thread, kLmmseSmemCap, &smem);
+    if (!threads) {
+        sb_set_error("sb_lmmse_equalize: M = %d, K = %d needs %zu bytes of shared-memory scratch per vector, the limit is %zu",
+                     M, K, per_thread, kLmmseSmemCap);
+        return SB_EUNSUPPORTED;
+    }
     SB_CUDA(cudaFuncSetAttribute(lmmse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     lmmse_kernel<<<sb_grid(num, threads, 16), threads, smem, (cudaStream_t)stream>>>(
         (const float2*)d_y, (const float2*)d_h, (const float2*)d_s, (float2*)d_x_hat, d_no_eff, num, M, K);
@@ -1407,8 +1420,13 @@ extern "C" int sb_mimo_linalg(int32_t mode, const float* d_y, const float* d_h, 
     SB_CUDA(cudaGetDevice(&dev));
     SB_CUDA(cudaDeviceGetAttribute(&optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     size_t smem = 0;
-    int threads = scratch_threads(sizeof(float2) * ((size_t)M * M + 2 * (size_t)M * K), (size_t)optin, &smem);
-    if (!threads) { sb_set_error("sb_mimo_linalg: M = %d too large for the per-thread shared-memory path", M); return SB_EUNSUPPORTED; }
+    const size_t per_thread = sizeof(float2) * ((size_t)M * M + 2 * (size_t)M * K);
+    int threads = scratch_threads(per_thread, (size_t)optin, &smem);
+    if (!threads) {
+        sb_set_error("sb_mimo_linalg: M = %d, K = %d needs %zu bytes of shared-memory scratch per matrix, the device offers %d",
+                     M, K, per_thread, optin);
+        return SB_EUNSUPPORTED;
+    }
     SB_CUDA(cudaFuncSetAttribute(mimo_linalg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     mimo_linalg_kernel<<<sb_grid(num, threads, 16), threads, smem, (cudaStream_t)stream>>>(
         mode, (const float2*)d_y, (const float2*)d_h, (const float2*)d_s, (float2*)d_out0, d_out1, num, M, K);
@@ -1447,8 +1465,13 @@ extern "C" int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float
         return SB_OK;
     }
     size_t smem = 0;
-    int threads = scratch_threads(sizeof(float2) * LmmseScratch::elems(num_rx_ant, streams_per_rx), kLmmseSmemCap, &smem);
-    if (!threads) { sb_set_error("sb_ofdm_lmmse: %d receive antennas too many for the per-thread shared-memory path", num_rx_ant); return SB_EUNSUPPORTED; }
+    const size_t per_thread = sizeof(float2) * LmmseScratch::elems(num_rx_ant, streams_per_rx);
+    int threads = scratch_threads(per_thread, kLmmseSmemCap, &smem);
+    if (!threads) {
+        sb_set_error("sb_ofdm_lmmse: %d receive antennas, %d streams need %zu bytes of shared-memory scratch per resource "
+                     "element, the limit is %zu", num_rx_ant, streams_per_rx, per_thread, kLmmseSmemCap);
+        return SB_EUNSUPPORTED;
+    }
     SB_CUDA(cudaFuncSetAttribute(ofdm_lmmse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     ofdm_lmmse_kernel<<<sb_grid(total_re, threads, 16), threads, smem, (cudaStream_t)stream>>>(p);
     SB_LAUNCH_CHECK();
