@@ -60,7 +60,8 @@ struct QcParams {
 // ---- check-node updates on the edges pm[0], pm[Z], pm[2Z], ... of one check ------------------------------------
 // boxplus-phi (decoding.py:1126-1166), two independent edges per step (sb_math2.cuh).
 // Exact strength reductions (outputs are bit-identical, only instructions are saved), all decided warp-uniformly:
-//   (1) |x| >= 16.635532 (the phi clipping bound, :1113)  =>  phi(|x|) == 0 exactly              [saturated inputs]
+//   (1) |x| >= 16.635532 (the phi clipping bound, :1113)  =>  phi(|x|) == +0 exactly              [saturated inputs]
+//       The voting variant uses the wider exact bound |x| >= 14.7117348 (SB_PHI_ZERO).
 //   (2) p_e == 0  =>  P - p_e == P exactly  =>  phi(P - p_e) == phi(P), evaluated once per check
 //   (3) P - p_e <= 8.5e-8 (lower clipping bound)  =>  phi(P - p_e) == phi(8.5e-8) == phi_max
 // Once a codeword has converged most VN->CN messages except those of degree-1 VNs sit at +-llr_max >= 16.64, and a
@@ -73,43 +74,18 @@ struct QcParams {
 #define SB_PRAGMA_(x) _Pragma(#x)
 #define SB_UNROLL(n) SB_PRAGMA_(unroll n)
 #define SB_PHI_HI 16.635532f
-#define SB_PHI_LO 8.5e-8f
-// SC = false: plain evaluation; one vote per check on its first edge pair probes for saturation and raises *sat_flag,
-// which makes the CTA use the SC = true variant (one vote per row for a saturated row, else votes on every pair) from
-// the next iteration on.
-// Out of line on purpose: the five degree classes then share ONE copy of each variant's loops (the kernel is bound by
-// instruction fetch as much as by issue: 12.35 -> 11.85 ms per 4096 codewords at 2 dB; making phi itself a call costs more
-// than it saves, 12.8 ms).
-template <bool SC, class LT>
-__device__ __noinline__ void cn_phi_qc(float* pm, int Z, int deg, float clip, float phi_max, int* sat_flag,
-                                       const LT& lt) {
+// Least fp32 x above which phi(x) is +0 for every x in this arithmetic: e^x + 1 and e^x - 1 round to the same float
+// and the two logs cancel. Below it phi is not monotone (x = 14.7117338 gives 2^-20). Checked over every fp32 value up
+// to 16.635532 against the oracle and on the device by tests/test_ldpc_phi_union_gpu.py.
+#define SB_PHI_ZERO 14.7117348f
+// Plain variant: every edge is evaluated. One vote per check on its first edge pair probes for saturation and raises
+// *sat_flag, which makes the CTA use the voting variant cn_phi_qc_sc from the next iteration on.
+// Out of line on purpose (both variants): the five degree classes then share ONE copy of each variant's loops (the
+// kernel is bound by instruction fetch as much as by issue: 12.35 -> 11.85 ms per 4096 codewords at 2 dB; making phi
+// itself a call costs more than it saves, 12.8 ms).
+template <class LT>
+__device__ __noinline__ void cn_phi_qc(float* pm, int Z, int deg, float clip, int* sat_flag, const LT& lt) {
     const unsigned am = __activemask();                   // lanes of this warp working on the same block row
-    if (SC) {
-        // Saturated row (one vote per row): every edge but the last has |x| >= 16.635532. Their phi are +0 (1), so
-        // P = p_last exactly; each of them gets phi(P) whichever of (2), (3) or a full evaluation the general code below
-        // would take, and the last edge gets phi(P - p_last) = phi(+0) = phi_max (3). Two phi per row, no per-pair votes
-        // and no stores between the two passes.
-        unsigned par = 0;
-        bool sat = true;
-        for (int k = 0; k + 1 < deg; ++k) {
-            const unsigned b = __float_as_uint(pm[k * Z]);
-            par ^= b;
-            sat = sat && fabsf(__uint_as_float(b)) >= SB_PHI_HI;
-        }
-        if (__all_sync(am, sat)) {
-            float* ql = pm + (deg - 1) * Z;
-            const unsigned bl = __float_as_uint(*ql);
-            par = (par ^ bl) & 0x80000000u;
-            const float pl = sb_phif_s(__uint_as_float(bl & 0x7fffffffu), lt);
-            const unsigned y = __float_as_uint(fminf(sb_phif_s(pl, lt), clip));
-            for (int k = 0; k + 1 < deg; ++k) {
-                float* q = pm + k * Z;
-                *q = __uint_as_float(y | ((__float_as_uint(*q) ^ par) & 0x80000000u));
-            }
-            *ql = __uint_as_float(__float_as_uint(fminf(phi_max, clip)) | ((bl ^ par) & 0x80000000u));
-            return;
-        }
-    }
     float P = 0.f;
     unsigned par = 0;
     int l = 0;
@@ -120,13 +96,8 @@ SB_UNROLL(SB_PHI_UNROLL)
         unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
         par ^= b0 ^ b1;
         float a0 = __uint_as_float(b0 & 0x7fffffffu), a1 = __uint_as_float(b1 & 0x7fffffffu);
-        float2 p = make_float2(0.f, 0.f);
-        if (SC) {
-            if (!__all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) p = sb_phif2(make_float2(a0, a1), lt);   // (1)
-        } else {
-            p = sb_phif2(make_float2(a0, a1), lt);
-            if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;   // probe (benign race)
-        }
+        float2 p = sb_phif2(make_float2(a0, a1), lt);
+        if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;   // probe (benign race)
         P = __fadd_rn(P, p.x);                            // :1150 sequential sum, ascending VN
         P = __fadd_rn(P, p.y);
         *q0 = __uint_as_float(__float_as_uint(p.x) | (b0 & 0x80000000u));   // phi >= 0: sign bit carries sign(x)
@@ -136,59 +107,121 @@ SB_UNROLL(SB_PHI_UNROLL)
         float* q0 = pm + l * Z;
         unsigned b0 = __float_as_uint(*q0);
         par ^= b0;
-        float a0 = __uint_as_float(b0 & 0x7fffffffu);
-        float p = 0.f;
-        if (!SC || !__all_sync(am, a0 >= SB_PHI_HI)) p = sb_phif_s(a0, lt);
+        float p = sb_phif_s(__uint_as_float(b0 & 0x7fffffffu), lt);
         P = __fadd_rn(P, p);
         *q0 = __uint_as_float(__float_as_uint(p) | (b0 & 0x80000000u));
     }
     par &= 0x80000000u;
-    float yP = 0.f;                                       // phi(P), evaluated lazily (2)
-    bool have_yP = false;
     l = 0;
 SB_UNROLL(SB_PHI_UNROLL)
     for (; l + 1 < deg; l += 2) {
         float* q0 = pm + l * Z;
         float* q1 = q0 + Z;
         unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
-        float2 y;
-        if (SC && __all_sync(am, ((b0 | b1) & 0x7fffffffu) == 0u)) {                                 // (2)
-            if (!have_yP) { yP = sb_phif_s(P, lt); have_yP = true; }
-            y = make_float2(yP, yP);
-        } else {
-            float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
-                                  make_float2(P, P));     // (-p) + P  (:1155)
-            if (SC && __all_sync(am, m.x <= SB_PHI_LO && m.y <= SB_PHI_LO)) y = make_float2(phi_max, phi_max);   // (3)
-            else y = sb_phif2(m, lt);
-        }
+        float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
+                         make_float2(P, P));              // (-p) + P  (:1155)
+        float2 y = sb_phif2(m, lt);
         *q0 = __uint_as_float(__float_as_uint(fminf(y.x, clip)) | ((b0 ^ par) & 0x80000000u));   // :1161-1163
         *q1 = __uint_as_float(__float_as_uint(fminf(y.y, clip)) | ((b1 ^ par) & 0x80000000u));
     }
     if (l < deg) {
         float* q0 = pm + l * Z;
         unsigned b0 = __float_as_uint(*q0);
-        float y;
-        if (SC && __all_sync(am, (b0 & 0x7fffffffu) == 0u)) {
-            if (!have_yP) { yP = sb_phif_s(P, lt); have_yP = true; }
-            y = yP;
-        } else {
-            float m = __fadd_rn(__uint_as_float(b0 | 0x80000000u), P);
-            if (SC && __all_sync(am, m <= SB_PHI_LO)) y = phi_max;
-            else y = sb_phif_s(m, lt);
-        }
+        float y = sb_phif_s(__fadd_rn(__uint_as_float(b0 | 0x80000000u), P), lt);
         *q0 = __uint_as_float(__float_as_uint(fminf(y, clip)) | ((b0 ^ par) & 0x80000000u));
     }
 }
 
-// Exact-degree variant (deg == D, D <= SB_PHI_REG_MAXD): phi(|x|) of the whole row stays in registers between the two
-// passes (no STS in pass 1, no LDS / address arithmetic in pass 2), both passes fully unrolled. Same operation sequence
-// per element as cn_phi_qc, hence bit-identical. Used for deg <= SB_PHI_REG_MAXD in the plain variant only: skipped
-// straight-line code still has to be fetched, a skipped loop body does not, and the kernel is instruction-cache bound.
+// Voting variant (deg <= 32), for the iterations after the probe saw a saturated pair. One read pass builds the row's
+// union mask U: bit l is set if |x_l| < SB_PHI_ZERO in any lane of the warp. U is warp-uniform, and only its k positions
+// are evaluated:
+//   * U holds no edge but the last (the common row once a codeword has converged): every other edge has phi = +0 (1),
+//     so P = p_last exactly; those edges get phi(P) and the last edge phi(P - p_last) = phi(+0) = phi_max (3). Two phi
+//     per row.
+//   * otherwise, walking U in ascending order two at a time: phi(|x_l|) for l in U, summed into P in that order. A
+//     position outside U has phi = +0 in every lane (1), and P + (+0) == P, so P is bit-identical to the sum over all
+//     edges in ascending VN order. Then phi(P - p_l) for l in U, each lane on its own values: where (2) or (3) holds
+//     the evaluation itself gives what the rule gives (-0 + P == P; the clamp of phi maps P - p_l <= 8.5e-8 to
+//     phi_max). Every position outside U gets phi(P - 0) = phi(P), evaluated once. 2k + 1 phi per row.
+template <class LT>
+__device__ __noinline__ void cn_phi_qc_sc(float* pm, int Z, int deg, float clip, float phi_max, const LT& lt) {
+    unsigned par = 0, own = 0;
+    for (int l = 0; l < deg; ++l) {
+        const unsigned b = __float_as_uint(pm[l * Z]);
+        par ^= b;
+        own |= (fabsf(__uint_as_float(b)) < SB_PHI_ZERO ? 1u : 0u) << l;
+    }
+    par &= 0x80000000u;
+    const unsigned U = __reduce_or_sync(__activemask(), own);
+    if (!(U & ((1u << (deg - 1)) - 1u))) {
+        float* ql = pm + (deg - 1) * Z;
+        const unsigned bl = __float_as_uint(*ql);
+        const float pl = sb_phif_s(__uint_as_float(bl & 0x7fffffffu), lt);
+        const unsigned y = __float_as_uint(fminf(sb_phif_s(pl, lt), clip));
+        for (int l = 0; l + 1 < deg; ++l) {
+            float* q = pm + l * Z;
+            *q = __uint_as_float(y | ((__float_as_uint(*q) ^ par) & 0x80000000u));
+        }
+        *ql = __uint_as_float(__float_as_uint(fminf(phi_max, clip)) | ((bl ^ par) & 0x80000000u));
+        return;
+    }
+    float P = 0.f;
+    unsigned u = U;
+    for (; u & (u - 1); u &= u - 1) {                     // two or more positions left: the lowest two
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        u &= u - 1;
+        float* q1 = pm + (__ffs(u) - 1) * Z;
+        const unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
+        const float2 p = sb_phif2(make_float2(__uint_as_float(b0 & 0x7fffffffu), __uint_as_float(b1 & 0x7fffffffu)), lt);
+        P = __fadd_rn(P, p.x);                            // :1150 sequential sum, ascending VN
+        P = __fadd_rn(P, p.y);
+        *q0 = __uint_as_float(__float_as_uint(p.x) | (b0 & 0x80000000u));
+        *q1 = __uint_as_float(__float_as_uint(p.y) | (b1 & 0x80000000u));
+    }
+    if (u) {
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        const unsigned b0 = __float_as_uint(*q0);
+        const float p = sb_phif_s(__uint_as_float(b0 & 0x7fffffffu), lt);
+        P = __fadd_rn(P, p);
+        *q0 = __uint_as_float(__float_as_uint(p) | (b0 & 0x80000000u));
+    }
+    const unsigned rest = ~U & (0xffffffffu >> (32 - deg));
+    if (rest) {
+        const unsigned y = __float_as_uint(fminf(sb_phif_s(P, lt), clip));
+        for (unsigned r = rest; r; r &= r - 1) {
+            float* q = pm + (__ffs(r) - 1) * Z;
+            *q = __uint_as_float(y | ((__float_as_uint(*q) ^ par) & 0x80000000u));
+        }
+    }
+    for (u = U; u & (u - 1); u &= u - 1) {
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        u &= u - 1;
+        float* q1 = pm + (__ffs(u) - 1) * Z;
+        const unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
+        const float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
+                               make_float2(P, P));        // (-p) + P  (:1155)
+        const float2 y = sb_phif2(m, lt);
+        *q0 = __uint_as_float(__float_as_uint(fminf(y.x, clip)) | ((b0 ^ par) & 0x80000000u));   // :1161-1163
+        *q1 = __uint_as_float(__float_as_uint(fminf(y.y, clip)) | ((b1 ^ par) & 0x80000000u));
+    }
+    if (u) {
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        const unsigned b0 = __float_as_uint(*q0);
+        const float y = sb_phif_s(__fadd_rn(__uint_as_float(b0 | 0x80000000u), P), lt);
+        *q0 = __uint_as_float(__float_as_uint(fminf(y, clip)) | ((b0 ^ par) & 0x80000000u));
+    }
+}
+
+// Exact-degree variant of the plain cn_phi_qc (deg == D, D <= SB_PHI_REG_MAXD): phi(|x|) of the whole row stays in
+// registers between the two passes (no STS in pass 1, no LDS / address arithmetic in pass 2), both passes fully
+// unrolled. Same operation sequence per element as cn_phi_qc, hence bit-identical. The voting variant has no such
+// code: skipped straight-line code still has to be fetched, a skipped loop body does not, and the kernel is
+// instruction-cache bound.
 #ifndef SB_PHI_REG_MAXD
 #define SB_PHI_REG_MAXD 8
 #endif
-template <int D, bool SC, class LT>
-__device__ __forceinline__ void cn_phi_qc_reg(float* pm, int Z, float clip, float phi_max, int* sat_flag, const LT& lt) {
+template <int D, class LT>
+__device__ __forceinline__ void cn_phi_qc_reg(float* pm, int Z, float clip, int* sat_flag, const LT& lt) {
     const unsigned am = __activemask();
     unsigned w[D];                                        // phi(|x|) bits | sign(x)
     float P = 0.f;
@@ -198,13 +231,8 @@ __device__ __forceinline__ void cn_phi_qc_reg(float* pm, int Z, float clip, floa
         unsigned b0 = __float_as_uint(pm[l * Z]), b1 = __float_as_uint(pm[(l + 1) * Z]);
         par ^= b0 ^ b1;
         float a0 = __uint_as_float(b0 & 0x7fffffffu), a1 = __uint_as_float(b1 & 0x7fffffffu);
-        float2 q = make_float2(0.f, 0.f);
-        if (SC) {
-            if (!__all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) q = sb_phif2(make_float2(a0, a1), lt);
-        } else {
-            q = sb_phif2(make_float2(a0, a1), lt);
-            if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;
-        }
+        float2 q = sb_phif2(make_float2(a0, a1), lt);
+        if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;
         P = __fadd_rn(P, q.x);
         P = __fadd_rn(P, q.y);
         w[l] = __float_as_uint(q.x) | (b0 & 0x80000000u);
@@ -213,61 +241,42 @@ __device__ __forceinline__ void cn_phi_qc_reg(float* pm, int Z, float clip, floa
     if (D & 1) {
         unsigned b0 = __float_as_uint(pm[(D - 1) * Z]);
         par ^= b0;
-        float a0 = __uint_as_float(b0 & 0x7fffffffu);
-        float q = 0.f;
-        if (!SC || !__all_sync(am, a0 >= SB_PHI_HI)) q = sb_phif_s(a0, lt);
+        float q = sb_phif_s(__uint_as_float(b0 & 0x7fffffffu), lt);
         P = __fadd_rn(P, q);
         w[D - 1] = __float_as_uint(q) | (b0 & 0x80000000u);
     }
     par &= 0x80000000u;
-    float yP = 0.f;
-    bool have_yP = false;
 #pragma unroll
     for (int l = 0; l + 1 < D; l += 2) {
         const unsigned b0 = w[l], b1 = w[l + 1];
-        float2 y;
-        if (SC && __all_sync(am, ((b0 | b1) & 0x7fffffffu) == 0u)) {
-            if (!have_yP) { yP = sb_phif_s(P, lt); have_yP = true; }
-            y = make_float2(yP, yP);
-        } else {
-            float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
-                                  make_float2(P, P));
-            if (SC && __all_sync(am, m.x <= SB_PHI_LO && m.y <= SB_PHI_LO)) y = make_float2(phi_max, phi_max);
-            else y = sb_phif2(m, lt);
-        }
+        float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
+                         make_float2(P, P));
+        float2 y = sb_phif2(m, lt);
         pm[l * Z] = __uint_as_float(__float_as_uint(fminf(y.x, clip)) | ((b0 ^ par) & 0x80000000u));
         pm[(l + 1) * Z] = __uint_as_float(__float_as_uint(fminf(y.y, clip)) | ((b1 ^ par) & 0x80000000u));
     }
     if (D & 1) {
         const unsigned b0 = w[D - 1];
-        float y;
-        if (SC && __all_sync(am, (b0 & 0x7fffffffu) == 0u)) {
-            if (!have_yP) { yP = sb_phif_s(P, lt); have_yP = true; }
-            y = yP;
-        } else {
-            float m = __fadd_rn(__uint_as_float(b0 | 0x80000000u), P);
-            if (SC && __all_sync(am, m <= SB_PHI_LO)) y = phi_max;
-            else y = sb_phif_s(m, lt);
-        }
+        float y = sb_phif_s(__fadd_rn(__uint_as_float(b0 | 0x80000000u), P), lt);
         pm[(D - 1) * Z] = __uint_as_float(__float_as_uint(fminf(y, clip)) | ((b0 ^ par) & 0x80000000u));
     }
 }
 
-template <bool SC, int CLS, class LT>
-__device__ __forceinline__ void cn_phi_dispatch(float* pm, int Z, int deg, float clip, float phi_max, int* sat_flag,
-                                                const LT& lt) {
-#ifndef SB_PHI_REG_SC
-#define SB_PHI_REG_SC 0                                   // 0: register rows only in the plain (non-voting) variant
-#endif
+// The voting variant takes rows of up to 32 edges (one mask bit per edge); heavier rows (class 0 only, none in the 5G
+// base graphs) run the plain variant, whose probe then re-raises the already raised flag.
+template <int CLS, class LT>
+__device__ __forceinline__ void cn_phi_dispatch(float* pm, int Z, int deg, float clip, float phi_max, bool sc,
+                                                int* sat_flag, const LT& lt) {
+    if (sc && (CLS > 0 || deg <= 32)) { cn_phi_qc_sc<LT>(pm, Z, deg, clip, phi_max, lt); return; }
 #if SB_PHI_REG_MAXD > 0
-#define SB_PHI_CASE(D) if ((SB_PHI_REG_SC || !SC) && D <= SB_PHI_REG_MAXD && deg == D) { cn_phi_qc_reg<D, SC, LT>(pm, Z, clip, phi_max, sat_flag, lt); return; }
+#define SB_PHI_CASE(D) if (D <= SB_PHI_REG_MAXD && deg == D) { cn_phi_qc_reg<D, LT>(pm, Z, clip, sat_flag, lt); return; }
     if (CLS == 4) { SB_PHI_CASE(3) SB_PHI_CASE(4) }
     if (CLS == 3) { SB_PHI_CASE(5) SB_PHI_CASE(6) SB_PHI_CASE(7) SB_PHI_CASE(8) }
     if (CLS == 2) { SB_PHI_CASE(9) SB_PHI_CASE(10) }
     if (CLS == 1) { SB_PHI_CASE(19) }
 #undef SB_PHI_CASE
 #endif
-    cn_phi_qc<SC, LT>(pm, Z, deg, clip, phi_max, sat_flag, lt);
+    cn_phi_qc<LT>(pm, Z, deg, clip, sat_flag, lt);
 }
 
 __device__ __forceinline__ void cn_tanh_qc(float* pm, int Z, int deg, float clip) {
@@ -351,8 +360,7 @@ template <int RULE, int CLS, class LT>
 __device__ __forceinline__ void cn_qc(float* pm, int Z, int deg, float clip, float offset, float phi_max, bool sc,
                                       int* sat_flag, const LT& lt) {
     if (RULE == SB_CN_BOXPLUS_PHI) {
-        if (sc) cn_phi_dispatch<true, CLS, LT>(pm, Z, deg, clip, phi_max, sat_flag, lt);
-        else cn_phi_dispatch<false, CLS, LT>(pm, Z, deg, clip, phi_max, sat_flag, lt);
+        cn_phi_dispatch<CLS, LT>(pm, Z, deg, clip, phi_max, sc, sat_flag, lt);
     }
     else if (RULE == SB_CN_BOXPLUS) cn_tanh_qc(pm, Z, deg, clip);
     else {
