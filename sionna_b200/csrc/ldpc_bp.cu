@@ -104,10 +104,7 @@ __global__ void __launch_bounds__(1024, 1) ldpc_bp_kernel(const __grid_constant_
     for (int i = tid; i < p.Lc; i += T) s_cn_cnt[i] = p.cn_cnt[i];
     for (int i = tid; i <= p.Lv; i += T) s_vn_off[i] = p.vn_off[i];
     for (int i = tid; i < p.Lv; i += T) s_vn_cnt[i] = p.vn_cnt[i];
-    if (SMEM && p.use_tma && tid == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (SMEM && p.use_tma && tid == 0) mbar_init(bar);
     __syncthreads();
 
     const SlotT* __restrict__ vn_slot = reinterpret_cast<const SlotT*>(p.vn_slot);
@@ -116,29 +113,9 @@ __global__ void __launch_bounds__(1024, 1) ldpc_bp_kernel(const __grid_constant_
     const int n_cn_items = p.sched ? p.n_active : C;
 
     for (long long b = blockIdx.x; b < p.B; b += gridDim.x) {
-        // ---- channel LLRs: clip, negate (decoding.py:552-565), rate recovery (:1444-1475) ---------
-        const float* row = p.llr + (size_t)b * p.n_in;
-        if (SMEM && p.use_tma) {
-            float* stage = v2c;                          // message array is free until the init below
-            if (tid == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                mbar_expect_tx(bar, (uint32_t)p.n_in * 4u);
-                tma_bulk_g2s(stage, row, (uint32_t)p.n_in * 4u, bar);
-            }
-            mbar_wait(bar, tma_phase);
-            tma_phase ^= 1u;
-            for (int r = tid; r < N; r += T) {
-                int ii = p.in_idx[r];
-                float l = ii >= 0 ? stage[ii] : (ii == -1 ? 0.f : -clip);
-                llr_s[r] = __fmul_rn(clipf(l, clip), -1.f);
-            }
-        } else {
-            for (int r = tid; r < N; r += T) {
-                int ii = p.in_idx[r];
-                float l = ii >= 0 ? __ldg(row + ii) : (ii == -1 ? 0.f : -clip);
-                llr_s[r] = __fmul_rn(clipf(l, clip), -1.f);
-            }
-        }
+        // ---- channel LLRs by VN rank, staged in the message array -----------------------------------
+        load_channel_llr(llr_s, p.llr + (size_t)b * p.n_in, p.in_idx, N, p.n_in, clip, SMEM && p.use_tma, v2c, bar,
+                         tma_phase, tid, T);
         __syncthreads();
         // ---- initial messages: v2c = llr of the edge's VN (:571) or the caller's state (:573); c2v = 0
         if (p.state_in) {
@@ -156,13 +133,10 @@ __global__ void __launch_bounds__(1024, 1) ldpc_bp_kernel(const __grid_constant_
             for (int e = tid; e < E; e += T) c2v[e] = 0.f;
         __syncthreads();
 
-        if (p.num_iter == 0) {                           // x_hat = llr_ch (:603-608)
-            for (int r = tid; r < N; r += T) {
-                int o = p.out_pos[r];
-                if (o >= 0) {
-                    float x = llr_s[r];
-                    p.out[(size_t)b * p.n_out + o] = p.hard_out ? (0.f >= x ? 1.f : 0.f) : __fmul_rn(x, -1.f);
-                }
+        if (p.num_iter == 0) {                           // x_hat = llr_ch (decoding.py:603-608)
+            for (int v = tid; v < N; v += T) {
+                int o = p.out_pos[v];
+                if (o >= 0) p.out[(size_t)b * p.n_out + o] = decoder_out(llr_s[v], p.hard_out);
             }
         }
 
@@ -204,18 +178,15 @@ __global__ void __launch_bounds__(1024, 1) ldpc_bp_kernel(const __grid_constant_
                         }
                         if (final_pass) {
                             int o = p.out_pos[r];
-                            if (o >= 0)
-                                p.out[(size_t)b * p.n_out + o] =
-                                    p.hard_out ? (0.f >= x_tot ? 1.f : 0.f) : __fmul_rn(x_tot, -1.f);        // :622-626
+                            if (o >= 0) p.out[(size_t)b * p.n_out + o] = decoder_out(x_tot, p.hard_out);
                         }
                     }
                 }
                 __syncthreads();
             }
         }
-        if (p.state_out) {                               // :636
-            float* st = p.state_out + (size_t)b * E;
-            for (int e = tid; e < E; e += T) st[e] = __fmul_rn(v2c[p.slot_of_edge[e]], -1.f);
+        if (p.state_out) {
+            store_state(p.state_out + (size_t)b * E, v2c, p.slot_of_edge, E, tid, T);
             __syncthreads();
         }
     }
@@ -377,32 +348,24 @@ extern "C" void sb_ldpc_graph_destroy(sb_ldpc_graph* g) {
     delete g;
 }
 
-template <typename T>
-static int upload(T** dptr, const std::vector<T>& h) {
-    size_t n = h.size() ? h.size() : 1;
-    SB_CUDA(cudaMalloc((void**)dptr, n * sizeof(T)));
-    if (h.size()) SB_CUDA(cudaMemcpy(*dptr, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return SB_OK;
-}
-
 static int ensure_uploaded(sb_ldpc_graph* g) {
     int dev = 0;
     SB_CUDA(cudaGetDevice(&dev));
     if (g->uploaded && g->device == dev) return SB_OK;
     free_device(g);
     int rc;
-    if ((rc = upload(&g->d_cn_off, g->cn_off))) return rc;
-    if ((rc = upload(&g->d_cn_cnt, g->cn_cnt))) return rc;
-    if ((rc = upload(&g->d_vn_off, g->vn_off))) return rc;
-    if ((rc = upload(&g->d_vn_cnt, g->vn_cnt))) return rc;
-    if ((rc = upload(&g->d_in_idx, g->in_idx))) return rc;
-    if ((rc = upload(&g->d_out_pos, g->out_pos))) return rc;
-    if ((rc = upload(&g->d_slot_of_edge, g->slot_of_edge))) return rc;
-    if ((rc = upload(&g->d_sched, g->sched))) return rc;
-    if ((rc = upload(&g->d_vn_slot32, g->vn_slot))) return rc;
+    if ((rc = sb_upload(&g->d_cn_off, g->cn_off))) return rc;
+    if ((rc = sb_upload(&g->d_cn_cnt, g->cn_cnt))) return rc;
+    if ((rc = sb_upload(&g->d_vn_off, g->vn_off))) return rc;
+    if ((rc = sb_upload(&g->d_vn_cnt, g->vn_cnt))) return rc;
+    if ((rc = sb_upload(&g->d_in_idx, g->in_idx))) return rc;
+    if ((rc = sb_upload(&g->d_out_pos, g->out_pos))) return rc;
+    if ((rc = sb_upload(&g->d_slot_of_edge, g->slot_of_edge))) return rc;
+    if ((rc = sb_upload(&g->d_sched, g->sched))) return rc;
+    if ((rc = sb_upload(&g->d_vn_slot32, g->vn_slot))) return rc;
     std::vector<uint16_t> s16(g->vn_slot.size());
     for (size_t i = 0; i < s16.size(); ++i) s16[i] = (uint16_t)g->vn_slot[i];
-    if ((rc = upload(&g->d_vn_slot16, s16))) return rc;
+    if ((rc = sb_upload(&g->d_vn_slot16, s16))) return rc;
     SB_CUDA(cudaDeviceGetAttribute(&g->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     SB_CUDA(cudaDeviceGetAttribute(&g->num_sms, cudaDevAttrMultiProcessorCount, dev));
     g->uploaded = true;
@@ -442,19 +405,6 @@ static int pick_threads(const sb_ldpc_graph* g) {
     return best;
 }
 
-template <int RULE, bool SMEM>
-static int launch_bp(const sb_ldpc_graph* g, const BpParams& p, int threads, size_t smem, cudaStream_t stream) {
-    auto kern = ldpc_bp_kernel<RULE, SMEM>;
-    SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 0;
-    SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
-    if (occ < 1) { sb_set_error("sb_ldpc_decode: kernel does not fit (threads %d, smem %zu)", threads, smem); return SB_EUNSUPPORTED; }
-    long long grid = std::min<long long>(p.B, std::min<long long>((long long)g->num_sms * occ, kMaxGrid));
-    kern<<<(unsigned)grid, threads, smem, stream>>>(p);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
-}
-
 static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t batch, int32_t num_iter, int32_t cn_rule,
                             int32_t vn_rule, float offset, float llr_max, int32_t hard_out, const float* d_state_in,
                             float* d_state_out, float* d_out, void* d_ws, size_t ws_bytes, void* stream, int32_t early,
@@ -485,7 +435,6 @@ static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t
     SB_CHECK_ARG(cn_rule >= SB_CN_BOXPLUS_PHI && cn_rule <= SB_CN_IDENTITY, "sb_ldpc_decode: unknown cn_rule %d", cn_rule);
     SB_CHECK_ARG(vn_rule == SB_VN_SUM || vn_rule == SB_VN_IDENTITY, "sb_ldpc_decode: unknown vn_rule %d", vn_rule);
     SB_CHECK_ARG(llr_max >= 0.f, "sb_ldpc_decode: llr_max must be >= 0");
-    if (batch == 0) return SB_OK;
     auto* g = const_cast<sb_ldpc_graph*>(gc);
     int rc = ensure_uploaded(g);
     if (rc) return rc;
@@ -524,7 +473,8 @@ static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t
     cudaStream_t st = (cudaStream_t)stream;
 #define SB_BP_CASE(R)                                                             \
     case R:                                                                       \
-        return on_chip ? launch_bp<R, true>(g, p, threads, smem, st) : launch_bp<R, false>(g, p, threads, smem, st);
+        return sb_launch_decoder(on_chip ? ldpc_bp_kernel<R, true> : ldpc_bp_kernel<R, false>, p, g, threads, smem, \
+                                 kMaxGrid, st, "sb_ldpc_decode");
     switch (cn_rule) {
         SB_BP_CASE(SB_CN_BOXPLUS_PHI)
         SB_BP_CASE(SB_CN_BOXPLUS)

@@ -16,17 +16,47 @@
 // Summation orders (ascending VN inside a CN, ascending CN inside a VN) are those of ldpc_bp.cu, so both kernels
 // and the CPU oracle (math_mode 1, order "kernel") agree bit for bit.
 #include <algorithm>
+#include <climits>
+#include <iterator>
 #include <numeric>
 #include <vector>
 #include "sb_common.h"
 #include "sb_math.h"
 #include "sb_math2.cuh"
 #include "ldpc_graph.h"
+#include "ldpc_rules.cuh"
 
 namespace {
 
-constexpr int kRowClasses = 5;    // CN degree classes, heaviest first: >20 (loop), <=20, <=12, <=8, <=4
-constexpr int kColClasses = 11;   // VN classes, see col_class() on the host side
+// ---- degree classes, read by the host planner (sb_ldpc_graph_set_qc) and by the kernel ---------------------------
+// Rows and columns are processed class by class, heaviest first. Class k holds the degrees d with
+// kMax[k + 1] < d <= kMax[k]; its code keeps a row (column) of up to kMax[k] edges in registers. kLoop marks the
+// classes that take any larger degree and run loop code instead.
+constexpr int kLoop = INT_MAX;
+// CN classes: > 20 (loop), <= 20, <= 12, <= 8, <= 4
+constexpr int kRowMax[] = {kLoop, 20, 12, 8, 4};
+// VN classes: 0...6 by degree; 7...9 for columns with an edge into a partial (pruning-cut) block row, whose edges need
+// a per-entry limit; 10: degree-1 columns whose update is fused into the CN phase (the last edge of their row).
+constexpr int kColCut = 7, kColFused = 10;
+constexpr int kColMax[] = {kLoop, 32, 20, 12, 8, 4, 2, kLoop, 12, 4, 1};
+constexpr int kRowClasses = (int)std::size(kRowMax);
+constexpr int kColClasses = (int)std::size(kColMax);
+
+constexpr bool decreasing(const int* m, int lo, int hi) {
+    for (int k = lo + 1; k < hi; ++k)
+        if (m[k] >= m[k - 1]) return false;
+    return true;
+}
+static_assert(decreasing(kRowMax, 0, kRowClasses), "row class bounds must decrease");
+static_assert(decreasing(kColMax, 0, kColCut) && decreasing(kColMax, kColCut, kColFused), "column class bounds must decrease");
+static_assert(kColFused == kColClasses - 1 && kColMax[kColFused] == 1, "the fused class holds degree-1 columns only");
+
+// the lightest class of [lo, hi) whose bound holds degree d
+constexpr int degree_class(const int* m, int lo, int hi, int d) {
+    int k = hi - 1;
+    while (k > lo && d > m[k]) --k;
+    return k;
+}
 
 struct QcParams {
     int Z, n_rows, n_cols, nnz, N, E, E_alloc, n_in, n_out;
@@ -66,70 +96,87 @@ struct QcParams {
 //   (3) P - p_e <= 8.5e-8 (lower clipping bound)  =>  phi(P - p_e) == phi(8.5e-8) == phi_max
 // Once a codeword has converged most VN->CN messages except those of degree-1 VNs sit at +-llr_max >= 16.64, and a
 // check costs ~2 phi evaluations instead of 2*deg; the per-iteration cost therefore depends on the channel SNR.
-#ifndef SB_PHI_UNROLL
-// edge pairs per trip of the phi loops (an A/B variant is built with -DSB_PHI_UNROLL=n and selected with
-// SIONNA_B200_LIB)
-#define SB_PHI_UNROLL 2
-#endif
-#define SB_PRAGMA_(x) _Pragma(#x)
-#define SB_UNROLL(n) SB_PRAGMA_(unroll n)
 #define SB_PHI_HI 16.635532f
 // Least fp32 x above which phi(x) is +0 for every x in this arithmetic: e^x + 1 and e^x - 1 round to the same float
 // and the two logs cancel. Below it phi is not monotone (x = 14.7117338 gives 2^-20). Checked over every fp32 value up
 // to 16.635532 against the oracle and on the device by tests/test_ldpc_phi_union_gpu.py.
 #define SB_PHI_ZERO 14.7117348f
+// The two passes of the update, written once for every variant below: pass 1 on the edge words b = bits(x), pass 2 on
+// the staged words w = phi(|x|) | sign(x); one edge pair (two independent phi chains, sb_math2.cuh) or one edge.
+// Pass 1: phi(|x|), summed into P in ascending VN order (:1150); returns w (phi >= 0: the sign bit carries sign(x)).
+// `probe(|x0|, |x1|)` runs between the phi pair and the sum (the plain variant's saturation vote).
+template <class LT, class Probe>
+__device__ __forceinline__ uint2 phi_pass1_pair(unsigned b0, unsigned b1, float& P, const LT& lt, Probe probe) {
+    const float a0 = __uint_as_float(b0 & 0x7fffffffu), a1 = __uint_as_float(b1 & 0x7fffffffu);
+    const float2 p = sb_phif2(make_float2(a0, a1), lt);
+    probe(a0, a1);
+    P = __fadd_rn(P, p.x);
+    P = __fadd_rn(P, p.y);
+    return make_uint2(__float_as_uint(p.x) | (b0 & 0x80000000u), __float_as_uint(p.y) | (b1 & 0x80000000u));
+}
+template <class LT>
+__device__ __forceinline__ unsigned phi_pass1(unsigned b0, float& P, const LT& lt) {
+    const float p = sb_phif_s(__uint_as_float(b0 & 0x7fffffffu), lt);
+    P = __fadd_rn(P, p);
+    return __float_as_uint(p) | (b0 & 0x80000000u);
+}
+// Pass 2: phi((-p) + P) (:1155), clipped, sign(x) * prod(signs) (:1161-1163); par holds the product in bit 31.
+template <class LT>
+__device__ __forceinline__ uint2 phi_pass2_pair(unsigned w0, unsigned w1, float P, unsigned par, float clip, const LT& lt) {
+    const float2 m = fadd2(make_float2(__uint_as_float(w0 | 0x80000000u), __uint_as_float(w1 | 0x80000000u)),
+                           make_float2(P, P));
+    const float2 y = sb_phif2(m, lt);
+    return make_uint2(__float_as_uint(fminf(y.x, clip)) | ((w0 ^ par) & 0x80000000u),
+                      __float_as_uint(fminf(y.y, clip)) | ((w1 ^ par) & 0x80000000u));
+}
+template <class LT>
+__device__ __forceinline__ unsigned phi_pass2(unsigned w0, float P, unsigned par, float clip, const LT& lt) {
+    const float y = sb_phif_s(__fadd_rn(__uint_as_float(w0 | 0x80000000u), P), lt);
+    return __float_as_uint(fminf(y, clip)) | ((w0 ^ par) & 0x80000000u);
+}
+__device__ __forceinline__ unsigned ldw(const float* q) { return __float_as_uint(*q); }
+__device__ __forceinline__ void stw(float* q, unsigned w) { *q = __uint_as_float(w); }
+
 // Plain variant: every edge is evaluated. One vote per check on its first edge pair probes for saturation and raises
 // *sat_flag, which makes the CTA use the voting variant cn_phi_qc_sc from the next iteration on.
 // Out of line on purpose (both variants): the five degree classes then share ONE copy of each variant's loops (the
 // kernel is bound by instruction fetch as much as by issue: 12.35 -> 11.85 ms per 4096 codewords at 2 dB; making phi
-// itself a call costs more than it saves, 12.8 ms).
+// itself a call costs more than it saves, 12.8 ms). Two edge pairs per loop trip.
 template <class LT>
 __device__ __noinline__ void cn_phi_qc(float* pm, int Z, int deg, float clip, int* sat_flag, const LT& lt) {
     const unsigned am = __activemask();                   // lanes of this warp working on the same block row
     float P = 0.f;
     unsigned par = 0;
     int l = 0;
-SB_UNROLL(SB_PHI_UNROLL)
+#pragma unroll 2
     for (; l + 1 < deg; l += 2) {
         float* q0 = pm + l * Z;
         float* q1 = q0 + Z;
-        unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
+        const unsigned b0 = ldw(q0), b1 = ldw(q1);
         par ^= b0 ^ b1;
-        float a0 = __uint_as_float(b0 & 0x7fffffffu), a1 = __uint_as_float(b1 & 0x7fffffffu);
-        float2 p = sb_phif2(make_float2(a0, a1), lt);
-        if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;   // probe (benign race)
-        P = __fadd_rn(P, p.x);                            // :1150 sequential sum, ascending VN
-        P = __fadd_rn(P, p.y);
-        *q0 = __uint_as_float(__float_as_uint(p.x) | (b0 & 0x80000000u));   // phi >= 0: sign bit carries sign(x)
-        *q1 = __uint_as_float(__float_as_uint(p.y) | (b1 & 0x80000000u));
+        const uint2 w = phi_pass1_pair(b0, b1, P, lt, [&](float a0, float a1) {
+            if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;   // probe (benign race)
+        });
+        stw(q0, w.x);
+        stw(q1, w.y);
     }
     if (l < deg) {
         float* q0 = pm + l * Z;
-        unsigned b0 = __float_as_uint(*q0);
+        const unsigned b0 = ldw(q0);
         par ^= b0;
-        float p = sb_phif_s(__uint_as_float(b0 & 0x7fffffffu), lt);
-        P = __fadd_rn(P, p);
-        *q0 = __uint_as_float(__float_as_uint(p) | (b0 & 0x80000000u));
+        stw(q0, phi_pass1(b0, P, lt));
     }
     par &= 0x80000000u;
     l = 0;
-SB_UNROLL(SB_PHI_UNROLL)
+#pragma unroll 2
     for (; l + 1 < deg; l += 2) {
         float* q0 = pm + l * Z;
         float* q1 = q0 + Z;
-        unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
-        float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
-                         make_float2(P, P));              // (-p) + P  (:1155)
-        float2 y = sb_phif2(m, lt);
-        *q0 = __uint_as_float(__float_as_uint(fminf(y.x, clip)) | ((b0 ^ par) & 0x80000000u));   // :1161-1163
-        *q1 = __uint_as_float(__float_as_uint(fminf(y.y, clip)) | ((b1 ^ par) & 0x80000000u));
+        const uint2 y = phi_pass2_pair(ldw(q0), ldw(q1), P, par, clip, lt);
+        stw(q0, y.x);
+        stw(q1, y.y);
     }
-    if (l < deg) {
-        float* q0 = pm + l * Z;
-        unsigned b0 = __float_as_uint(*q0);
-        float y = sb_phif_s(__fadd_rn(__uint_as_float(b0 | 0x80000000u), P), lt);
-        *q0 = __uint_as_float(__float_as_uint(fminf(y, clip)) | ((b0 ^ par) & 0x80000000u));
-    }
+    if (l < deg) stw(pm + l * Z, phi_pass2(ldw(pm + l * Z), P, par, clip, lt));
 }
 
 // Voting variant (deg <= 32), for the iterations after the probe saw a saturated pair. One read pass builds the row's
@@ -171,19 +218,13 @@ __device__ __noinline__ void cn_phi_qc_sc(float* pm, int Z, int deg, float clip,
         float* q0 = pm + (__ffs(u) - 1) * Z;
         u &= u - 1;
         float* q1 = pm + (__ffs(u) - 1) * Z;
-        const unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
-        const float2 p = sb_phif2(make_float2(__uint_as_float(b0 & 0x7fffffffu), __uint_as_float(b1 & 0x7fffffffu)), lt);
-        P = __fadd_rn(P, p.x);                            // :1150 sequential sum, ascending VN
-        P = __fadd_rn(P, p.y);
-        *q0 = __uint_as_float(__float_as_uint(p.x) | (b0 & 0x80000000u));
-        *q1 = __uint_as_float(__float_as_uint(p.y) | (b1 & 0x80000000u));
+        const uint2 w = phi_pass1_pair(ldw(q0), ldw(q1), P, lt, [](float, float) {});
+        stw(q0, w.x);
+        stw(q1, w.y);
     }
     if (u) {
         float* q0 = pm + (__ffs(u) - 1) * Z;
-        const unsigned b0 = __float_as_uint(*q0);
-        const float p = sb_phif_s(__uint_as_float(b0 & 0x7fffffffu), lt);
-        P = __fadd_rn(P, p);
-        *q0 = __uint_as_float(__float_as_uint(p) | (b0 & 0x80000000u));
+        stw(q0, phi_pass1(ldw(q0), P, lt));
     }
     const unsigned rest = ~U & (0xffffffffu >> (32 - deg));
     if (rest) {
@@ -197,29 +238,21 @@ __device__ __noinline__ void cn_phi_qc_sc(float* pm, int Z, int deg, float clip,
         float* q0 = pm + (__ffs(u) - 1) * Z;
         u &= u - 1;
         float* q1 = pm + (__ffs(u) - 1) * Z;
-        const unsigned b0 = __float_as_uint(*q0), b1 = __float_as_uint(*q1);
-        const float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
-                               make_float2(P, P));        // (-p) + P  (:1155)
-        const float2 y = sb_phif2(m, lt);
-        *q0 = __uint_as_float(__float_as_uint(fminf(y.x, clip)) | ((b0 ^ par) & 0x80000000u));   // :1161-1163
-        *q1 = __uint_as_float(__float_as_uint(fminf(y.y, clip)) | ((b1 ^ par) & 0x80000000u));
+        const uint2 y = phi_pass2_pair(ldw(q0), ldw(q1), P, par, clip, lt);
+        stw(q0, y.x);
+        stw(q1, y.y);
     }
     if (u) {
         float* q0 = pm + (__ffs(u) - 1) * Z;
-        const unsigned b0 = __float_as_uint(*q0);
-        const float y = sb_phif_s(__fadd_rn(__uint_as_float(b0 | 0x80000000u), P), lt);
-        *q0 = __uint_as_float(__float_as_uint(fminf(y, clip)) | ((b0 ^ par) & 0x80000000u));
+        stw(q0, phi_pass2(ldw(q0), P, par, clip, lt));
     }
 }
 
-// Exact-degree variant of the plain cn_phi_qc (deg == D, D <= SB_PHI_REG_MAXD): phi(|x|) of the whole row stays in
-// registers between the two passes (no STS in pass 1, no LDS / address arithmetic in pass 2), both passes fully
-// unrolled. Same operation sequence per element as cn_phi_qc, hence bit-identical. The voting variant has no such
-// code: skipped straight-line code still has to be fetched, a skipped loop body does not, and the kernel is
+// Exact-degree variant of the plain cn_phi_qc (deg == D, the degrees 3...8 of the 5G base graphs): phi(|x|) of the
+// whole row stays in registers between the two passes (no STS in pass 1, no LDS / address arithmetic in pass 2), both
+// passes fully unrolled. Same operation sequence per element as cn_phi_qc, hence bit-identical. The voting variant has
+// no such code: skipped straight-line code still has to be fetched, a skipped loop body does not, and the kernel is
 // instruction-cache bound.
-#ifndef SB_PHI_REG_MAXD
-#define SB_PHI_REG_MAXD 8
-#endif
 template <int D, class LT>
 __device__ __forceinline__ void cn_phi_qc_reg(float* pm, int Z, float clip, int* sat_flag, const LT& lt) {
     const unsigned am = __activemask();
@@ -228,38 +261,33 @@ __device__ __forceinline__ void cn_phi_qc_reg(float* pm, int Z, float clip, int*
     unsigned par = 0;
 #pragma unroll
     for (int l = 0; l + 1 < D; l += 2) {
-        unsigned b0 = __float_as_uint(pm[l * Z]), b1 = __float_as_uint(pm[(l + 1) * Z]);
+        const unsigned b0 = ldw(pm + l * Z), b1 = ldw(pm + (l + 1) * Z);
         par ^= b0 ^ b1;
-        float a0 = __uint_as_float(b0 & 0x7fffffffu), a1 = __uint_as_float(b1 & 0x7fffffffu);
-        float2 q = sb_phif2(make_float2(a0, a1), lt);
-        if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;
-        P = __fadd_rn(P, q.x);
-        P = __fadd_rn(P, q.y);
-        w[l] = __float_as_uint(q.x) | (b0 & 0x80000000u);
-        w[l + 1] = __float_as_uint(q.y) | (b1 & 0x80000000u);
+        const uint2 q = phi_pass1_pair(b0, b1, P, lt, [&](float a0, float a1) {
+            if (l == 0 && __all_sync(am, a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;
+        });
+        w[l] = q.x;
+        w[l + 1] = q.y;
     }
     if (D & 1) {
-        unsigned b0 = __float_as_uint(pm[(D - 1) * Z]);
+        const unsigned b0 = ldw(pm + (D - 1) * Z);
         par ^= b0;
-        float q = sb_phif_s(__uint_as_float(b0 & 0x7fffffffu), lt);
-        P = __fadd_rn(P, q);
-        w[D - 1] = __float_as_uint(q) | (b0 & 0x80000000u);
+        w[D - 1] = phi_pass1(b0, P, lt);
     }
     par &= 0x80000000u;
 #pragma unroll
     for (int l = 0; l + 1 < D; l += 2) {
-        const unsigned b0 = w[l], b1 = w[l + 1];
-        float2 m = fadd2(make_float2(__uint_as_float(b0 | 0x80000000u), __uint_as_float(b1 | 0x80000000u)),
-                         make_float2(P, P));
-        float2 y = sb_phif2(m, lt);
-        pm[l * Z] = __uint_as_float(__float_as_uint(fminf(y.x, clip)) | ((b0 ^ par) & 0x80000000u));
-        pm[(l + 1) * Z] = __uint_as_float(__float_as_uint(fminf(y.y, clip)) | ((b1 ^ par) & 0x80000000u));
+        const uint2 y = phi_pass2_pair(w[l], w[l + 1], P, par, clip, lt);
+        stw(pm + l * Z, y.x);
+        stw(pm + (l + 1) * Z, y.y);
     }
-    if (D & 1) {
-        const unsigned b0 = w[D - 1];
-        float y = sb_phif_s(__fadd_rn(__uint_as_float(b0 | 0x80000000u), P), lt);
-        pm[(D - 1) * Z] = __uint_as_float(__float_as_uint(fminf(y, clip)) | ((b0 ^ par) & 0x80000000u));
-    }
+    if (D & 1) stw(pm + (D - 1) * Z, phi_pass2(w[D - 1], P, par, clip, lt));
+}
+
+// deg == one of DS: the register variant of that degree; returns whether it ran
+template <class LT, int... DS>
+__device__ __forceinline__ bool cn_phi_reg_of(float* pm, int Z, int deg, float clip, int* sat_flag, const LT& lt) {
+    return ((deg == DS && (cn_phi_qc_reg<DS, LT>(pm, Z, clip, sat_flag, lt), true)) || ...);
 }
 
 // The voting variant takes rows of up to 32 edges (one mask bit per edge); heavier rows (class 0 only, none in the 5G
@@ -268,42 +296,35 @@ template <int CLS, class LT>
 __device__ __forceinline__ void cn_phi_dispatch(float* pm, int Z, int deg, float clip, float phi_max, bool sc,
                                                 int* sat_flag, const LT& lt) {
     if (sc && (CLS > 0 || deg <= 32)) { cn_phi_qc_sc<LT>(pm, Z, deg, clip, phi_max, lt); return; }
-#if SB_PHI_REG_MAXD > 0
-#define SB_PHI_CASE(D) if (D <= SB_PHI_REG_MAXD && deg == D) { cn_phi_qc_reg<D, LT>(pm, Z, clip, sat_flag, lt); return; }
-    if (CLS == 4) { SB_PHI_CASE(3) SB_PHI_CASE(4) }
-    if (CLS == 3) { SB_PHI_CASE(5) SB_PHI_CASE(6) SB_PHI_CASE(7) SB_PHI_CASE(8) }
-    if (CLS == 2) { SB_PHI_CASE(9) SB_PHI_CASE(10) }
-    if (CLS == 1) { SB_PHI_CASE(19) }
-#undef SB_PHI_CASE
-#endif
+    if (CLS == 4 && cn_phi_reg_of<LT, 3, 4>(pm, Z, deg, clip, sat_flag, lt)) return;
+    if (CLS == 3 && cn_phi_reg_of<LT, 5, 6, 7, 8>(pm, Z, deg, clip, sat_flag, lt)) return;
     cn_phi_qc<LT>(pm, Z, deg, clip, sat_flag, lt);
 }
 
-__device__ __forceinline__ void cn_tanh_qc(float* pm, int Z, int deg, float clip) {
-    const float atanh_clip = (float)(1 - 1e-7);
-    float prod = 1.f;
-#pragma unroll 2
-    for (int l = 0; l < deg; ++l) {
-        float* q = pm + l * Z;
-        float t = sb_tanhf(__fmul_rn(*q, 0.5f));
-        if (t == 0.f) t = 1e-12f;
-        prod = __fmul_rn(prod, t);
-        *q = t;
-    }
-#pragma unroll 2
-    for (int l = 0; l < deg; ++l) {
-        float* q = pm + l * Z;
-        float e = __fmul_rn(__fdiv_rn(1.f, *q), prod);
-        if (fabsf(e) < 1e-7f) e = 0.f;
-        e = clipf(e, atanh_clip);
-        *q = clipf(__fmul_rn(2.f, sb_atanhf(e)), clip);
-    }
-}
+// Check-node edges pm[0], pm[Z], pm[2Z], ... for the rules of ldpc_rules.cuh
+struct StrideEdges {
+    float* pm;
+    int Z;
+    __device__ __forceinline__ float in(int l) const { return pm[l * Z]; }
+    __device__ __forceinline__ void out(int l, float v) const { pm[l * Z] = v; }
+    __device__ __forceinline__ float staged(int l) const { return pm[l * Z]; }
+};
 
 // (offset-)min-sum with the row in registers. Preconditions checked on the host: |message| <= llr_max and
 // (deg-1)*llr_max < 99000, so the reference's 1e5 sentinel logic (decoding.py:849-887) reduces exactly to
 //   unique minimum -> that edge gets fl(fl(m2 - m1) + m1), all others m1;  repeated minimum -> all edges m1.
 // Offset, max(.,0) and clipping act on only two distinct magnitudes and are hoisted out of the edge loop.
+// minsum_mags: those two magnitudes from the row's two smallest incoming ones m1 <= m2, {elsewhere, at the minimum}.
+__device__ __forceinline__ float2 minsum_mags(float m1, float m2, int deg, float clip, float offset) {
+    float min_e = (m2 == m1) ? m1 : __fadd_rn(__fsub_rn(m2, m1), m1);
+    if (deg == 1) min_e = __fadd_rn(100000.f, m1);
+    return make_float2(fminf(fmaxf(__fsub_rn(m1, offset), 0.f), clip), fminf(fmaxf(__fsub_rn(min_e, offset), 0.f), clip));
+}
+// outgoing message of the edge with incoming message v; par holds the row's sign parity in bit 31
+__device__ __forceinline__ float minsum_msg(float v, float m1, float2 o, unsigned par) {
+    const float mag = (fabsf(v) == m1) ? o.y : o.x;
+    return __uint_as_float(__float_as_uint(mag) | ((__float_as_uint(v) ^ par) & 0x80000000u));
+}
 template <int DMAX, bool EXACT>                           // EXACT: deg == DMAX, no per-edge guards
 __device__ __forceinline__ void cn_minsum_qc(float* pm, int Z, int deg, float clip, float offset) {
     float x[DMAX];                                        // every element is assigned unconditionally (registers)
@@ -320,15 +341,10 @@ __device__ __forceinline__ void cn_minsum_qc(float* pm, int Z, int deg, float cl
         par ^= __float_as_uint(v);
     }
     par &= 0x80000000u;
-    float min_e = (m2 == m1) ? m1 : __fadd_rn(__fsub_rn(m2, m1), m1);
-    if (deg == 1) min_e = __fadd_rn(100000.f, m1);
-    const float o1 = fminf(fmaxf(__fsub_rn(m1, offset), 0.f), clip);
-    const float oe = fminf(fmaxf(__fsub_rn(min_e, offset), 0.f), clip);
+    const float2 o = minsum_mags(m1, m2, deg, clip, offset);
 #pragma unroll
     for (int l = 0; l < DMAX; ++l) {
-        float v = x[l];
-        float mag = (fabsf(v) == m1) ? oe : o1;
-        float y = __uint_as_float(__float_as_uint(mag) | ((__float_as_uint(v) ^ par) & 0x80000000u));
+        const float y = minsum_msg(x[l], m1, o, par);
         if (EXACT || l < deg) pm[l * Z] = y;
     }
 }
@@ -345,44 +361,40 @@ __device__ __forceinline__ void cn_minsum_qc_loop(float* pm, int Z, int deg, flo
         par ^= __float_as_uint(v);
     }
     par &= 0x80000000u;
-    float min_e = (m2 == m1) ? m1 : __fadd_rn(__fsub_rn(m2, m1), m1);
-    if (deg == 1) min_e = __fadd_rn(100000.f, m1);
-    const float o1 = fminf(fmaxf(__fsub_rn(m1, offset), 0.f), clip);
-    const float oe = fminf(fmaxf(__fsub_rn(min_e, offset), 0.f), clip);
-    for (int l = 0; l < deg; ++l) {
-        float v = pm[l * Z];
-        float mag = (fabsf(v) == m1) ? oe : o1;
-        pm[l * Z] = __uint_as_float(__float_as_uint(mag) | ((__float_as_uint(v) ^ par) & 0x80000000u));
-    }
+    const float2 o = minsum_mags(m1, m2, deg, clip, offset);
+    for (int l = 0; l < deg; ++l) pm[l * Z] = minsum_msg(pm[l * Z], m1, o, par);
 }
 
 template <int RULE, int CLS, class LT>
 __device__ __forceinline__ void cn_qc(float* pm, int Z, int deg, float clip, float offset, float phi_max, bool sc,
                                       int* sat_flag, const LT& lt) {
-    if (RULE == SB_CN_BOXPLUS_PHI) {
+    if constexpr (RULE == SB_CN_BOXPLUS_PHI) {
         cn_phi_dispatch<CLS, LT>(pm, Z, deg, clip, phi_max, sc, sat_flag, lt);
-    }
-    else if (RULE == SB_CN_BOXPLUS) cn_tanh_qc(pm, Z, deg, clip);
-    else {
+    } else if constexpr (RULE == SB_CN_BOXPLUS) {
+        cn_tanh(StrideEdges{pm, Z}, deg, clip);
+    } else {
+        constexpr int D = kRowMax[CLS];
         const float off = (RULE == SB_CN_MINSUM) ? 0.f : offset;
         // exact-degree code for the degrees of the 5G base graphs, guarded buckets otherwise (deg is warp-uniform)
-        if (CLS == 4) {
+        if constexpr (D == kLoop) {
+            cn_minsum_qc_loop(pm, Z, deg, clip, off);
+        } else if constexpr (CLS == 4) {
             if (deg == 3) cn_minsum_qc<3, true>(pm, Z, deg, clip, off);
             else if (deg == 4) cn_minsum_qc<4, true>(pm, Z, deg, clip, off);
-            else cn_minsum_qc<4, false>(pm, Z, deg, clip, off);
-        } else if (CLS == 3) {
+            else cn_minsum_qc<D, false>(pm, Z, deg, clip, off);
+        } else if constexpr (CLS == 3) {                  // 5...8: every degree of the class is exact
             if (deg == 5) cn_minsum_qc<5, true>(pm, Z, deg, clip, off);
             else if (deg == 6) cn_minsum_qc<6, true>(pm, Z, deg, clip, off);
             else if (deg == 7) cn_minsum_qc<7, true>(pm, Z, deg, clip, off);
-            else cn_minsum_qc<8, true>(pm, Z, deg, clip, off);
-        } else if (CLS == 2) {
+            else cn_minsum_qc<D, true>(pm, Z, deg, clip, off);
+        } else if constexpr (CLS == 2) {
             if (deg == 9) cn_minsum_qc<9, true>(pm, Z, deg, clip, off);
             else if (deg == 10) cn_minsum_qc<10, true>(pm, Z, deg, clip, off);
-            else cn_minsum_qc<12, false>(pm, Z, deg, clip, off);
-        } else if (CLS == 1) {
+            else cn_minsum_qc<D, false>(pm, Z, deg, clip, off);
+        } else {
             if (deg == 19) cn_minsum_qc<19, true>(pm, Z, deg, clip, off);
-            else cn_minsum_qc<20, false>(pm, Z, deg, clip, off);
-        } else cn_minsum_qc_loop(pm, Z, deg, clip, off);
+            else cn_minsum_qc<D, false>(pm, Z, deg, clip, off);
+        }
     }
 }
 
@@ -468,38 +480,34 @@ __device__ __forceinline__ float vn_qc_loop(uint32_t msg_s, uint32_t ce_s, int d
     return x_tot;
 }
 
-// VN classes (host: col_class()): 0 loop (deg > 32), 1 <=32, 2 <=20, 3 <=12, 4 <=8, 5 <=4, 6 <=2; with edges into a
-// pruning-cut row: 7 loop, 8 <=12, 9 <=4; 10: degree-1 columns whose update is fused into the CN phase.
-// EX: exact-degree variants (min-sum kernels; the phi kernels sit at the register cap and keep the guarded buckets)
+// VN update of a column of class CLS (kColMax). EX: exact-degree variants (min-sum kernels; the phi kernels sit at the
+// register cap and keep the guarded buckets).
 template <int MODE, int CLS, bool EX>
 __device__ __forceinline__ float vn_cls(uint32_t msgb, uint32_t ce, int deg, int j4, int Z4, float llr, float clip) {
-    if (CLS == 1) return vn_qc<32, false, false, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
-    if (CLS == 2) return vn_qc<20, false, false, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
-    // exact-degree code (no guards) for every degree up to 12; deg is warp-uniform
-    if (CLS == 3) {
-        if (EX && deg == 9) return vn_qc<9, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        if (EX && deg == 10) return vn_qc<10, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        if (EX && deg == 11) return vn_qc<11, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        return vn_qc<12, false, true, MODE, EX>(msgb, ce, deg, j4, Z4, llr, clip);
+    constexpr int D = kColMax[CLS];
+    if constexpr (D == kLoop) {
+        return vn_qc_loop<MODE>(msgb, ce, deg, j4, Z4, llr, clip);
+    } else if constexpr (CLS >= kColCut) {
+        return vn_qc<D, true, true, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
+    } else if constexpr (D > 12) {                        // re-reads its messages instead of keeping them in registers
+        return vn_qc<D, false, false, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
+    } else {
+        // exact-degree code (no guards) for every degree up to 12; deg is warp-uniform
+        if constexpr (CLS == 3) {
+            if (EX && deg == 9) return vn_qc<9, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 10) return vn_qc<10, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 11) return vn_qc<11, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+        } else if constexpr (CLS == 4) {
+            if (EX && deg == 5) return vn_qc<5, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 6) return vn_qc<6, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 7) return vn_qc<7, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+        } else if constexpr (CLS == 5) {
+            if (EX && deg == 3) return vn_qc<3, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+        } else {
+            if (EX && deg == 1) return vn_qc<1, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+        }
+        return vn_qc<D, false, true, MODE, EX>(msgb, ce, deg, j4, Z4, llr, clip);
     }
-    if (CLS == 4) {
-        if (EX && deg == 5) return vn_qc<5, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        if (EX && deg == 6) return vn_qc<6, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        if (EX && deg == 7) return vn_qc<7, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        return vn_qc<8, false, true, MODE, EX>(msgb, ce, deg, j4, Z4, llr, clip);
-    }
-    if (CLS == 5) {
-        if (EX && deg == 3) return vn_qc<3, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        return vn_qc<4, false, true, MODE, EX>(msgb, ce, deg, j4, Z4, llr, clip);
-    }
-    if (CLS == 6) {
-        if (EX && deg == 1) return vn_qc<1, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-        return vn_qc<2, false, true, MODE, EX>(msgb, ce, deg, j4, Z4, llr, clip);
-    }
-    if (CLS == 8) return vn_qc<12, true, true, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
-    if (CLS == 9) return vn_qc<4, true, true, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
-    if (CLS == 10) return vn_qc<1, true, true, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
-    return vn_qc_loop<MODE>(msgb, ce, deg, j4, Z4, llr, clip);
 }
 
 struct WarpCtx {
@@ -571,8 +579,7 @@ __device__ __forceinline__ void vn_class(const QcParams& p, const WarpCtx& w, ui
                 int o = p.out_pos[v];
                 if (o >= 0) {
                     x_tot = clipf(x_tot, clip);                                              // :730
-                    p.out[(size_t)b * p.n_out + o] = p.hard_out ? (0.f >= x_tot ? 1.f : 0.f) // :622-626
-                                                                : __fmul_rn(x_tot, -1.f);
+                    p.out[(size_t)b * p.n_out + o] = decoder_out(x_tot, p.hard_out);              // :622-626
                 }
             }
         }
@@ -599,15 +606,12 @@ __device__ __forceinline__ void vn_all(const QcParams& p, const WarpCtx& w, uint
 
 // Threads per CTA. 24 warps (80 registers/thread) for every rule: 30 warps at 64 registers were measured for the min-sum
 // kernels and lost 7 % (5.32 vs 4.97 ms / 4096 codewords: more barrier and spill time than latency hiding gained).
-#ifndef SB_QC_PHI_THREADS
-#define SB_QC_PHI_THREADS 768                             // A/B hook: -DSB_QC_PHI_THREADS=1024 builds the 64-register variant
-#endif
-__host__ __device__ constexpr int qc_max_threads(int rule) { return rule == SB_CN_BOXPLUS_PHI ? SB_QC_PHI_THREADS : 768; }
+constexpr int kQcThreads = 768;
 
 // REP: copies of the phi log table (16, 8 or 1). EARLY: the early-termination variant (hard-decision bytes + syndrome
 // pass); a separate instantiation so that the default kernel carries none of it (as a run-time flag it cost 2 %).
 template <int RULE, int REP, bool EARLY>
-__global__ void __launch_bounds__(qc_max_threads(RULE), 1) ldpc_bp_qc_kernel(const __grid_constant__ QcParams p) {
+__global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_constant__ QcParams p) {
     const int T = blockDim.x, tid = threadIdx.x, lane = tid & 31, warp = tid >> 5, W = T >> 5;
     const int Z = p.Z, N = p.N, Zb = (Z + 31) >> 5;
     // carve-up by byte offsets from the __shared__ base (keeps the shared address space visible to the compiler): the
@@ -640,10 +644,7 @@ __global__ void __launch_bounds__(qc_max_threads(RULE), 1) ldpc_bp_qc_kernel(con
     for (int i = tid; i < p.nnz; i += T) s_ce_p[i] = p.col_edge[i];
     const LogTab<REP> lt(lane);
     if (RULE == SB_CN_BOXPLUS_PHI) LogTab<REP>::fill(tid, T);
-    if (p.use_tma && tid == 0) {
-        mbar_init(bar, 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (p.use_tma && tid == 0) mbar_init(bar);
     __syncthreads();
 
     const float clip = p.llr_max;
@@ -651,40 +652,18 @@ __global__ void __launch_bounds__(qc_max_threads(RULE), 1) ldpc_bp_qc_kernel(con
     uint32_t tma_phase = 0;
 
     for (long long b = blockIdx.x; b < p.B; b += gridDim.x) {
-        // ---- channel LLRs (decoding.py:552-565, 1444-1475), natural VN order -----------------------------------
-        const float* row = p.llr + (size_t)b * p.n_in;
-        if (p.use_tma) {
-            if (tid == 0) {
-                asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-                mbar_expect_tx(bar, (uint32_t)p.n_in * 4u);
-                tma_bulk_g2s(msg, row, (uint32_t)p.n_in * 4u, bar);
-            }
-            mbar_wait(bar, tma_phase);
-            tma_phase ^= 1u;
-            for (int v = tid; v < N; v += T) {
-                int ii = p.in_idx[v];
-                float l = ii >= 0 ? msg[ii] : (ii == -1 ? 0.f : -clip);
-                llr_s[v] = __fmul_rn(clipf(l, clip), -1.f);
-            }
-        } else {
-            for (int v = tid; v < N; v += T) {
-                int ii = p.in_idx[v];
-                float l = ii >= 0 ? __ldg(row + ii) : (ii == -1 ? 0.f : -clip);
-                llr_s[v] = __fmul_rn(clipf(l, clip), -1.f);
-            }
-        }
+        // ---- channel LLRs in natural VN order, staged in the message array ---------------------------------------
+        load_channel_llr(llr_s, p.llr + (size_t)b * p.n_in, p.in_idx, N, p.n_in, clip, p.use_tma, msg, bar, tma_phase,
+                         tid, T);
         __syncthreads();
         if (tid == 0) *sat_flag = 0;
         // ---- v2c = llr of the edge's VN (decoding.py:571) ---------------------------------------------------------
         vn_all<1, true>(p, w, msgb, llr_s, s_col, s_ce, clip, false, true, b);
         __syncthreads();
-        if (p.num_iter == 0) {
+        if (p.num_iter == 0) {                           // x_hat = llr_ch (decoding.py:603-608)
             for (int v = tid; v < N; v += T) {
                 int o = p.out_pos[v];
-                if (o >= 0) {
-                    float x = llr_s[v];
-                    p.out[(size_t)b * p.n_out + o] = p.hard_out ? (0.f >= x ? 1.f : 0.f) : __fmul_rn(x, -1.f);
-                }
+                if (o >= 0) p.out[(size_t)b * p.n_out + o] = decoder_out(llr_s[v], p.hard_out);
             }
         }
         // Early termination (opt-in; the reference always runs num_iter iterations, decoding.py:105-107). The VN phase
@@ -719,8 +698,7 @@ __global__ void __launch_bounds__(qc_max_threads(RULE), 1) ldpc_bp_qc_kernel(con
         }
         if (EARLY && p.iters_out && tid == 0) p.iters_out[b] = limit;
         if (p.state_out) {
-            float* st = p.state_out + (size_t)b * p.E;
-            for (int e = tid; e < p.E; e += T) st[e] = __fmul_rn(msg[p.slot_of_edge[e]], -1.f);
+            store_state(p.state_out + (size_t)b * p.E, msg, p.slot_of_edge, p.E, tid, T);
             __syncthreads();
         }
     }
@@ -731,23 +709,16 @@ size_t qc_smem_bytes(const sb_ldpc_graph* g, int tab_rep, int early = 0) {
            (size_t)g->qc_nnz * 8 + 16 + 16 + (size_t)tab_rep * SB_LOGTAB_N * 8;
 }
 
-template <typename T>
-int upload_ints(T** d, const std::vector<T>& h) {
-    SB_CUDA(cudaMalloc((void**)d, std::max<size_t>(1, h.size()) * sizeof(T)));
-    if (h.size()) SB_CUDA(cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return SB_OK;
-}
-
 int qc_ensure_uploaded(sb_ldpc_graph* g) {
     if (g->qc_uploaded) return SB_OK;
     int rc;
-    if ((rc = upload_ints(&g->d_qc_row_info, g->qc_row_info))) return rc;
-    if ((rc = upload_ints(&g->d_qc_col_info, g->qc_col_info))) return rc;
-    if ((rc = upload_ints(&g->d_qc_col_edge, g->qc_col_edge))) return rc;
-    if ((rc = upload_ints(&g->d_qc_in_idx, g->qc_in_idx))) return rc;
-    if ((rc = upload_ints(&g->d_qc_out_pos, g->qc_out_pos))) return rc;
-    if ((rc = upload_ints(&g->d_qc_slot_of_edge, g->qc_slot_of_edge))) return rc;
-    if ((rc = upload_ints(&g->d_qc_row_edge, g->qc_row_edge))) return rc;
+    if ((rc = sb_upload(&g->d_qc_row_info, g->qc_row_info))) return rc;
+    if ((rc = sb_upload(&g->d_qc_col_info, g->qc_col_info))) return rc;
+    if ((rc = sb_upload(&g->d_qc_col_edge, g->qc_col_edge))) return rc;
+    if ((rc = sb_upload(&g->d_qc_in_idx, g->qc_in_idx))) return rc;
+    if ((rc = sb_upload(&g->d_qc_out_pos, g->qc_out_pos))) return rc;
+    if ((rc = sb_upload(&g->d_qc_slot_of_edge, g->qc_slot_of_edge))) return rc;
+    if ((rc = sb_upload(&g->d_qc_row_edge, g->qc_row_edge))) return rc;
     g->qc_uploaded = true;
     return SB_OK;
 }
@@ -759,14 +730,7 @@ int launch_qc_e(const sb_ldpc_graph* g, const QcParams& p, int threads, size_t s
         if (p.tab_rep == 8) kern = ldpc_bp_qc_kernel<RULE, 8, EARLY>;
         if (p.tab_rep == 1) kern = ldpc_bp_qc_kernel<RULE, 1, EARLY>;
     }
-    SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int occ = 0;
-    SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
-    if (occ < 1) { sb_set_error("sb_ldpc_decode(qc): kernel does not fit (threads %d, smem %zu)", threads, smem); return SB_EUNSUPPORTED; }
-    long long grid = std::min<long long>(p.B, (long long)g->num_sms * occ);
-    kern<<<(unsigned)grid, threads, smem, stream>>>(p);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
+    return sb_launch_decoder(kern, p, g, threads, smem, LLONG_MAX, stream, "sb_ldpc_decode(qc)");
 }
 
 template <int RULE>
@@ -837,14 +801,12 @@ extern "C" int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entri
             col_fused[last.c] = 1;
         }
     }
-    auto row_class = [&](int r) { int d = rdeg[r]; return d > 20 ? 0 : d > 12 ? 1 : d > 8 ? 2 : d > 4 ? 3 : 4; };
+    auto row_class = [&](int r) { return degree_class(kRowMax, 0, kRowClasses, rdeg[r]); };
     auto col_class = [&](int c) {
-        if (col_fused[c]) return 10;
+        if (col_fused[c]) return kColFused;
         bool check = false;
         for (const Ent& en : by_col[c]) check = check || zrow(en.r) < Z;
-        int d = cdeg[c];
-        if (check) return d > 12 ? 7 : d > 4 ? 8 : 9;
-        return d > 32 ? 0 : d > 20 ? 1 : d > 12 ? 2 : d > 8 ? 3 : d > 4 ? 4 : d > 2 ? 5 : 6;
+        return check ? degree_class(kColMax, kColCut, kColFused, cdeg[c]) : degree_class(kColMax, 0, kColCut, cdeg[c]);
     };
     std::vector<int> rorder(n_rows), corder(n_cols);
     std::iota(rorder.begin(), rorder.end(), 0);
@@ -858,10 +820,10 @@ extern "C" int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entri
     // consecutive ones (a round gives every group at most one item) and hand the round's heaviest item to the group with
     // the smallest load so far. Degree order alone left the benchmark graph's four groups with 56/53/52/49 edges per lane
     // in the CN phase and 56/53/41/40 in the VN phase; this gives 54/54/53/49 and 48/48/47/47. G is fixed by Z and the CTA
-    // size (qc_max_threads / 32 / ceil(Z / 32)), the same for every rule.
+    // size (kQcThreads / 32 / ceil(Z / 32)), the same for every rule.
     {
         const int Zb_ = (Z + 31) / 32;
-        const int G = std::max(1, (qc_max_threads(0) / 32) / Zb_);
+        const int G = std::max(1, (kQcThreads / 32) / Zb_);
         auto balance = [&](std::vector<int>& order, const std::vector<int>& deg, auto cls_of) {
             std::vector<long long> load(G, 0);
             size_t pos = 0;
@@ -888,9 +850,9 @@ extern "C" int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entri
         balance(rorder, rdeg, row_class);
         balance(corder, cdeg, col_class);
     }
-    std::vector<int> row_cls_end(5, 0), col_cls_end(11, 0);
-    for (int r = 0; r < n_rows; ++r) for (int k = row_class(r); k < 5; ++k) ++row_cls_end[k];
-    for (int c = 0; c < n_cols; ++c) for (int k = col_class(c); k < 11; ++k) ++col_cls_end[k];
+    std::vector<int> row_cls_end(kRowClasses, 0), col_cls_end(kColClasses, 0);
+    for (int r = 0; r < n_rows; ++r) for (int k = row_class(r); k < kRowClasses; ++k) ++row_cls_end[k];
+    for (int c = 0; c < n_cols; ++c) for (int k = col_class(c); k < kColClasses; ++k) ++col_cls_end[k];
     // base-entry numbering: rows in processing order, ascending column inside a row
     std::vector<int> be_of((size_t)n_rows * n_cols, -1);
     std::vector<int> row_info(4 * n_rows), row_edge;
@@ -957,7 +919,6 @@ __global__ void debug_phi_kernel(const float* x, float* o1, float* o2, long long
 extern "C" int sb_debug_phi(const float* d_x, float* d_scalar, float* d_packed, int64_t n, void* stream) {
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_x && d_scalar && d_packed && n >= 0 && n % 2 == 0, "sb_debug_phi: bad arguments");
-    if (n == 0) return SB_OK;
     debug_phi_kernel<<<(unsigned)((n / 2 + 255) / 256), 256, LogTab<16>::bytes, (cudaStream_t)stream>>>(d_x, d_scalar,
                                                                                                          d_packed, n);
     SB_LAUNCH_CHECK();
@@ -995,7 +956,7 @@ int sb_qc_try_decode(sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_
     p.early = early; p.iters_out = d_iters; p.row_edge = (const int2*)g->d_qc_row_edge;
     p.use_tma = (g->n_in % 4 == 0) && (g->n_in <= p.E_alloc) && ((reinterpret_cast<uintptr_t>(d_llr) & 15) == 0);
     const int Zb = (g->qc_Z + 31) / 32;                    // 32-lane slices per block row (<= 12 for Z <= 384)
-    const int max_warps = qc_max_threads(cn_rule) / 32;
+    const int max_warps = kQcThreads / 32;
     int groups = std::max(1, std::min(max_warps / Zb, std::max(g->qc_rows, g->qc_cols)));
     const int threads = groups * Zb * 32;                  // every warp owns one slice index for the whole launch
     for (int k = 0; k < kRowClasses; ++k) p.row_cls_mod[k] = (k ? g->qc_row_cls_end[k - 1] : 0) % groups;

@@ -2,6 +2,7 @@
 // ldpc_bp_qc.cu (quasi-cyclic fast path), plus small device helpers used by both kernels.
 #pragma once
 #include <stdint.h>
+#include <algorithm>
 #include <vector>
 #include "sb_common.h"
 
@@ -44,13 +45,38 @@ int sb_qc_try_decode(sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_
                      int32_t* d_iters = nullptr);
 void sb_qc_free_device(sb_ldpc_graph* g);
 
+// Device copy of a host table (at least one element, so that an empty table still gets a valid pointer).
+template <typename T>
+int sb_upload(T** d, const std::vector<T>& h) {
+    SB_CUDA(cudaMalloc((void**)d, std::max<size_t>(1, h.size()) * sizeof(T)));
+    if (h.size()) SB_CUDA(cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+    return SB_OK;
+}
+
 #if defined(__CUDACC__)
+// Launch of a persistent decoder kernel: opts in to `smem` bytes of dynamic shared memory, checks that a CTA of
+// `threads` fits on an SM, and runs min(batch, resident CTAs, max_grid) CTAs that stride over the codewords.
+template <class Kernel, class Params>
+int sb_launch_decoder(Kernel kern, const Params& p, const sb_ldpc_graph* g, int threads, size_t smem, long long max_grid,
+                      cudaStream_t stream, const char* who) {
+    SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    int occ = 0;
+    SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
+    if (occ < 1) { sb_set_error("%s: kernel does not fit (threads %d, smem %zu)", who, threads, smem); return SB_EUNSUPPORTED; }
+    long long grid = std::min<long long>(p.B, std::min<long long>((long long)g->num_sms * occ, max_grid));
+    kern<<<(unsigned)grid, threads, smem, stream>>>(p);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
 __device__ __forceinline__ float clipf(float x, float c) { return fminf(fmaxf(x, -c), c); }
 
 // ---- mbarrier / TMA bulk-copy helpers (cp.async.bulk, 1-D) ------------------------------------------
 __device__ __forceinline__ uint32_t smem_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
-__device__ __forceinline__ void mbar_init(uint64_t* bar, int count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count));
+// one-arrival barrier, made visible to the async proxy before the first bulk copy
+__device__ __forceinline__ void mbar_init(uint64_t* bar) {
+    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(1));
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
 }
 __device__ __forceinline__ void mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
     asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
@@ -71,6 +97,45 @@ __device__ __forceinline__ void tma_bulk_g2s(void* dst_smem, const void* src_gme
                      smem_u32(dst_smem)),
                  "l"(src_gmem), "r"(bytes), "r"(smem_u32(bar))
                  : "memory");
+}
+
+// ---- per-codeword steps of the fused decoder kernels (ldpc_bp.cu, ldpc_bp_qc.cu); thread tid of T ------------------
+// Decoder output of a VN from its internal LLR (positive: bit 0): hard decision or logit (decoding.py:622-626).
+__device__ __forceinline__ float decoder_out(float x, int hard_out) {
+    return hard_out ? (0.f >= x ? 1.f : 0.f) : __fmul_rn(x, -1.f);
+}
+
+// Channel LLRs of one codeword, clipped and negated (decoding.py:552-565), with rate recovery (:1444-1475): in_idx[v] is
+// the input column of VN v, -1 for a punctured VN (0) and -2 for a filler VN (-clip). With `tma`, thread 0 first copies
+// the n_in inputs into `stage`, shared memory that is free until the messages are initialised.
+__device__ __forceinline__ void load_channel_llr(float* llr_s, const float* row, const int* in_idx, int N, int n_in,
+                                                 float clip, bool tma, float* stage, uint64_t* bar, uint32_t& phase,
+                                                 int tid, int T) {
+    if (tma) {
+        if (tid == 0) {
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            mbar_expect_tx(bar, (uint32_t)n_in * 4u);
+            tma_bulk_g2s(stage, row, (uint32_t)n_in * 4u, bar);
+        }
+        mbar_wait(bar, phase);
+        phase ^= 1u;
+        for (int v = tid; v < N; v += T) {
+            int ii = in_idx[v];
+            float l = ii >= 0 ? stage[ii] : (ii == -1 ? 0.f : -clip);
+            llr_s[v] = __fmul_rn(clipf(l, clip), -1.f);
+        }
+    } else {
+        for (int v = tid; v < N; v += T) {
+            int ii = in_idx[v];
+            float l = ii >= 0 ? __ldg(row + ii) : (ii == -1 ? 0.f : -clip);
+            llr_s[v] = __fmul_rn(clipf(l, clip), -1.f);
+        }
+    }
+}
+
+// Decoder state (decoding.py:636): the v2c message of every reference edge, as a logit.
+__device__ __forceinline__ void store_state(float* st, const float* v2c, const int* slot_of_edge, int E, int tid, int T) {
+    for (int e = tid; e < E; e += T) st[e] = __fmul_rn(v2c[slot_of_edge[e]], -1.f);
 }
 
 #endif
