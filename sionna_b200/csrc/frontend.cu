@@ -94,10 +94,7 @@ __global__ void __launch_bounds__(kTile) ofdm_frontend_kernel(const __grid_const
     const float es = p.e_sum[re];
     for (long long b = g; b < p.B; b += p.nbg) {
         float2 Bm[K * (K + 1) / 2], z[K];
-#pragma unroll
-        for (int e = 0; e < K * (K + 1) / 2; ++e) Bm[e] = make_float2(0.f, 0.f);
-#pragma unroll
-        for (int k = 0; k < K; ++k) z[k] = make_float2(0.f, 0.f);
+        lmmse_diag_clear<K>(Bm, z);
         const float2* yb = p.y + (b * p.RX + rx) * (long long)p.ANT * p.GRID;
         const float* nb = p.no + b * p.no_stride[0] + rx * p.no_stride[1];
 #pragma unroll 1
@@ -173,32 +170,6 @@ __global__ void __launch_bounds__(kTile) ofdm_frontend_kernel(const __grid_const
     }
 }
 
-template <int K, int METHOD>
-int launch_front(FrontParams& p, int h, cudaStream_t st) {
-    p.tiles = (p.SF + kTile - 1) / kTile;
-    const long long per_slice = (long long)p.tiles * p.RX;
-    p.nbg = (int)std::max<long long>(1, std::min<long long>(p.B, ((long long)sb_num_sms() * 8 + per_slice - 1) / per_slice));
-    const long long grid = per_slice * p.nbg;
-    if (grid > 0x7fffffffLL) return SB_EUNSUPPORTED;
-    const size_t smem = (sizeof(float2) + sizeof(int)) * (size_t)K * p.NT * kTile;
-#define SB_FRONT_CASE(HH)                                                                                              \
-    case HH:                                                                                                           \
-        if (smem > 48 * 1024 &&                                                                                        \
-            cudaFuncSetAttribute(ofdm_frontend_kernel<K, HH, METHOD>, cudaFuncAttributeMaxDynamicSharedMemorySize,     \
-                                 (int)smem) != cudaSuccess)                                                            \
-            return SB_EUNSUPPORTED;                                                                                    \
-        ofdm_frontend_kernel<K, HH, METHOD><<<(unsigned)grid, kTile, smem, st>>>(p);                                   \
-        break;
-    switch (h) { SB_FRONT_CASE(1) SB_FRONT_CASE(2) SB_FRONT_CASE(3) SB_FRONT_CASE(4) SB_FRONT_CASE(5) default: return SB_EUNSUPPORTED; }
-#undef SB_FRONT_CASE
-    return SB_OK;
-}
-
-template <int K>
-int launch_front_m(FrontParams& p, int h, int method, cudaStream_t st) {
-    return method == 1 ? launch_front<K, 1>(p, h, st) : launch_front<K, 0>(p, h, st);
-}
-
 }  // namespace
 
 extern "C" int sb_ofdm_frontend(const float* d_y, const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired,
@@ -228,13 +199,23 @@ extern "C" int sb_ofdm_frontend(const float* d_y, const float* d_no, const int64
     const int h = d_llr ? bits_per_dim : 1;
     if (d_llr)
         for (int t = 0; t < (1 << h); ++t) { p.lev[0][t] = h_lev_re[t]; p.lev[1][t] = h_lev_im[t]; }
-    int rc;
-    switch (streams_per_rx) {
-        case 1: rc = launch_front_m<1>(p, h, method, (cudaStream_t)stream); break;
-        case 2: rc = launch_front_m<2>(p, h, method, (cudaStream_t)stream); break;
-        case 3: rc = launch_front_m<3>(p, h, method, (cudaStream_t)stream); break;
-        default: rc = launch_front_m<4>(p, h, method, (cudaStream_t)stream); break;
-    }
+    p.tiles = (p.SF + kTile - 1) / kTile;
+    const long long per_slice = (long long)p.tiles * p.RX;
+    p.nbg = (int)std::max<long long>(1, std::min<long long>(p.B, ((long long)sb_num_sms() * 8 + per_slice - 1) / per_slice));
+    const long long grid = per_slice * p.nbg;
+    const size_t smem = (sizeof(float2) + sizeof(int)) * (size_t)streams_per_rx * p.NT * kTile;
+    const int rc = grid > 0x7fffffffLL ? SB_EUNSUPPORTED : sb_dispatch<1, 4>(streams_per_rx, [&](auto K) {
+        return sb_dispatch<1, 5>(h, [&](auto H) {
+            return sb_dispatch<0, 1>(method, [&](auto METHOD) {
+                auto kern = ofdm_frontend_kernel<K, H, METHOD>;
+                if (smem > 48 * 1024 &&
+                    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
+                    return SB_EUNSUPPORTED;
+                kern<<<(unsigned)grid, kTile, smem, (cudaStream_t)stream>>>(p);
+                return SB_OK;
+            });
+        });
+    });
     if (rc) { sb_set_error("sb_ofdm_frontend: unsupported configuration"); return rc; }
     SB_LAUNCH_CHECK();
     return SB_OK;

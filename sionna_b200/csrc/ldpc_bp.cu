@@ -471,19 +471,10 @@ static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t
     const int threads = pick_threads(g);
     const size_t smem = bp_smem_bytes(g, on_chip);
     cudaStream_t st = (cudaStream_t)stream;
-#define SB_BP_CASE(R)                                                             \
-    case R:                                                                       \
-        return sb_launch_decoder(on_chip ? ldpc_bp_kernel<R, true> : ldpc_bp_kernel<R, false>, p, g, threads, smem, \
+    return sb_dispatch<SB_CN_BOXPLUS_PHI, SB_CN_IDENTITY>(cn_rule, [&](auto R) {
+        return sb_launch_decoder(on_chip ? ldpc_bp_kernel<R, true> : ldpc_bp_kernel<R, false>, p, g, threads, smem,
                                  kMaxGrid, st, "sb_ldpc_decode");
-    switch (cn_rule) {
-        SB_BP_CASE(SB_CN_BOXPLUS_PHI)
-        SB_BP_CASE(SB_CN_BOXPLUS)
-        SB_BP_CASE(SB_CN_MINSUM)
-        SB_BP_CASE(SB_CN_OFFSET_MINSUM)
-        SB_BP_CASE(SB_CN_IDENTITY)
-    }
-#undef SB_BP_CASE
-    return SB_EINVAL;
+    });
 }
 
 // Debug / test export of the host-side plan (no device needed): copies the tables into caller arrays.

@@ -144,18 +144,10 @@ extern "C" int sb_ldpc_flat_cn(const float* d_v2c, float* d_c2v, const int32_t* 
     SB_CHECK_ARG(cn_rule >= SB_CN_BOXPLUS_PHI && cn_rule <= SB_CN_IDENTITY, "sb_ldpc_flat_cn: unknown cn_rule %d", cn_rule);
     cudaStream_t st = (cudaStream_t)stream;
     const int grid = sb_grid((long long)num_nodes * batch, 128, 16);
-#define SB_FLAT_CASE(R)                                                                                                  \
-    case R:                                                                                                              \
-        flat_cn_kernel<R><<<grid, 128, 0, st>>>(d_v2c, d_c2v, d_cn_ptr, d_v2c_perm, d_cn_list, num_nodes, batch, llr_max, offset); \
-        break;
-    switch (cn_rule) {
-        SB_FLAT_CASE(SB_CN_BOXPLUS_PHI)
-        SB_FLAT_CASE(SB_CN_BOXPLUS)
-        SB_FLAT_CASE(SB_CN_MINSUM)
-        SB_FLAT_CASE(SB_CN_OFFSET_MINSUM)
-        SB_FLAT_CASE(SB_CN_IDENTITY)
-    }
-#undef SB_FLAT_CASE
+    sb_dispatch<SB_CN_BOXPLUS_PHI, SB_CN_IDENTITY>(cn_rule, [&](auto R) {
+        flat_cn_kernel<R><<<grid, 128, 0, st>>>(d_v2c, d_c2v, d_cn_ptr, d_v2c_perm, d_cn_list, num_nodes, batch, llr_max, offset);
+        return SB_OK;
+    });
     SB_LAUNCH_CHECK();
     return SB_OK;
 }

@@ -724,18 +724,13 @@ int qc_ensure_uploaded(sb_ldpc_graph* g) {
 }
 
 template <int RULE, bool EARLY>
-int launch_qc_e(const sb_ldpc_graph* g, const QcParams& p, int threads, size_t smem, cudaStream_t stream) {
+int launch_qc(const sb_ldpc_graph* g, const QcParams& p, int threads, size_t smem, cudaStream_t stream) {
     auto kern = ldpc_bp_qc_kernel<RULE, 16, EARLY>;
     if constexpr (RULE == SB_CN_BOXPLUS_PHI) {
         if (p.tab_rep == 8) kern = ldpc_bp_qc_kernel<RULE, 8, EARLY>;
         if (p.tab_rep == 1) kern = ldpc_bp_qc_kernel<RULE, 1, EARLY>;
     }
     return sb_launch_decoder(kern, p, g, threads, smem, LLONG_MAX, stream, "sb_ldpc_decode(qc)");
-}
-
-template <int RULE>
-int launch_qc(const sb_ldpc_graph* g, const QcParams& p, int threads, size_t smem, cudaStream_t stream) {
-    return p.early ? launch_qc_e<RULE, true>(g, p, threads, smem, stream) : launch_qc_e<RULE, false>(g, p, threads, smem, stream);
 }
 
 }  // namespace
@@ -961,12 +956,9 @@ int sb_qc_try_decode(sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_
     const int threads = groups * Zb * 32;                  // every warp owns one slice index for the whole launch
     for (int k = 0; k < kRowClasses; ++k) p.row_cls_mod[k] = (k ? g->qc_row_cls_end[k - 1] : 0) % groups;
     for (int k = 0; k < kColClasses; ++k) p.col_cls_mod[k] = (k ? g->qc_col_cls_end[k - 1] : 0) % groups;
-    switch (cn_rule) {
-        case SB_CN_BOXPLUS_PHI: rc = launch_qc<SB_CN_BOXPLUS_PHI>(g, p, threads, smem, stream); break;
-        case SB_CN_BOXPLUS: rc = launch_qc<SB_CN_BOXPLUS>(g, p, threads, smem, stream); break;
-        case SB_CN_MINSUM: rc = launch_qc<SB_CN_MINSUM>(g, p, threads, smem, stream); break;
-        default: rc = launch_qc<SB_CN_OFFSET_MINSUM>(g, p, threads, smem, stream); break;
-    }
+    rc = sb_dispatch<SB_CN_BOXPLUS_PHI, SB_CN_OFFSET_MINSUM>(cn_rule, [&](auto R) {
+        return p.early ? launch_qc<R, true>(g, p, threads, smem, stream) : launch_qc<R, false>(g, p, threads, smem, stream);
+    });
     *handled = (rc == SB_OK);
     return rc;
 }

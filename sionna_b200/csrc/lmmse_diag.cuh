@@ -1,14 +1,22 @@
-// lmmse_diag.cuh -- LMMSE equalisation of one resource element whose interference-plus-noise covariance is diagonal
+// lmmse_diag.cuh -- LMMSE equalisation of one resource element whose interference-plus-noise covariance S is diagonal
 // (no interfering streams): everything lives in registers. Shared by the OFDM equaliser kernel (ofdm_mimo.cu) and the
 // fused receive front-end (frontend.cu), so both run the same arithmetic.
-//   input : B = H_w^H H_w (K x K Hermitian, lower triangle, row a holds (a, 0..a)) and z = H_w^H y_w of the WHITENED
-//           channel H_w = S^-1/2 H, y_w = S^-1/2 y
+//   input : B = H_w^H H_w (K x K Hermitian, lower triangle, row a holds (a, 0..a), zeroed by lmmse_diag_clear) and
+//           z = H_w^H y_w of the WHITENED channel H_w = S^-1/2 H, y_w = S^-1/2 y
 //   A = B + I = C C^H, A^-1 = C^-H C^-1;  G y_w = A^-1 z;  diag(G H_w)_k = sum_j (A^-1)_kj B_jk
 //   output: x_hat_k = (G y_w)_k / diag_k, no_eff_k = Re(1 / diag_k - 1)     (mimo/equalization.py:217-231)
 #pragma once
 #include "sb_common.h"
 
 namespace sb_lmmse {
+template <int K>
+__device__ __forceinline__ void lmmse_diag_clear(float2* Bm, float2* z) {
+#pragma unroll
+    for (int e = 0; e < K * (K + 1) / 2; ++e) Bm[e] = make_float2(0.f, 0.f);
+#pragma unroll
+    for (int k = 0; k < K; ++k) z[k] = make_float2(0.f, 0.f);
+}
+
 template <int K>
 __device__ __forceinline__ void lmmse_diag_solve(const float2* Bm, const float2* z, float2* xh, float* ne) {
     // A = B + I = C C^H (lower, in registers)

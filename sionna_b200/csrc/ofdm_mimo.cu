@@ -995,12 +995,8 @@ __global__ void __launch_bounds__(128, 4) ofdm_lmmse_diag_kernel(const OfdmEqPar
         int des[K];
 #pragma unroll
         for (int k = 0; k < K; ++k) des[k] = p.des[rx * K + k];
-        float2 Bm[K * (K + 1) / 2];                             // lower triangle, row a: entries (a, 0..a)
-        float2 z[K];
-#pragma unroll
-        for (int e = 0; e < K * (K + 1) / 2; ++e) Bm[e] = make_float2(0.f, 0.f);
-#pragma unroll
-        for (int k = 0; k < K; ++k) z[k] = make_float2(0.f, 0.f);
+        float2 Bm[K * (K + 1) / 2], z[K];
+        sb_lmmse::lmmse_diag_clear<K>(Bm, z);
         // antennas in chunks of 4: all loads of a chunk (y, K channel columns, the error variances, no) are issued before
         // any of them is used, so 4 * (K + 1) 8-byte loads per thread are in flight instead of one dependent load at a
         // time (the one-antenna-per-trip version was latency bound: long_scoreboard 3.4 warps per issue, 27 % of HBM peak).
@@ -1070,11 +1066,6 @@ __global__ void __launch_bounds__(128, 4) ofdm_lmmse_diag_kernel(const OfdmEqPar
             }
         }
     }
-}
-
-template <int K>
-void launch_lmmse_diag(const OfdmEqParams& p, long long total, cudaStream_t stream) {
-    ofdm_lmmse_diag_kernel<K><<<sb_grid(total, 128, 16), 128, 0, stream>>>(p);
 }
 
 int make_plan(int n, FftPlan* plan) {
@@ -1455,12 +1446,10 @@ extern "C" int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float
     p.S = num_symbols; p.F = num_subcarriers; p.K = streams_per_rx; p.KU = interferers_per_rx; p.ND = num_data;
     long long total_re = batch * num_rx * (long long)num_symbols * num_subcarriers;
     if (interferers_per_rx == 0 && streams_per_rx <= 4) {     // diagonal noise covariance: register kernel
-        switch (streams_per_rx) {
-            case 1: launch_lmmse_diag<1>(p, total_re, (cudaStream_t)stream); break;
-            case 2: launch_lmmse_diag<2>(p, total_re, (cudaStream_t)stream); break;
-            case 3: launch_lmmse_diag<3>(p, total_re, (cudaStream_t)stream); break;
-            default: launch_lmmse_diag<4>(p, total_re, (cudaStream_t)stream); break;
-        }
+        sb_dispatch<1, 4>(streams_per_rx, [&](auto K) {
+            ofdm_lmmse_diag_kernel<K><<<sb_grid(total_re, 128, 16), 128, 0, (cudaStream_t)stream>>>(p);
+            return SB_OK;
+        });
         SB_LAUNCH_CHECK();
         return SB_OK;
     }

@@ -66,13 +66,30 @@ __device__ __forceinline__ float softplusf(float x) {
 }
 __device__ __forceinline__ float log_sigmoidf(float x) { return -softplusf(-x); }
 
+// Stores the M LLRs of the symbols base + threadIdx.x (those < n_sym) through the warp's own tile of 32 * M floats of
+// shared memory (s_out: 32 * M floats per warp of the CTA), so that a warp's global stores are contiguous; no CTA barrier.
+template <int M>
+__device__ __forceinline__ void store_llrs_warp(float* s_out, const float* out, long long base, long long n_sym,
+                                                float* __restrict__ llr) {
+    const int lane = threadIdx.x & 31, wbase = (threadIdx.x >> 5) * 32 * M;
+    __syncwarp();                                                   // previous tile's copy-out has finished
+    if (base + threadIdx.x < n_sym) {
+#pragma unroll
+        for (int i = 0; i < M; ++i) s_out[wbase + lane * M + i] = out[i];
+    }
+    __syncwarp();
+    const long long wfirst = base + (threadIdx.x & ~31);
+    const long long rem = n_sym - wfirst;
+    const int cnt = rem <= 0 ? 0 : (int)((rem < 32 ? rem : 32) * M);
+    for (int q = lane; q < cnt; q += 32) llr[wfirst * M + q] = s_out[wbase + q];
+}
+
 // One thread per symbol, M = bits per symbol at compile time. Exponents e_j = -|y - c_j|^2 / max(no, tiny) (+ prior
 // term) are evaluated once per pass and feed all 2M groups {points with bit i = v} at the same time:
 //   pass 1: group maxima (maxlog: done);  pass 2 (app): sum_j exp(e_j - max_group) per group, two groups per packed
 //   FP32x2 exp (sb_math2.cuh, bit-identical to sb_expf); LLR_i = logsumexp(bit i = 1) - logsumexp(bit i = 0).
 // Per group the operation order is the one of tf.reduce_logsumexp over the points in ascending label order, which is
-// what the CPU oracle (oracle/mapping_ref.c) evaluates. The M LLRs of a warp's 32 symbols are staged through shared
-// memory so that global stores are contiguous.
+// what the CPU oracle (oracle/mapping_ref.c) evaluates. The LLRs leave through store_llrs_warp.
 template <int M>
 __device__ __forceinline__ float demap_exponent(float2 yy, float2 c, float n0, const float* ls1, const float* ls0, int j,
                                                 bool with_prior) {
@@ -95,7 +112,7 @@ __global__ void __launch_bounds__(128) demap_kernel(const float2* __restrict__ y
                                                     float* __restrict__ llr, long long n_sym, int hard_out) {
     extern __shared__ float2 s_pts[];
     constexpr int NPTS = 1 << M;
-    float* s_out = reinterpret_cast<float*>(s_pts + NPTS);          // [blockDim.x * M] staging for coalesced stores
+    float* s_out = reinterpret_cast<float*>(s_pts + NPTS);          // [blockDim.x * M] store_llrs_warp tiles
     for (int i = threadIdx.x; i < NPTS; i += blockDim.x) s_pts[i] = points[i];
     __syncthreads();
     const float tiny = 1.17549435e-38f;   // np.finfo(float32).tiny (mapping.py:653)
@@ -173,15 +190,7 @@ __global__ void __launch_bounds__(128) demap_kernel(const float2* __restrict__ y
 #pragma unroll
             for (int i = 0; i < M; ++i) out[i] = hard_out ? (out[i] > 0.f ? 1.f : 0.f) : out[i];   // utils/misc.py:270
         }
-        __syncthreads();                                            // previous tile's copy-out has finished
-        if (s < n_sym) {
-#pragma unroll
-            for (int i = 0; i < M; ++i) s_out[threadIdx.x * M + i] = out[i];
-        }
-        __syncthreads();
-        const long long rem = n_sym - base;
-        const int cnt = (int)((rem < (long long)blockDim.x ? rem : (long long)blockDim.x) * M);
-        for (int e = threadIdx.x; e < cnt; e += blockDim.x) llr[base * M + e] = s_out[e];
+        store_llrs_warp<M>(s_out, out, base, n_sym, llr);
     }
 }
 
@@ -197,7 +206,7 @@ __global__ void __launch_bounds__(128) demap_qam_kernel(const float2* __restrict
                                                         const float* __restrict__ lev_im, float* __restrict__ llr,
                                                         long long n_sym, int hard_out) {
     constexpr int L = 1 << H, M = 2 * H;
-    extern __shared__ float s_out_q[];                              // [blockDim.x * M]
+    extern __shared__ float s_out_q[];                              // [blockDim.x * M] store_llrs_warp tiles
     float lr[L], li[L];
 #pragma unroll
     for (int t = 0; t < L; ++t) { lr[t] = lev_re[t]; li[t] = lev_im[t]; }
@@ -211,41 +220,8 @@ __global__ void __launch_bounds__(128) demap_qam_kernel(const float2* __restrict
             const float inv_n0 = __fdiv_rn(1.0f, fmaxf(no[s / no_inner], tiny));   // one division per symbol
             demap_qam_symbol<METHOD, H>(yy, inv_n0, lr, li, lev_re, lev_im, hard_out, out);
         }
-        // stage the warp's 32 x M LLRs through its own shared-memory tile: contiguous global stores, no CTA barrier
-        {
-            const int lane = threadIdx.x & 31, wbase = (threadIdx.x >> 5) * 32 * M;
-            __syncwarp();                                           // previous tile's copy-out has finished
-            if (s < n_sym) {
-#pragma unroll
-                for (int i = 0; i < M; ++i) s_out_q[wbase + lane * M + i] = out[i];
-            }
-            __syncwarp();
-            const long long wfirst = base + (threadIdx.x & ~31);
-            const long long rem = n_sym - wfirst;
-            const int cnt = rem <= 0 ? 0 : (int)((rem < 32 ? rem : 32) * M);
-            for (int q = lane; q < cnt; q += 32) llr[wfirst * M + q] = s_out_q[wbase + q];
-        }
+        store_llrs_warp<M>(s_out_q, out, base, n_sym, llr);
     }
-}
-
-template <int METHOD>
-void launch_demap_qam(int h, int grid, cudaStream_t st, const float2* y, const float* no, long long no_inner,
-                      const float* lev_re, const float* lev_im, float* llr, long long n_sym, int hard_out) {
-    const size_t smem = sizeof(float) * 128 * 2 * h;
-#define SB_QAM_CASE(HH) case HH: demap_qam_kernel<METHOD, HH><<<grid, 128, smem, st>>>(y, no, no_inner, lev_re, lev_im, llr, n_sym, hard_out); break;
-    switch (h) { SB_QAM_CASE(1) SB_QAM_CASE(2) SB_QAM_CASE(3) SB_QAM_CASE(4) SB_QAM_CASE(5) }
-#undef SB_QAM_CASE
-}
-
-template <int METHOD>
-void launch_demap(int m, int grid, size_t smem, cudaStream_t st, const float2* y, const float* no, long long no_inner,
-                  const float2* pts, const float* prior, long long prior_inner, float* llr, long long n_sym, int hard_out) {
-#define SB_DEMAP_CASE(MM) case MM: demap_kernel<METHOD, MM><<<grid, 128, smem, st>>>(y, no, no_inner, pts, prior, prior_inner, llr, n_sym, hard_out); break;
-    switch (m) {
-        SB_DEMAP_CASE(1) SB_DEMAP_CASE(2) SB_DEMAP_CASE(3) SB_DEMAP_CASE(4) SB_DEMAP_CASE(5) SB_DEMAP_CASE(6)
-        SB_DEMAP_CASE(7) SB_DEMAP_CASE(8) SB_DEMAP_CASE(9) SB_DEMAP_CASE(10) SB_DEMAP_CASE(11) SB_DEMAP_CASE(12)
-    }
-#undef SB_DEMAP_CASE
 }
 
 // ---------------------------------------------------------------------------------------------------------
@@ -270,31 +246,27 @@ __global__ void awgn_kernel(const float2* x, const float* __restrict__ no, long 
     }
 }
 
-// real-valued variant used for LLR-domain test sources (GaussianPriorSource): out = mean + std * N(0,1)
-__global__ void normal_kernel(float* __restrict__ out, long long n, float mean, float stdv, unsigned long long seed,
-                              unsigned long long offset) {
+// Real-valued Philox draws, four outputs per Philox block. NORMAL: out = a + b * N(0,1) by two Box-Muller pairs
+// (GaussianPriorSource); otherwise out = a + (b - a) * u, u in [0, 1) with 24 random bits (TDL Doppler / angle / phase).
+template <bool NORMAL>
+__global__ void philox_fill_kernel(float* __restrict__ out, long long n, float a, float b, unsigned long long seed,
+                                   unsigned long long offset) {
     long long stride = (long long)gridDim.x * blockDim.x;
+    const float w = b - a;
     for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; 4 * p < n; p += stride) {
         uint4 r = philox4x32_10(seed, offset, (unsigned long long)p);
-        float2 g0 = box_muller(r.x, r.y), g1 = box_muller(r.z, r.w);
-        float v[4] = {g0.x, g0.y, g1.x, g1.y};
+        float v[4];
+        if (NORMAL) {
+            float2 g0 = box_muller(r.x, r.y), g1 = box_muller(r.z, r.w);
+            v[0] = g0.x; v[1] = g0.y; v[2] = g1.x; v[3] = g1.y;
+        } else {
+            unsigned u[4] = {r.x, r.y, r.z, r.w};
+#pragma unroll
+            for (int k = 0; k < 4; ++k) v[k] = (float)(u[k] >> 8) * 5.9604644775390625e-08f;   // 2^-24
+        }
 #pragma unroll
         for (int k = 0; k < 4; ++k)
-            if (4 * p + k < n) out[4 * p + k] = mean + stdv * v[k];
-    }
-}
-
-// uniform variant: out = lo + (hi - lo) * u, u in [0, 1) with 24 random bits (TDL Doppler / angle / phase draws)
-__global__ void uniform_kernel(float* __restrict__ out, long long n, float lo, float hi, unsigned long long seed,
-                               unsigned long long offset) {
-    long long stride = (long long)gridDim.x * blockDim.x;
-    const float w = hi - lo;
-    for (long long p = (long long)blockIdx.x * blockDim.x + threadIdx.x; 4 * p < n; p += stride) {
-        uint4 r = philox4x32_10(seed, offset, (unsigned long long)p);
-        unsigned v[4] = {r.x, r.y, r.z, r.w};
-#pragma unroll
-        for (int k = 0; k < 4; ++k)
-            if (4 * p + k < n) out[4 * p + k] = lo + w * ((float)(v[k] >> 8) * 5.9604644775390625e-08f);   // 2^-24
+            if (4 * p + k < n) out[4 * p + k] = a + (NORMAL ? b : w) * v[k];
     }
 }
 
@@ -330,42 +302,33 @@ __global__ void count_errors_kernel(const float* __restrict__ b, const float* __
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// CRCEncoder.call (fec/crc.py:175-215): the reference multiplies the bit row with a dense [k, L] generator matrix and
-// reduces mod 2; the CRC is linear, so the parity word is the XOR of the (bit-packed) matrix rows selected by the set
-// bits. One warp per row: lanes stride over the k bits, XOR-reduce, then write [bits | parity] (MSB = first parity bit).
-__global__ void crc_encode_kernel(const float* __restrict__ bits, const unsigned* __restrict__ gtab, int k, int L,
-                                  float* __restrict__ out, long long rows) {
+// CRCEncoder.call (fec/crc.py:175-215) and, CHECK, CRCDecoder.call (fec/crc.py:300-327). The reference multiplies the
+// bit row with a dense [n, L] generator matrix and reduces mod 2; the CRC is linear, so the parity word is the XOR of
+// the (bit-packed) matrix rows selected by the set bits. One warp per row of n bits: lanes stride over the bits,
+// XOR-reduce, then
+//   encode: out row = [bits | parity] (n + L values, MSB = first parity bit);
+//   check:  the row is a whole word [info | parity], valid = (parity of the word == 0); out (optional) gets the
+//           n - L information bits.
+template <bool CHECK>
+__global__ void crc_kernel(const float* __restrict__ x, const unsigned* __restrict__ gtab, int n, int L,
+                           float* __restrict__ out, unsigned char* __restrict__ valid, long long rows) {
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    for (long long r = (long long)blockIdx.x * nwarps + warp; r < rows; r += (long long)gridDim.x * nwarps) {
-        const float* b = bits + r * k;
-        float* o = out + r * (long long)(k + L);
-        unsigned acc = 0;
-        for (int i = lane; i < k; i += 32) {
-            float v = b[i];
-            o[i] = v;
-            if (((int)v) & 1) acc ^= gtab[i];
-        }
-        acc = __reduce_xor_sync(0xffffffffu, acc);
-        if (lane < L) o[k + lane] = (float)((acc >> (L - 1 - lane)) & 1u);
-    }
-}
-
-// CRCDecoder.call (fec/crc.py:300-327): the whole word [info | parity] (n bits) is run through the encoder again and the
-// check passes iff the new parity is all zero. One warp per row; also copies the n - L information bits.
-__global__ void crc_check_kernel(const float* __restrict__ x, const unsigned* __restrict__ gtab, int n, int L,
-                                 float* __restrict__ info, unsigned char* __restrict__ valid, long long rows) {
-    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5, nwarps = blockDim.x >> 5;
-    const int k = n - L;
+    const int k = CHECK ? n - L : n;                                // bits copied to out
+    const long long out_len = CHECK ? k : n + L;
     for (long long r = (long long)blockIdx.x * nwarps + warp; r < rows; r += (long long)gridDim.x * nwarps) {
         const float* b = x + r * (long long)n;
         unsigned acc = 0;
         for (int i = lane; i < n; i += 32) {
             float v = b[i];
-            if (info && i < k) info[r * (long long)k + i] = v;
+            if (!CHECK || (out && i < k)) out[r * out_len + i] = v;
             if (((int)v) & 1) acc ^= gtab[i];
         }
         acc = __reduce_xor_sync(0xffffffffu, acc);
-        if (lane == 0) valid[r] = acc == 0u ? 1 : 0;
+        if (CHECK) {
+            if (lane == 0) valid[r] = acc == 0u ? 1 : 0;
+        } else if (lane < L) {
+            out[r * out_len + k + lane] = (float)((acc >> (L - 1 - lane)) & 1u);
+        }
     }
 }
 
@@ -388,7 +351,6 @@ __global__ void scramble_kernel(const float* __restrict__ x, const float* __rest
 extern "C" int sb_binary_source(float* d_out, int64_t n, uint64_t seed, uint64_t offset, void* stream) {
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_out && n >= 0, "sb_binary_source: bad arguments");
-    if (n == 0) return SB_OK;
     binary_source_kernel<<<sb_grid((n + 127) / 128, 128, 8), 128, 0, (cudaStream_t)stream>>>(d_out, n, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
@@ -398,7 +360,6 @@ extern "C" int sb_qam_map(const float* d_bits, const float* d_points, int32_t m,
                           int64_t n_sym, void* stream) {
     if (n_sym == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_bits && d_points && d_out && m >= 1 && m <= 12 && n_sym >= 0, "sb_qam_map: bad arguments");
-    if (n_sym == 0) return SB_OK;
     size_t smem = sizeof(float2) << m;
     qam_map_kernel<<<sb_grid(n_sym, 256, 8), 256, smem, (cudaStream_t)stream>>>(
         d_bits, (const float2*)d_points, m, (float2*)d_out, d_idx_out, n_sym);
@@ -414,15 +375,15 @@ extern "C" int sb_demap(const float* d_y, const float* d_no, int64_t no_inner, c
                  "sb_demap: bad arguments");
     SB_CHECK_ARG(method == 0 || method == 1, "sb_demap: method must be 0 (app) or 1 (maxlog)");
     SB_CHECK_ARG(!d_prior || prior_inner >= 1, "sb_demap: prior_inner must be >= 1");
-    if (n_sym == 0) return SB_OK;
-    size_t smem = (sizeof(float2) << m) + sizeof(float) * 128 * m;
-    int grid = sb_grid(n_sym, 128, 8);
-    if (method == 0)
-        launch_demap<0>(m, grid, smem, (cudaStream_t)stream, (const float2*)d_y, d_no, no_inner, (const float2*)d_points,
-                        d_prior, prior_inner, d_llr, n_sym, hard_out);
-    else
-        launch_demap<1>(m, grid, smem, (cudaStream_t)stream, (const float2*)d_y, d_no, no_inner, (const float2*)d_points,
-                        d_prior, prior_inner, d_llr, n_sym, hard_out);
+    const size_t smem = (sizeof(float2) << m) + sizeof(float) * 128 * m;
+    const int grid = sb_grid(n_sym, 128, 8);
+    sb_dispatch<0, 1>(method, [&](auto METHOD) {
+        return sb_dispatch<1, 12>(m, [&](auto M) {
+            demap_kernel<METHOD, M><<<grid, 128, smem, (cudaStream_t)stream>>>(
+                (const float2*)d_y, d_no, no_inner, (const float2*)d_points, d_prior, prior_inner, d_llr, n_sym, hard_out);
+            return SB_OK;
+        });
+    });
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -433,13 +394,15 @@ extern "C" int sb_demap_qam(const float* d_y, const float* d_no, int64_t no_inne
     if (n_sym == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_y && d_no && d_levels_re && d_levels_im && d_llr && m >= 2 && m <= 10 && m % 2 == 0 && no_inner >= 1 &&
                      (method == 0 || method == 1), "sb_demap_qam: bad arguments (m even, 2..10; method 0 | 1)");
-    int grid = sb_grid(n_sym, 128, 8);
-    if (method == 0)
-        launch_demap_qam<0>(m / 2, grid, (cudaStream_t)stream, (const float2*)d_y, d_no, no_inner, d_levels_re, d_levels_im,
-                            d_llr, n_sym, hard_out);
-    else
-        launch_demap_qam<1>(m / 2, grid, (cudaStream_t)stream, (const float2*)d_y, d_no, no_inner, d_levels_re, d_levels_im,
-                            d_llr, n_sym, hard_out);
+    const size_t smem = sizeof(float) * 128 * m;
+    const int grid = sb_grid(n_sym, 128, 8);
+    sb_dispatch<0, 1>(method, [&](auto METHOD) {
+        return sb_dispatch<1, 5>(m / 2, [&](auto H) {
+            demap_qam_kernel<METHOD, H><<<grid, 128, smem, (cudaStream_t)stream>>>((const float2*)d_y, d_no, no_inner, d_levels_re,
+                                                                                   d_levels_im, d_llr, n_sym, hard_out);
+            return SB_OK;
+        });
+    });
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -448,7 +411,6 @@ extern "C" int sb_awgn(const float* d_x, const float* d_no, int64_t no_inner, fl
                        uint64_t offset, void* stream) {
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_x && d_no && d_y && n >= 0 && no_inner >= 1, "sb_awgn: bad arguments");
-    if (n == 0) return SB_OK;
     awgn_kernel<<<sb_grid((n + 1) / 2, 256, 8), 256, 0, (cudaStream_t)stream>>>((const float2*)d_x, d_no, no_inner,
                                                                               (float2*)d_y, n, seed, offset);
     SB_LAUNCH_CHECK();
@@ -458,8 +420,7 @@ extern "C" int sb_awgn(const float* d_x, const float* d_no, int64_t no_inner, fl
 extern "C" int sb_normal(float* d_out, int64_t n, float mean, float stddev, uint64_t seed, uint64_t offset, void* stream) {
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_out && n >= 0, "sb_normal: bad arguments");
-    if (n == 0) return SB_OK;
-    normal_kernel<<<sb_grid((n + 3) / 4, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_out, n, mean, stddev, seed, offset);
+    philox_fill_kernel<true><<<sb_grid((n + 3) / 4, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_out, n, mean, stddev, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -467,7 +428,7 @@ extern "C" int sb_normal(float* d_out, int64_t n, float mean, float stddev, uint
 extern "C" int sb_uniform(float* d_out, int64_t n, float lo, float hi, uint64_t seed, uint64_t offset, void* stream) {
     if (n == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_out && n >= 0 && hi >= lo, "sb_uniform: bad arguments");
-    uniform_kernel<<<sb_grid((n + 3) / 4, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_out, n, lo, hi, seed, offset);
+    philox_fill_kernel<false><<<sb_grid((n + 3) / 4, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_out, n, lo, hi, seed, offset);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -476,7 +437,6 @@ extern "C" int sb_count_errors(const float* d_b, const float* d_b_hat, int64_t r
                                void* stream) {
     if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_b && d_b_hat && d_counters && rows >= 0 && k >= 1, "sb_count_errors: bad arguments");
-    if (rows == 0) return SB_OK;
     count_errors_kernel<<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(
         d_b, d_b_hat, rows, k, (unsigned long long*)d_counters);
     SB_LAUNCH_CHECK();
@@ -488,8 +448,8 @@ extern "C" int sb_crc_encode(const float* d_bits, const uint32_t* d_gen_rows, in
     if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_bits && d_gen_rows && d_out && k >= 1 && crc_length >= 1 && crc_length <= 32 && rows >= 0,
                  "sb_crc_encode: bad arguments");
-    if (rows == 0) return SB_OK;
-    crc_encode_kernel<<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_bits, d_gen_rows, k, crc_length, d_out, rows);
+    crc_kernel<false><<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_bits, d_gen_rows, k, crc_length, d_out,
+                                                                                   nullptr, rows);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -499,7 +459,8 @@ extern "C" int sb_crc_check(const float* d_x, const uint32_t* d_gen_rows, int32_
     if (rows == 0) return SB_OK;
     SB_CHECK_ARG(d_x && d_gen_rows && d_valid && crc_length >= 1 && crc_length <= 32 && n >= crc_length && rows >= 0,
                  "sb_crc_check: bad arguments");
-    crc_check_kernel<<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_x, d_gen_rows, n, crc_length, d_info, d_valid, rows);
+    crc_kernel<true><<<sb_grid(rows * 32, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_x, d_gen_rows, n, crc_length, d_info,
+                                                                                  d_valid, rows);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -508,7 +469,6 @@ extern "C" int sb_scramble(const float* d_x, const float* d_seq, int32_t binary,
                            int32_t seq_rows, void* stream) {
     if (rows == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_x && d_seq && d_out && rows >= 0 && n >= 1 && seq_rows >= 1, "sb_scramble: bad arguments");
-    if (rows == 0) return SB_OK;
     scramble_kernel<<<sb_grid(rows * n, 256, 8), 256, 0, (cudaStream_t)stream>>>(d_x, d_seq, binary, d_out, rows, n, seq_rows);
     SB_LAUNCH_CHECK();
     return SB_OK;

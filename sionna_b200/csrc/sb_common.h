@@ -4,6 +4,7 @@
 #include <stdarg.h>
 #include <stdio.h>
 #include <algorithm>
+#include <type_traits>
 #include "../../include/sionna_b200.h"
 
 // thread-local error message (defined in common.cu)
@@ -47,6 +48,18 @@ static inline int sb_num_sms(void) {
 static inline int sb_grid(long long items, int per_cta, int ctas_per_sm) {
     const long long ctas = (items + per_cta - 1) / per_cta;
     return (int)std::max<long long>(1, std::min<long long>(ctas, (long long)sb_num_sms() * ctas_per_sm));
+}
+
+// Compile-time dispatch of a small runtime integer: f(std::integral_constant<int, v>{}) for v in [LO, HI], whose int
+// result is returned; SB_EUNSUPPORTED for any other v.
+template <int LO, int HI, class F>
+static inline int sb_dispatch(int v, F&& f) {
+    if constexpr (LO > HI) {
+        return SB_EUNSUPPORTED;
+    } else {
+        if (v == LO) return f(std::integral_constant<int, LO>{});
+        return sb_dispatch<LO + 1, HI>(v, f);
+    }
 }
 
 // Row-wise element kernels: blockDim = (tx, ty) with tx = row length rounded up to a warp (<= 256) and ty rows per CTA;

@@ -9,6 +9,7 @@ import torch
 
 from ..block import Block
 from ..config import config
+from .._lib_helpers import philox_fill
 from ..._lib import lib, check, ptr, current_stream
 
 _MODELS = os.path.join(os.path.dirname(os.path.abspath(__file__)), "tdl_models.npz")
@@ -25,10 +26,7 @@ def subcarrier_frequencies(num_subcarriers, subcarrier_spacing, precision=None):
 
 def _uniform(shape, lo, hi):
     """config.tf_rng.uniform(shape, lo, hi) on the device (``sb_uniform``, Philox4x32-10)."""
-    out = torch.empty([int(v) for v in shape], dtype=torch.float32, device=config.device)
-    seed, off = config.next_philox()
-    check(lib().sb_uniform(ptr(out), out.numel(), float(lo), float(hi), seed, off, current_stream()), "sb_uniform")
-    return out
+    return philox_fill("sb_uniform", shape, lo, hi, config.device)
 
 
 class _TableCache:

@@ -5,7 +5,7 @@ import torch
 
 from ..block import Block
 from ..config import config
-from .._lib_helpers import philox_normal
+from .._lib_helpers import philox_fill
 
 
 class GaussianPriorSource(Block):
@@ -33,7 +33,7 @@ class GaussianPriorSource(Block):
             sigma_llr = np.sqrt(4.0 / no)
             mu_llr = sigma_llr ** 2 / 2
         shape = [int(s) for s in output_shape]
-        return philox_normal(shape, -mu_llr, sigma_llr, self.device).to(self.rdtype)
+        return philox_fill("sb_normal", shape, -mu_llr, sigma_llr, self.device).to(self.rdtype)
 
 
 def llr2mi(llr, s=None, reduce_dims=True):
