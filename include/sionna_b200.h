@@ -348,6 +348,37 @@ int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float* d_err_var
                   int32_t num_subcarriers, int32_t streams_per_rx, int32_t interferers_per_rx, int32_t num_data,
                   void* stream);
 
+/* MaximumLikelihoodDetector.call (mimo/detection.py:473-537, whiten_channel mimo/utils.py:292-357, SymbolLogits2LLRs.call
+ * mapping.py:927-967), complex64: d_y [num, M], d_h [num, M, K], d_s [num, M, M], optional d_prior [num, K, num_points]
+ * symbol logits (bit priors are converted by the caller, LLRs2SymbolLogits mapping.py:1045-1059), d_points [num_points]
+ * complex (any constellation). method 0 app (logsumexp) / 1 maxlog (max); output 0 bit / 1 symbol; hard_out 0 / 1.
+ * d_out: bit LLRs or hard bits [num, K, log2 num_points] (float), symbol logits [num, K, num_points] (float) or hard
+ * symbol indices [num, K] (int32, first maximum). d_workspace: device memory of at least
+ * sb_ml_workspace_bytes(num, K) bytes, 8-byte aligned (per-problem whitened triangular records and output positions;
+ * SB_ENOMEM if it is missing or smaller).
+ * Malformed arguments return SB_EINVAL; 1 <= K <= 8, num_points a power of two in 2 ... 1024, num_points^K <= 65536
+ * and any M >= 1 (M < K allowed) whose whitening scratch 8 (M^2 + M K + M) bytes per problem fits 200 KB are
+ * supported, larger configurations return SB_EUNSUPPORTED with a message. */
+int sb_mimo_ml(const float* d_y, const float* d_h, const float* d_s, const float* d_prior, const float* d_points,
+               void* d_out, void* d_workspace, size_t workspace_bytes, int64_t num, int32_t M, int32_t K,
+               int32_t num_points, int32_t method, int32_t output, int32_t hard_out, void* stream);
+/* Workspace bytes sb_mimo_ml / sb_ofdm_ml need for num_problems problems of K streams: 8 (K^2 + 2 K + 1) per problem
+ * (sb_ofdm_ml: num_problems = batch * num_rx * num_symbols * num_subcarriers); 0 for K outside 1 ... 8. */
+size_t sb_ml_workspace_bytes(int64_t num_problems, int32_t K);
+/* OFDM MaximumLikelihoodDetector / MaximumLikelihoodDetectorWithPrior (ofdm/detection.py:448-738): sb_ofdm_lmmse's
+ * inputs, strides, tables and broadcast rules (S = H_u H_u^H + diag(no) + diag(sum err_var) assembled per resource
+ * element), then sb_mimo_ml's detector with K = streams_per_rx. d_prior (optional): symbol logits in the output layout
+ * [batch, num_tx_streams, num_data, num_points]. d_out: [batch, num_tx_streams, num_data * log2 num_points] (bits),
+ * [batch, num_tx_streams, num_data, num_points] (logits) or [batch, num_tx_streams, num_data] (int32 indices).
+ * Workspace and limits as sb_mimo_ml with M = num_rx_ant. */
+int sb_ofdm_ml(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
+               const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired, const int32_t* d_undesired,
+               const int32_t* d_out_stream, const int32_t* d_data_pos, const float* d_prior, const float* d_points,
+               void* d_out, void* d_workspace, size_t workspace_bytes, int64_t batch, int32_t num_rx,
+               int32_t num_rx_ant, int32_t num_tx_streams, int32_t num_symbols, int32_t num_subcarriers,
+               int32_t streams_per_rx, int32_t interferers_per_rx, int32_t num_data, int32_t num_points, int32_t method,
+               int32_t output, int32_t hard_out, void* stream);
+
 /* Fused receive front-end (csrc/frontend.cu): LS estimation at the pilots (+ PUSCH CDM de-spreading) + nearest /
  * linear interpolation + OFDM equaliser glue + LMMSE equalisation + square-QAM demapping in ONE launch, for receivers
  * without interfering streams and 1..4 streams (ofdm/channel_estimation.py:138-285, 364-734, ofdm/equalization.py:126-275,

@@ -70,6 +70,9 @@ SIGNATURES = {
     "sb_mimo_linalg": (i32, [i32, vp, vp, vp, vp, vp, i64, i32, i32, vp]),
     "sb_ofdm_frontend": (i32, [vp] * 15 + [i64] + [i32] * 11 + [vp]),
     "sb_ofdm_lmmse": (i32, [vp] * 12 + [i64] + [i32] * 8 + [vp]),
+    "sb_mimo_ml": (i32, [vp] * 7 + [sz, i64] + [i32] * 6 + [vp]),
+    "sb_ml_workspace_bytes": (sz, [i64, i32]),
+    "sb_ofdm_ml": (i32, [vp] * 14 + [sz, i64] + [i32] * 12 + [vp]),
 }
 
 

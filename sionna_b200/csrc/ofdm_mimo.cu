@@ -19,8 +19,14 @@
 // round-trip test tolerance, test/unit/ofdm/test_ofdm.py:85-96).
 #include "sb_common.h"
 #include "lmmse_diag.cuh"
+#include "dense_mimo.cuh"
 
 namespace {
+
+using sb_dense::Scratch;
+using sb_dense::chol_lower;
+using sb_dense::whiten;
+using sb_dense::OfdmEqParams;
 
 // ---------------------------------------------------------------------------------------------------------------
 // Mixed-radix Stockham FFT in shared memory: one CTA transforms one length-N vector (ping-pong buffers, twiddle table
@@ -710,49 +716,11 @@ __global__ void interp_lin_kernel(const T* __restrict__ h, const int* __restrict
 
 // ---------------------------------------------------------------------------------------------------------------
 // Dense per-vector linear algebra, complex64, one thread per received vector; matrices live in shared memory interleaved
-// by thread (element e of thread t at [e * T + t]: conflict-free). The LMMSE kernels and the mimo_linalg modes are
-// compositions of these steps:
-//   chol_lower       L = chol(S), in place                                   (utils/linalg.py:28-32)
-//   whiten           y_w = L^-1 y, H_w = L^-1 H                              (mimo/utils.py:343-347)
+// by thread (Scratch, dense_mimo.cuh). The LMMSE kernels and the mimo_linalg modes are compositions of these steps:
+//   chol_lower, whiten                                                        (dense_mimo.cuh)
 //   tx_lmmse_matrix  G = (H^H H + I)^-1 H^H via chol + cholesky_solve        (mimo/equalization.py:95-97)
 //   lmmse_epilogue   x_hat = G y / diag(G H), no_eff = Re(1 / diag(G H) - 1)  (mimo/equalization.py:217-231)
 // ---------------------------------------------------------------------------------------------------------------
-struct Scratch {
-    float2* p;
-    int T, t;
-    __device__ __forceinline__ float2& operator()(int e) const { return p[(size_t)e * T + t]; }
-};
-
-// A = L L^H (lower, n x n), in place
-__device__ void chol_lower(const Scratch& A, int n) {
-    for (int j = 0; j < n; ++j) {
-        float d = A(j * n + j).x;
-        for (int k = 0; k < j; ++k) { float2 l = A(j * n + k); d -= l.x * l.x + l.y * l.y; }
-        d = sqrtf(d);
-        A(j * n + j) = make_float2(d, 0.f);
-        for (int i = j + 1; i < n; ++i) {
-            float2 v = A(i * n + j);
-            for (int k = 0; k < j; ++k) v = csub(v, cmulc(A(i * n + k), A(j * n + k)));
-            A(i * n + j) = make_float2(v.x / d, v.y / d);
-        }
-    }
-}
-
-// forward substitution with the Cholesky factor L (M x M), in place: Y = L^-1 Y (M), H = L^-1 H (M x K)
-__device__ void whiten(const Scratch& L, const Scratch& Y, const Scratch& H, int M, int K) {
-    for (int i = 0; i < M; ++i) {
-        float d = L(i * M + i).x;
-        float2 v = Y(i);
-        for (int k = 0; k < i; ++k) v = csub(v, cmul(L(i * M + k), Y(k)));
-        Y(i) = make_float2(v.x / d, v.y / d);
-        for (int c = 0; c < K; ++c) {
-            float2 w = H(i * K + c);
-            for (int k = 0; k < i; ++k) w = csub(w, cmul(L(i * M + k), H(k * K + c)));
-            H(i * K + c) = make_float2(w.x / d, w.y / d);
-        }
-    }
-}
-
 // solve (C C^H) x = b for one column, b_i = b(i), x_i in X(i * ldx + col); C lower triangular n x n
 template <typename BF>
 __device__ void chol_solve_col(const Scratch& C, int n, const BF& b, const Scratch& X, int ldx, int col) {
@@ -902,66 +870,25 @@ __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const
     }
 }
 
-// OFDMEqualizer + LMMSE fused. Per (b, rx, sym, sc):
-//   y    [B, RX, ANT, S, F]          (effective subcarriers only)
-//   hhat [B, RX, ANT, TXS, S, F]     TXS = num_tx * num_streams_per_tx
-//   ev   err_var with strides given by ev_stride[7] elements for dims (b, rx, ant, txs, s, f) (0 = broadcast)
-//   no   [B, RX, ANT] via no_stride (b, rx, ant)
-//   des [RX, K], und [RX, KU]: TXS indices of the desired / interfering streams of receiver rx
-//   out_ts [RX, K]: output stream row (tx*streams + st) after stream_ind re-ordering; data_pos [TXS, S*F]: position among
-//   the data symbols of that stream or -1 -> x_hat / no_eff [B, TXS, num_data]
-struct OfdmEqParams {
-    const float2* y; const float2* hhat; const float* ev; const float* no;
-    long long ev_stride[6]; long long no_stride[3];
-    const int* des; const int* und; const int* out_ts; const int* data_pos;
-    float2* xh; float* ne;
-    long long B; int RX, ANT, TXS, S, F, K, KU, ND;
-};
+// OFDMEqualizer + LMMSE fused (inputs and tables: OfdmEqParams, dense_mimo.cuh) -> x_hat / no_eff [B, TXS, num_data]
 __global__ void ofdm_lmmse_kernel(const OfdmEqParams p) {
     extern __shared__ float2 smem[];
     const int T = blockDim.x, t = threadIdx.x, M = p.ANT, K = p.K;
     const LmmseScratch w(smem, T, t, M, K);
     float2 xo[16];
     float no_e[16];
-    const long long SF = (long long)p.S * p.F;
-    const long long total = p.B * p.RX * SF;
+    const long long total = p.B * p.RX * (long long)p.S * p.F;
     for (long long i = (long long)blockIdx.x * T + t; i < total; i += (long long)gridDim.x * T) {
-        long long re = i % SF;
-        int rx = (int)((i / SF) % p.RX);
-        long long b = i / (SF * p.RX);
-        int s = (int)(re / p.F), f = (int)(re % p.F);
+        const sb_dense::OfdmRe e = sb_dense::ofdm_re(p, i);
         // skip resource elements that carry data for none of this receiver's streams
-        bool any = false;
-        for (int k = 0; k < K; ++k) any = any || p.data_pos[(size_t)p.out_ts[rx * K + k] * SF + re] >= 0;
-        if (!any) continue;
-        for (int m = 0; m < M; ++m) {
-            long long ybase = ((b * p.RX + rx) * M + m) * SF + re;
-            w.Y(m) = p.y[ybase];
-            long long hb = ((b * p.RX + rx) * M + m) * (long long)p.TXS;
-            for (int k = 0; k < K; ++k) w.H(m * K + k) = p.hhat[(hb + p.des[rx * K + k]) * SF + re];
-            // S = H_u H_u^H + diag(no) + diag(sum_txs err_var)   (equalization.py:205-218)
-            float evs = 0.f;
-            for (int q = 0; q < p.TXS; ++q)
-                evs += p.ev[b * p.ev_stride[0] + rx * p.ev_stride[1] + m * p.ev_stride[2] + q * p.ev_stride[3] +
-                            s * p.ev_stride[4] + f * p.ev_stride[5]];
-            float nn = p.no[b * p.no_stride[0] + rx * p.no_stride[1] + m * p.no_stride[2]];
-            for (int m2 = 0; m2 <= m; ++m2) {
-                float2 acc = make_float2(0.f, 0.f);
-                long long hb2 = ((b * p.RX + rx) * M + m2) * (long long)p.TXS;
-                for (int u = 0; u < p.KU; ++u)
-                    acc = cadd(acc, cmulc(p.hhat[(hb + p.und[rx * p.KU + u]) * SF + re],
-                                          p.hhat[(hb2 + p.und[rx * p.KU + u]) * SF + re]));
-                if (m2 == m) acc.x += nn + evs;
-                w.S(m * M + m2) = acc;
-            }
-        }
+        if (!sb_dense::ofdm_re_has_data(p, e)) continue;
+        sb_dense::ofdm_load_re(p, e, w.Y, w.H, w.S);
         lmmse_core(w, M, K, xo, no_e);
         for (int k = 0; k < K; ++k) {
-            int ts = p.out_ts[rx * K + k];
-            int dp = p.data_pos[(size_t)ts * SF + re];
-            if (dp >= 0) {
-                p.xh[(b * p.TXS + ts) * (long long)p.ND + dp] = xo[k];
-                p.ne[(b * p.TXS + ts) * (long long)p.ND + dp] = no_e[k];
+            const long long o = sb_dense::ofdm_out_index(p, e, k);
+            if (o >= 0) {
+                p.xh[o] = xo[k];
+                p.ne[o] = no_e[k];
             }
         }
     }
@@ -1365,18 +1292,7 @@ extern "C" int sb_pusch_ls_combine(float* d_h, float* d_err_var, int64_t rows, i
     return SB_OK;
 }
 
-// Threads per CTA of a thread-per-vector scratch kernel: per_thread bytes of shared memory each and at most cap bytes in
-// all. At most 128 and a multiple of 32 when a warp fits; otherwise the largest power of two that fits (16 ... 1), so
-// large matrices still run, at low occupancy. 0 if not even one thread fits.
-static int scratch_threads(size_t per_thread, size_t cap, size_t* smem) {
-    const int fit = (int)std::min<size_t>(128, cap / per_thread);
-    int t = fit / 32 * 32;
-    if (t == 0)
-        for (t = 16; t > fit; t /= 2) {}
-    if (t == 0) return 0;
-    *smem = per_thread * t;
-    return t;
-}
+using sb_dense::scratch_threads;
 constexpr size_t kLmmseSmemCap = 200 * 1024;
 
 extern "C" int sb_lmmse_equalize(const float* d_y, const float* d_h, const float* d_s, float* d_x_hat, float* d_no_eff,

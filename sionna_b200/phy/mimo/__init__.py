@@ -1,5 +1,5 @@
-"""MIMO (mirror of sionna.phy.mimo for the hot path): stream management, LMMSE equalisation, linear detection."""
+"""MIMO (mirror of sionna.phy.mimo for the hot path): stream management, LMMSE equalisation, linear and maximum-likelihood detection."""
 from .stream_management import StreamManagement
 from .equalization import lmmse_equalizer, lmmse_matrix
 from .utils import whiten_channel
-from .detection import LinearDetector
+from .detection import LinearDetector, MaximumLikelihoodDetector

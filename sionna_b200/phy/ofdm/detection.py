@@ -1,8 +1,15 @@
-"""OFDM MIMO detection (mirror of /root/reference/src/sionna/phy/ofdm/detection.py:20-317, 740-847): ``LinearDetector``
-= fused LMMSE equalisation (``sb_ofdm_lmmse``) + demapping with the per-symbol effective noise variance (``sb_demap``)."""
+"""OFDM MIMO detection (mirror of /root/reference/src/sionna/phy/ofdm/detection.py:20-847): ``LinearDetector``
+= fused LMMSE equalisation (``sb_ofdm_lmmse``) + demapping with the per-symbol effective noise variance (``sb_demap``);
+``MaximumLikelihoodDetector`` / ``MaximumLikelihoodDetectorWithPrior`` = fused covariance assembly + ML detection
+(``sb_ofdm_ml``)."""
+import numpy as np
+import torch
+
+from ..._lib import lib, check, ptr, current_stream
 from ..block import Block
 from ..mapping import Constellation, Demapper
-from .equalization import LMMSEEqualizer
+from ..mimo.detection import llrs_to_symbol_logits, ml_check_limits, ml_workspace
+from .equalization import LMMSEEqualizer, OFDMEqualizer
 
 
 class LinearDetector(Block):
@@ -32,3 +39,83 @@ class LinearDetector(Block):
     def call(self, y, h_hat, err_var, no):
         x_hat, no_eff = self._equalizer(y, h_hat, err_var, no)
         return self._demapper(x_hat, no_eff)
+
+
+class MaximumLikelihoodDetector(Block):
+    """MaximumLikelihoodDetector(output, demapping_method, resource_grid, stream_management, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None)
+
+    ML detection for OFDM MIMO (detection.py:524-647) on the fused ``sb_ofdm_ml`` kernel: the interference-plus-noise
+    covariance of every resource element is assembled on chip from ``OFDMEqualizer``'s stream tables, then every
+    candidate vector of the receiver's streams is scored as in ``mimo.MaximumLikelihoodDetector``.
+    ``call(y, h_hat, err_var, no)`` -> ``[batch, num_tx, num_streams, num_data_symbols*num_bits_per_symbol]`` LLRs / hard
+    bits (``output="bit"``), ``[batch, num_tx, num_streams, num_data_symbols, num_points]`` logits or
+    ``[batch, num_tx, num_streams, num_data_symbols]`` int32 indices (``output="symbol"``)."""
+
+    def __init__(self, output, demapping_method, resource_grid, stream_management, constellation_type=None,
+                 num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None, **kwargs):
+        super().__init__(precision=precision, **kwargs)
+        assert output in ("bit", "symbol"), "Unknown output"
+        assert demapping_method in ("app", "maxlog"), "Unknown demapping method"
+        self._output = output
+        self._method = 0 if demapping_method == "app" else 1
+        self._hard_out = bool(hard_out)
+        self._constellation = Constellation.check_or_create(constellation_type=constellation_type,
+                                                            num_bits_per_symbol=num_bits_per_symbol,
+                                                            constellation=constellation, precision=precision)
+        ml_check_limits(stream_management.num_streams_per_rx, self._constellation.num_points)
+        self._eq = OFDMEqualizer("lmmse", resource_grid, stream_management, precision=precision)
+
+    @property
+    def constellation(self):
+        return self._constellation
+
+    def call(self, y, h_hat, err_var, no):
+        return self._detect(y, h_hat, None, err_var, no)
+
+    def _detect(self, y, h_hat, prior, err_var, no):
+        eq = self._eq
+        rg, sm = eq._resource_grid, eq._stream_management
+        dev = self.device
+        y_eff, h, ev, ev_st, no_t, no_st = eq._kernel_inputs(y, h_hat, err_var, no)
+        b, rx, ant, s_, f_ = y_eff.shape
+        txs = sm.num_tx * sm.num_streams_per_tx
+        des, und, out_ts, data_pos = eq._tables(dev)
+        nd = rg.pilot_pattern.num_data_symbols
+        m = self._constellation.num_bits_per_symbol
+        npts = 2 ** m
+        pr = None
+        if prior is not None:
+            pr = torch.as_tensor(prior).to(device=dev, dtype=torch.float32)
+            if self._output == "bit":
+                pr = llrs_to_symbol_logits(pr.reshape(b, txs, nd, m), m)
+            pr = pr.reshape(b, txs, nd, npts).contiguous()
+        shp = [b, sm.num_tx, sm.num_streams_per_tx]
+        if self._output == "bit":
+            out = torch.zeros(shp + [nd * m], dtype=torch.float32, device=dev)
+        elif self._hard_out:
+            out = torch.zeros(shp + [nd], dtype=torch.int32, device=dev)
+        else:
+            out = torch.zeros(shp + [nd, npts], dtype=torch.float32, device=dev)
+        pts = self._constellation().to(device=dev, dtype=torch.complex64).contiguous()
+        ev_arr = np.asarray(ev_st, np.int64)                    # host stride arrays: alive until the call returns
+        no_arr = np.asarray(no_st, np.int64)
+        ws = ml_workspace(b * rx * s_ * f_, sm.num_streams_per_rx, dev)
+        check(lib().sb_ofdm_ml(ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
+                               ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos), ptr(pr), ptr(pts), ptr(out),
+                               ptr(ws), ws.numel(), b, rx, ant, txs, s_, f_,
+                               sm.num_streams_per_rx, sm.num_interfering_streams_per_rx, nd, npts, self._method,
+                               int(self._output == "symbol"), int(self._hard_out), current_stream()), "sb_ofdm_ml")
+        return out
+
+
+class MaximumLikelihoodDetectorWithPrior(MaximumLikelihoodDetector):
+    """MaximumLikelihoodDetectorWithPrior(output, demapping_method, resource_grid, stream_management, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None)
+
+    ``MaximumLikelihoodDetector`` with prior knowledge of the transmitted signals (detection.py:650-738):
+    ``call(y, h_hat, prior, err_var, no)``, ``prior`` = bit LLRs ``[batch, num_tx, num_streams,
+    num_data_symbols*num_bits_per_symbol]`` (``output="bit"``) or point logits ``[batch, num_tx, num_streams,
+    num_data_symbols, num_points]`` (``output="symbol"``). Stream k of a receiver takes the prior of the transmitted
+    stream it detects."""
+
+    def call(self, y, h_hat, prior, err_var, no):
+        return self._detect(y, h_hat, prior, err_var, no)

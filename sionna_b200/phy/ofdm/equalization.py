@@ -64,6 +64,28 @@ class OFDMEqualizer(Block):
             raise NotImplementedError("OFDM equalisation runs complex64 kernels only.")
         rg, sm = self._resource_grid, self._stream_management
         dev = self.device
+        y_eff, h, ev, ev_st, no_t, no_st = self._kernel_inputs(y, h_hat, err_var, no)
+        b, rx, ant, s_, f_ = y_eff.shape
+        txs = sm.num_tx * sm.num_streams_per_tx
+        des, und, out_ts, data_pos = self._tables(dev)
+        nd = rg.pilot_pattern.num_data_symbols
+        if self._equalizer != "lmmse":
+            return self._unfused(y_eff, h, ev, ev_st, no_t, no_st)
+        x_hat = torch.zeros((b, sm.num_tx, sm.num_streams_per_tx, nd), dtype=torch.complex64, device=dev)
+        no_eff = torch.zeros((b, sm.num_tx, sm.num_streams_per_tx, nd), dtype=torch.float32, device=dev)
+        ev_arr = (np.asarray(ev_st, np.int64))
+        no_arr = (np.asarray(no_st, np.int64))
+        check(lib().sb_ofdm_lmmse(ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
+                                  ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos), ptr(x_hat), ptr(no_eff),
+                                  b, rx, ant, txs, s_, f_, sm.num_streams_per_rx, sm.num_interfering_streams_per_rx, nd,
+                                  current_stream()), "sb_ofdm_lmmse")
+        return x_hat, no_eff
+
+    def _kernel_inputs(self, y, h_hat, err_var, no):
+        """The fused kernels' inputs: y [B, rx, ant, S, F] without nulled subcarriers, h [B, rx, ant, txs, S, F] and
+        err_var / no as contiguous tensors with their broadcast strides (0 on broadcast dims)."""
+        sm = self._stream_management
+        dev = self.device
         y_eff = self._removed_nulled_scs(y).to(torch.complex64).contiguous()          # [B, rx, ant, S, F]
         b, rx, ant, s_, f_ = y_eff.shape
         txs = sm.num_tx * sm.num_streams_per_tx
@@ -78,19 +100,7 @@ class OFDMEqualizer(Block):
         no_t = torch.as_tensor(no).to(device=dev, dtype=torch.float32)
         no_t = no_t.reshape(list(no_t.shape) + [1] * (3 - no_t.dim()))                 # expand_to_rank(no, 3, -1)
         no_t, no_st = _strides_for(no_t, [b, rx, ant])
-        des, und, out_ts, data_pos = self._tables(dev)
-        nd = rg.pilot_pattern.num_data_symbols
-        if self._equalizer != "lmmse":
-            return self._unfused(y_eff, h, ev, ev_st, no_t, no_st)
-        x_hat = torch.zeros((b, sm.num_tx, sm.num_streams_per_tx, nd), dtype=torch.complex64, device=dev)
-        no_eff = torch.zeros((b, sm.num_tx, sm.num_streams_per_tx, nd), dtype=torch.float32, device=dev)
-        ev_arr = (np.asarray(ev_st, np.int64))
-        no_arr = (np.asarray(no_st, np.int64))
-        check(lib().sb_ofdm_lmmse(ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
-                                  ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos), ptr(x_hat), ptr(no_eff),
-                                  b, rx, ant, txs, s_, f_, sm.num_streams_per_rx, sm.num_interfering_streams_per_rx, nd,
-                                  current_stream()), "sb_ofdm_lmmse")
-        return x_hat, no_eff
+        return y_eff, h, ev, ev_st, no_t, no_st
 
     def _unfused(self, y_eff, h, ev, ev_st, no_t, no_st):
         """Generic equaliser callable: materialise y [B,rx,S,F,M], H [..,M,K], S [..,M,M] as the reference does
