@@ -138,12 +138,13 @@ __device__ __forceinline__ unsigned ldw(const float* q) { return __float_as_uint
 __device__ __forceinline__ void stw(float* q, unsigned w) { *q = __uint_as_float(w); }
 
 // Plain variant: every edge is evaluated. One vote per check on its first edge pair probes for saturation and raises
-// *sat_flag, which makes the CTA use the voting variant cn_phi_qc_sc from the next iteration on.
-// Out of line on purpose (both variants): the five degree classes then share ONE copy of each variant's loops (the
+// *sat_flag, which makes the CTA run the voting pass (cn_vote_pass) from the next iteration on.
+// Out of line on purpose (both this and cn_vote_row): the five degree classes then share ONE copy of the loops (the
 // kernel is bound by instruction fetch as much as by issue: 12.35 -> 11.85 ms per 4096 codewords at 2 dB; making phi
-// itself a call costs more than it saves, 12.8 ms). Two edge pairs per loop trip.
+// itself a call costs more than it saves, 12.8 ms). Two edge pairs per loop trip. The log table is passed by value, so
+// its lane offset stays in a register instead of going through the stack.
 template <class LT>
-__device__ __noinline__ void cn_phi_qc(float* pm, int Z, int deg, float clip, int* sat_flag, const LT& lt) {
+__device__ __noinline__ void cn_phi_qc(float* pm, int Z, int deg, float clip, int* sat_flag, LT lt) {
     const unsigned am = __activemask();                   // lanes of this warp working on the same block row
     float P = 0.f;
     unsigned par = 0;
@@ -179,39 +180,40 @@ __device__ __noinline__ void cn_phi_qc(float* pm, int Z, int deg, float clip, in
     if (l < deg) stw(pm + l * Z, phi_pass2(ldw(pm + l * Z), P, par, clip, lt));
 }
 
-// Voting variant (deg <= 32), for the iterations after the probe saw a saturated pair. One read pass builds the row's
-// union mask U: bit l is set if |x_l| < SB_PHI_ZERO in any lane of the warp. U is warp-uniform, and only its k positions
-// are evaluated:
+// Voting variant (deg <= 32), for the iterations after the probe saw a saturated pair. A read pass (cn_vote_pass) builds
+// the row's union mask U: bit l is set if |x_l| < SB_PHI_ZERO in any lane of the warp. U is warp-uniform, and only its
+// k positions are evaluated:
 //   * U holds no edge but the last (the common row once a codeword has converged): every other edge has phi = +0 (1),
 //     so P = p_last exactly; those edges get phi(P) and the last edge phi(P - p_last) = phi(+0) = phi_max (3). Two phi
 //     per row.
-//   * otherwise, walking U in ascending order two at a time: phi(|x_l|) for l in U, summed into P in that order. A
-//     position outside U has phi = +0 in every lane (1), and P + (+0) == P, so P is bit-identical to the sum over all
-//     edges in ascending VN order. Then phi(P - p_l) for l in U, each lane on its own values: where (2) or (3) holds
-//     the evaluation itself gives what the rule gives (-0 + P == P; the clamp of phi maps P - p_l <= 8.5e-8 to
-//     phi_max). Every position outside U gets phi(P - 0) = phi(P), evaluated once. 2k + 1 phi per row.
+//   * otherwise (cn_vote_row), walking U in ascending order two at a time: phi(|x_l|) for l in U, summed into P in
+//     that order. A position outside U has phi = +0 in every lane (1), and P + (+0) == P, so P is bit-identical to the
+//     sum over all edges in ascending VN order. Then phi(P - p_l) for l in U, each lane on its own values: where (2) or
+//     (3) holds the evaluation itself gives what the rule gives (-0 + P == P; the clamp of phi maps P - p_l <= 8.5e-8
+//     to phi_max). Every position outside U gets phi(P - 0) = phi(P), evaluated once. 2k + 1 phi per row.
+// Outputs outside U take their sign from the lane's sign mask S (bit l = sign of x_l), so those edges are written
+// without being read again; the row's sign parity is popc(S) & 1.
+__device__ __forceinline__ unsigned vote_sign(unsigned S, int l, unsigned par) { return ((S >> l) << 31) ^ par; }
+
+// outputs of a row whose U holds no edge but the last: y on every other edge, ylast on the last one
+__device__ __forceinline__ void vote_store_fast(float* pm, int Z, int deg, unsigned S, unsigned y, unsigned ylast) {
+    const unsigned par = (unsigned)__popc(S) << 31;
+    for (int l = 0; l < deg - 1; ++l) stw(pm + l * Z, y | vote_sign(S, l, par));
+    stw(pm + (deg - 1) * Z, ylast | vote_sign(S, deg - 1, par));
+}
+
+// One voting row, given its union mask U and this lane's sign mask S: a row whose U holds no edge but the last
+// evaluates its two phi, any other row the 2k + 1 walk. `last` holds the bits of x_{deg-1}, ylast the output magnitude
+// of the last edge of a two-phi row.
 template <class LT>
-__device__ __noinline__ void cn_phi_qc_sc(float* pm, int Z, int deg, float clip, float phi_max, const LT& lt) {
-    unsigned par = 0, own = 0;
-    for (int l = 0; l < deg; ++l) {
-        const unsigned b = __float_as_uint(pm[l * Z]);
-        par ^= b;
-        own |= (fabsf(__uint_as_float(b)) < SB_PHI_ZERO ? 1u : 0u) << l;
-    }
-    par &= 0x80000000u;
-    const unsigned U = __reduce_or_sync(__activemask(), own);
-    if (!(U & ((1u << (deg - 1)) - 1u))) {
-        float* ql = pm + (deg - 1) * Z;
-        const unsigned bl = __float_as_uint(*ql);
-        const float pl = sb_phif_s(__uint_as_float(bl & 0x7fffffffu), lt);
-        const unsigned y = __float_as_uint(fminf(sb_phif_s(pl, lt), clip));
-        for (int l = 0; l + 1 < deg; ++l) {
-            float* q = pm + l * Z;
-            *q = __uint_as_float(y | ((__float_as_uint(*q) ^ par) & 0x80000000u));
-        }
-        *ql = __uint_as_float(__float_as_uint(fminf(phi_max, clip)) | ((bl ^ par) & 0x80000000u));
+__device__ __noinline__ void cn_vote_row(float* pm, int Z, int deg, unsigned U, unsigned S, unsigned last, float clip,
+                                         unsigned ylast, LT lt) {
+    if (!(U & ~(1u << (deg - 1)))) {
+        const float pl = sb_phif_s(__uint_as_float(last & 0x7fffffffu), lt);
+        vote_store_fast(pm, Z, deg, S, __float_as_uint(fminf(sb_phif_s(pl, lt), clip)), ylast);
         return;
     }
+    const unsigned par = (unsigned)__popc(S) << 31;
     float P = 0.f;
     unsigned u = U;
     for (; u & (u - 1); u &= u - 1) {                     // two or more positions left: the lowest two
@@ -230,8 +232,8 @@ __device__ __noinline__ void cn_phi_qc_sc(float* pm, int Z, int deg, float clip,
     if (rest) {
         const unsigned y = __float_as_uint(fminf(sb_phif_s(P, lt), clip));
         for (unsigned r = rest; r; r &= r - 1) {
-            float* q = pm + (__ffs(r) - 1) * Z;
-            *q = __uint_as_float(y | ((__float_as_uint(*q) ^ par) & 0x80000000u));
+            const int l = __ffs(r) - 1;
+            stw(pm + l * Z, y | vote_sign(S, l, par));
         }
     }
     for (u = U; u & (u - 1); u &= u - 1) {
@@ -290,12 +292,9 @@ __device__ __forceinline__ bool cn_phi_reg_of(float* pm, int Z, int deg, float c
     return ((deg == DS && (cn_phi_qc_reg<DS, LT>(pm, Z, clip, sat_flag, lt), true)) || ...);
 }
 
-// The voting variant takes rows of up to 32 edges (one mask bit per edge); heavier rows (class 0 only, none in the 5G
-// base graphs) run the plain variant, whose probe then re-raises the already raised flag.
+// the plain variant of a row of class CLS
 template <int CLS, class LT>
-__device__ __forceinline__ void cn_phi_dispatch(float* pm, int Z, int deg, float clip, float phi_max, bool sc,
-                                                int* sat_flag, const LT& lt) {
-    if (sc && (CLS > 0 || deg <= 32)) { cn_phi_qc_sc<LT>(pm, Z, deg, clip, phi_max, lt); return; }
+__device__ __forceinline__ void cn_phi_dispatch(float* pm, int Z, int deg, float clip, int* sat_flag, const LT& lt) {
     if (CLS == 4 && cn_phi_reg_of<LT, 3, 4>(pm, Z, deg, clip, sat_flag, lt)) return;
     if (CLS == 3 && cn_phi_reg_of<LT, 5, 6, 7, 8>(pm, Z, deg, clip, sat_flag, lt)) return;
     cn_phi_qc<LT>(pm, Z, deg, clip, sat_flag, lt);
@@ -366,10 +365,9 @@ __device__ __forceinline__ void cn_minsum_qc_loop(float* pm, int Z, int deg, flo
 }
 
 template <int RULE, int CLS, class LT>
-__device__ __forceinline__ void cn_qc(float* pm, int Z, int deg, float clip, float offset, float phi_max, bool sc,
-                                      int* sat_flag, const LT& lt) {
+__device__ __forceinline__ void cn_qc(float* pm, int Z, int deg, float clip, float offset, int* sat_flag, const LT& lt) {
     if constexpr (RULE == SB_CN_BOXPLUS_PHI) {
-        cn_phi_dispatch<CLS, LT>(pm, Z, deg, clip, phi_max, sc, sat_flag, lt);
+        cn_phi_dispatch<CLS, LT>(pm, Z, deg, clip, sat_flag, lt);
     } else if constexpr (RULE == SB_CN_BOXPLUS) {
         cn_tanh(StrideEdges{pm, Z}, deg, clip);
     } else {
@@ -520,27 +518,102 @@ __device__ __forceinline__ int first_of(int start, int start_mod, const WarpCtx&
     return start + (w.grp - start_mod + (w.grp < start_mod ? w.G : 0));
 }
 
+// The row's last edge goes to a degree-1 VN (row_info.w = fw >= 0): apply that VN's update right here
+// (decoding.py:714-729 with the single incoming message c2v, the edge's new value at q) so the VN phase can skip the column
+__device__ __forceinline__ void fused_vn(const QcParams& p, float* q, float c2v, int fw, int lane_i, const float* llr_s,
+                                         float clip, unsigned char* hd) {
+    int s = fw >> 16, vb = fw & 0xffff;                   // shift, column index
+    int j = lane_i + s;
+    j -= (j >= p.Z) ? p.Z : 0;
+    float x_tot = __fadd_rn(__fadd_rn(0.f, c2v), llr_s[vb * p.Z + j]);
+    *q = clipf(__fadd_rn(-c2v, x_tot), clip);
+    if (hd) hd[vb * p.Z + j] = 0.f >= x_tot ? 1 : 0;
+}
+
 template <int RULE, int CLS, class LT>
 __device__ __forceinline__ void cn_class(const QcParams& p, const WarpCtx& w, float* msg, const float* llr_s,
-                                         const int4* s_row, int start, int end, float clip, bool fuse,
-                                         float phi_max, bool sc, int* sat_flag, const LT& lt, unsigned char* hd) {
+                                         const int4* s_row, int start, int end, float clip, bool fuse, int* sat_flag,
+                                         const LT& lt, unsigned char* hd) {
     for (int rr = first_of(start, p.row_cls_mod[CLS], w); rr < end; rr += w.G) {
         int4 ri = s_row[rr];
         if (w.lane_i < ri.z) {
             float* pm = msg + ri.x * p.Z + w.lane_i;
-            cn_qc<RULE, CLS, LT>(pm, p.Z, ri.y, clip, p.offset, phi_max, sc, sat_flag, lt);
+            cn_qc<RULE, CLS, LT>(pm, p.Z, ri.y, clip, p.offset, sat_flag, lt);
             if (fuse && ri.w >= 0) {
-                // the row's last edge goes to a degree-1 VN: apply that VN's update right here (decoding.py:714-729
-                // with a single incoming message) so the VN phase can skip the column
-                int s = ri.w >> 16, vb = ri.w & 0xffff;     // shift, column index
-                int j = w.lane_i + s;
-                j -= (j >= p.Z) ? p.Z : 0;
                 float* q = pm + (ri.y - 1) * p.Z;
-                float c2v = *q;
-                float x_tot = __fadd_rn(__fadd_rn(0.f, c2v), llr_s[vb * p.Z + j]);
-                *q = clipf(__fadd_rn(-c2v, x_tot), clip);
-                if (hd) hd[vb * p.Z + j] = 0.f >= x_tot ? 1 : 0;
+                fused_vn(p, q, *q, ri.w, w.lane_i, llr_s, clip, hd);
             }
+        }
+    }
+}
+
+template <int RULE, class LT>
+__device__ __forceinline__ void cn_all(const QcParams& p, const WarpCtx& w, float* msg, const float* llr_s,
+                                       const int4* s_row, float clip, bool fuse, int* sat_flag, const LT& lt,
+                                       unsigned char* hd) {
+    const int* re = p.row_cls_end;
+    cn_class<RULE, 0, LT>(p, w, msg, llr_s, s_row, 0, re[0], clip, fuse, sat_flag, lt, hd);
+    cn_class<RULE, 1, LT>(p, w, msg, llr_s, s_row, re[0], re[1], clip, fuse, sat_flag, lt, hd);
+    cn_class<RULE, 2, LT>(p, w, msg, llr_s, s_row, re[1], re[2], clip, fuse, sat_flag, lt, hd);
+    cn_class<RULE, 3, LT>(p, w, msg, llr_s, s_row, re[2], re[3], clip, fuse, sat_flag, lt, hd);
+    cn_class<RULE, 4, LT>(p, w, msg, llr_s, s_row, re[3], re[4], clip, fuse, sat_flag, lt, hd);
+}
+
+// One row slice of the voting pass: its edges pm[0], pm[Z], ..., whether this lane holds a check of it, and the lane's
+// bits of the row's masks (bit l: |x_l| < SB_PHI_ZERO in own, sign of x_l in S)
+struct VoteRow {
+    float* pm;
+    int deg;                                              // 0: a row of more than 32 edges (plain variant)
+    bool act;
+    unsigned own, S, last;                                // last: bits of x_{deg-1}
+};
+
+__device__ __forceinline__ VoteRow vote_row(float* msg, int4 ri, const WarpCtx& w, int Z) {
+    VoteRow r;
+    r.pm = msg + ri.x * Z + w.lane_i;
+    r.deg = ri.y <= 32 ? ri.y : 0;
+    r.act = w.lane_i < ri.z && r.deg > 0;
+    r.own = r.S = r.last = 0;
+    if (r.act) {                                          // the last edge first: the masks are built from the top bit down
+        r.last = ldw(r.pm + (r.deg - 1) * Z);
+        r.own = fabsf(__uint_as_float(r.last)) < SB_PHI_ZERO ? 1u : 0u;
+        r.S = r.last >> 31;
+    }
+    return r;
+}
+
+// edge l (at pm[o], o = l * Z) of a row, l < deg - 1, descending
+__device__ __forceinline__ void vote_read(VoteRow& r, int l, int o) {
+    if (r.act && l < r.deg - 1) {
+        const unsigned b = ldw(r.pm + o);
+        r.own = __funnelshift_l(fabsf(__uint_as_float(b)) < SB_PHI_ZERO ? 0x80000000u : 0u, r.own, 1);
+        r.S = __funnelshift_l(b, r.S, 1);
+    }
+}
+
+// CN phase of the voting iterations: the warp's rows (rr = grp, grp + G, ...; the same rows as the class loops of
+// cn_all), class-agnostic: an inline read pass and the union mask, then cn_vote_row out of line. Rows of more than 32
+// edges (none in the 5G base graphs) run the plain variant, whose probe then re-raises the already raised flag. A lane
+// outside a row (lane_i >= zrow) reads nothing, adds nothing to the row's union mask and stores nothing into it.
+// Taking two rows per trip, with the phi of two converged rows as one phi pair, measured no faster at 2 dB and slower
+// at 0 dB and with early termination (H100 80GB HBM3, 700 W): 12.68-12.70 against 12.65-12.67 ms, 16.72-16.74 against
+// 16.55-16.57 ms, 10.69-10.71 against 10.53-10.54 ms.
+template <class LT>
+__device__ __forceinline__ void cn_vote_pass(const QcParams& p, const WarpCtx& w, float* msg, const float* llr_s,
+                                             const int4* s_row, float clip, bool fuse, float phi_max, int* sat_flag,
+                                             const LT& lt, unsigned char* hd) {
+    const int Z = p.Z;
+    const unsigned ylast = __float_as_uint(fminf(phi_max, clip));
+    for (int rr = w.grp; rr < p.n_rows; rr += w.G) {
+        const int4 ri = s_row[rr];
+        VoteRow r = vote_row(msg, ri, w, Z);
+        for (int l = r.deg - 2, o = l * Z; l >= 0; --l, o -= Z) vote_read(r, l, o);
+        const unsigned U = __reduce_or_sync(0xffffffffu, r.own);
+        if (r.act) cn_vote_row<LT>(r.pm, Z, r.deg, U, r.S, r.last, clip, ylast, lt);
+        if (ri.y > 32 && w.lane_i < ri.z) cn_phi_qc<LT>(r.pm, Z, ri.y, clip, sat_flag, lt);
+        if (fuse && ri.w >= 0 && w.lane_i < ri.z) {
+            float* q = r.pm + (ri.y - 1) * Z;
+            fused_vn(p, q, *q, ri.w, w.lane_i, llr_s, clip, hd);
         }
     }
 }
@@ -685,12 +758,12 @@ __global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_
             if (final_pass && tid == 0 && p.use_tma && b + gridDim.x < p.B)   // pull the next codeword's logits into L2 early
                 asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.llr + (size_t)(b + gridDim.x) * p.n_in),
                              "r"((uint32_t)p.n_in * 4u) : "memory");
-            const int* re = p.row_cls_end;
-            cn_class<RULE, 0, LogTab<REP>>(p, w, msg, llr_s, s_row, 0, re[0], clip, !final_pass, phi_max, sc, sat_flag, lt, hd);
-            cn_class<RULE, 1, LogTab<REP>>(p, w, msg, llr_s, s_row, re[0], re[1], clip, !final_pass, phi_max, sc, sat_flag, lt, hd);
-            cn_class<RULE, 2, LogTab<REP>>(p, w, msg, llr_s, s_row, re[1], re[2], clip, !final_pass, phi_max, sc, sat_flag, lt, hd);
-            cn_class<RULE, 3, LogTab<REP>>(p, w, msg, llr_s, s_row, re[2], re[3], clip, !final_pass, phi_max, sc, sat_flag, lt, hd);
-            cn_class<RULE, 4, LogTab<REP>>(p, w, msg, llr_s, s_row, re[3], re[4], clip, !final_pass, phi_max, sc, sat_flag, lt, hd);
+            if constexpr (RULE == SB_CN_BOXPLUS_PHI) {
+                if (sc) cn_vote_pass(p, w, msg, llr_s, s_row, clip, !final_pass, phi_max, sat_flag, lt, hd);
+                else cn_all<RULE>(p, w, msg, llr_s, s_row, clip, !final_pass, sat_flag, lt, hd);
+            } else {
+                cn_all<RULE>(p, w, msg, llr_s, s_row, clip, !final_pass, sat_flag, lt, hd);
+            }
             __syncthreads();
             // ---- VN phase ---------------------------------------------------------------------------------------
             vn_all<0, true>(p, w, msgb, llr_s, s_col, s_ce, clip, final_pass, final_pass, b, hd);
