@@ -101,9 +101,17 @@ def stream_management(assoc, num_streams_per_tx):
 
 
 # ---- LS estimation and interpolation ---------------------------------------------------------------------------------
-def ls_estimate(y_eff, mask, pilots, no):
+def _real(dtype):
+    return np.finfo(dtype).dtype.type
+
+
+def ls_estimate(y_eff, mask, pilots, no, dtype=None):
     """y_eff [B, rx, ant, S, F]; mask [tx, st, S, F]; pilots [tx, st, P]; no broadcastable to [B, rx, ant] ->
-    h, err [B, rx, ant, tx, st, P] (channel_estimation.py:138-150, 257-285)."""
+    h, err [B, rx, ant, tx, st, P] (channel_estimation.py:138-150, 257-285). ``dtype`` (np.complex64 / np.complex128)
+    evaluates in that precision; None keeps the inputs' types for h and float64 for err."""
+    if dtype is not None:
+        y_eff, pilots = np.asarray(y_eff).astype(dtype), np.asarray(pilots).astype(dtype)
+    rdt = np.float64 if dtype is None else _real(dtype)
     b, rx, ant = y_eff.shape[:3]
     p = pilots.shape[-1]
     yf = y_eff.reshape(b, rx, ant, -1)
@@ -111,14 +119,17 @@ def ls_estimate(y_eff, mask, pilots, no):
     yp = yf[..., pil_ind]                                            # [B, rx, ant, tx, st, P]
     with np.errstate(divide="ignore", invalid="ignore"):
         h = np.where(pilots == 0, 0, yp / pilots)
-        no_b = np.broadcast_to(np.asarray(no, np.float64).reshape(np.shape(no) + (1,) * (3 - np.ndim(no))), (b, rx, ant))
+        no_b = np.broadcast_to(np.asarray(no, rdt).reshape(np.shape(no) + (1,) * (3 - np.ndim(no))), (b, rx, ant))
         err = np.where(pilots == 0, 0, no_b[..., None, None, None] / np.abs(pilots) ** 2)
     return h, np.broadcast_to(err, h.shape)
 
 
-def nn_interp(x, mask, pilots):
-    """x [..., tx, st, P] -> [..., tx, st, S, F]: nearest non-zero pilot in Manhattan distance (:384-402)."""
+def nn_interp(x, mask, pilots, dtype=None):
+    """x [..., tx, st, P] -> [..., tx, st, S, F]: nearest non-zero pilot in Manhattan distance (:384-402), in ``dtype``
+    (None: the type of x)."""
     tx, st, s_, f_ = mask.shape
+    if dtype is not None:
+        x = np.asarray(x).astype(dtype)
     out = np.zeros(x.shape[:-1] + (s_, f_), x.dtype)
     for i in range(tx):
         for j in range(st):
@@ -137,11 +148,14 @@ def _lerp(x, x0, x1, y0, y1):
     return (x - x0) * slope + y0
 
 
-def lin_interp(x, mask, pilots, time_avg=False):
+def lin_interp(x, mask, pilots, time_avg=False, dtype=np.complex128):
     """x [..., tx, st, P] -> [..., tx, st, S, F] (channel_estimation.py:522-734): per pilot-carrying symbol, linear
-    inter/extrapolation over frequency from the two bracketing (or nearest two) non-zero pilots, then the same over time."""
+    inter/extrapolation over frequency from the two bracketing (or nearest two) non-zero pilots, then the same over time.
+    Evaluated in ``dtype`` (positions and slopes in its real type)."""
     tx, st, s_, f_ = mask.shape
-    out = np.zeros(x.shape[:-1] + (s_, f_), np.complex128)
+    rdt = _real(dtype)
+    x = np.asarray(x).astype(dtype)
+    out = np.zeros(x.shape[:-1] + (s_, f_), dtype)
     for i in range(tx):
         for j in range(st):
             pil = pilots[i, j]
@@ -152,7 +166,7 @@ def lin_interp(x, mask, pilots, time_avg=False):
                 if not idx:
                     continue
                 xs = np.array([pos[k][1] for k in idx])
-                row = np.zeros(x.shape[:-1][:-2] + (f_,), np.complex128)
+                row = np.zeros(x.shape[:-1][:-2] + (f_,), dtype)
                 for c in range(f_):
                     if len(idx) == 1:
                         k0 = k1 = 0
@@ -160,7 +174,7 @@ def lin_interp(x, mask, pilots, time_avg=False):
                         k1 = int(np.searchsorted(xs, c, side="left"))          # first pilot position >= c
                         k1 = min(max(k1, 1), len(idx) - 1)
                         k0 = k1 - 1
-                    row[..., c] = _lerp(c, xs[k0], xs[k1], x[..., i, j, idx[k0]], x[..., i, j, idx[k1]])
+                    row[..., c] = _lerp(rdt(c), rdt(xs[k0]), rdt(xs[k1]), x[..., i, j, idx[k0]], x[..., i, j, idx[k1]])
                 hf[a] = row
             syms = sorted(hf)
             if time_avg:
@@ -173,7 +187,7 @@ def lin_interp(x, mask, pilots, time_avg=False):
                     k1 = int(np.searchsorted(syms, a, side="left"))
                     k1 = min(max(k1, 1), len(syms) - 1)
                     k0 = k1 - 1
-                    out[..., i, j, a, :] = _lerp(a, syms[k0], syms[k1], hf[syms[k0]], hf[syms[k1]])
+                    out[..., i, j, a, :] = _lerp(rdt(a), rdt(syms[k0]), rdt(syms[k1]), hf[syms[k0]], hf[syms[k1]])
     return out
 
 

@@ -158,3 +158,36 @@ def test_linear_interpolator_random_channels_vs_independent_recipe(pilot_syms, t
             want = np.stack([_interp1_with_linear_extrapolation(sq, sorted(rows), np.array([rows[s][c] for s in sorted(rows)]))
                              for c in range(f_)], axis=1)
             assert np.allclose(out[b, tx, 0], want, atol=1e-12), (b, tx)
+
+
+@pytest.mark.parametrize("interp", ["nn", "lin", "lin_time_avg"])
+def test_ls_and_interpolation_in_complex64_equal_complex128_to_fp32_rounding(interp):
+    """oracle.ofdm.ls_estimate / nn_interp / lin_interp with dtype=np.complex64 evaluate the same sequence in single
+    precision (the yardstick the fused front-end's GPU tests measure against): results stay complex64 / float32 and sit
+    within fp32 rounding of the complex128 evaluation; the default dtype keeps the complex128 results bit for bit."""
+    rng = np.random.default_rng(7)
+    mask = F.kronecker_mask(2, 1, 14, 24, [2, 7, 11])
+    pil = np.zeros((2, 1, 3, 24), np.complex64)
+    pil[0, 0, :, 0::2] = (1 + 1j) / np.sqrt(2)
+    pil[1, 0, :, 1::2] = (1 - 1j) / np.sqrt(2)
+    pil = pil.reshape(2, 1, -1)
+    y = (rng.normal(size=(3, 1, 2, 14, 24)) + 1j * rng.normal(size=(3, 1, 2, 14, 24))).astype(np.complex64)
+    no = rng.uniform(0.01, 0.1, size=(3, 1, 2)).astype(np.float32)
+    h64, e64 = F.ls_estimate(y.astype(np.complex128), mask, pil, no.astype(np.float64), dtype=np.complex128)
+    h32, e32 = F.ls_estimate(y, mask, pil, no, dtype=np.complex64)
+    assert h32.dtype == np.complex64 and e32.dtype == np.float32 and h64.dtype == np.complex128 and e64.dtype == np.float64
+    h0, e0 = F.ls_estimate(y.astype(np.complex128), mask, pil.astype(np.complex128), no)   # default: as before
+    assert np.array_equal(h0, h64) and np.array_equal(e0, e64)
+    if interp == "nn":
+        r64, r32 = F.nn_interp(h64, mask, pil), F.nn_interp(h32, mask, pil, dtype=np.complex64)
+        q64, q32 = F.nn_interp(e64, mask, pil), F.nn_interp(e32, mask, pil, dtype=np.float32)
+    else:
+        ta = interp == "lin_time_avg"
+        r64, r32 = F.lin_interp(h64, mask, pil, ta), F.lin_interp(h32, mask, pil, ta, dtype=np.complex64)
+        q64, q32 = F.lin_interp(e64, mask, pil, ta).real, F.lin_interp(e32, mask, pil, ta, dtype=np.complex64).real
+        assert np.array_equal(F.lin_interp(h64, mask, pil, ta, dtype=np.complex128), r64)
+    assert r32.dtype == np.complex64 and q32.dtype == np.float32
+    eps = np.finfo(np.float32).eps
+    assert np.abs(r32 - r64).max() <= 8 * eps * np.abs(r64).max()
+    assert np.abs(q32 - q64).max() <= 8 * eps * np.abs(q64).max()
+    assert np.abs(r32 - r64).max() > 0                                                   # really single precision
