@@ -379,6 +379,36 @@ int sb_ofdm_ml(const float* d_y, const float* d_h_hat, const float* d_err_var, c
                int32_t streams_per_rx, int32_t interferers_per_rx, int32_t num_data, int32_t num_points, int32_t method,
                int32_t output, int32_t hard_out, void* stream);
 
+/* KBestDetector.call (mimo/detection.py:539-1037, complex2real_channel mimo/utils.py:194-242, List2LLRSimple
+ * mimo/utils.py:420-577, PAM2QAM mapping.py:1234-1320), complex64: d_y [num, M], d_h [num, M, K], d_s [num, M, M].
+ * num_points = |C| of the transmitted constellation (m = log2 num_points output bits per symbol). real_rep 0: d_points
+ * [num_points] complex (any constellation); real_rep 1 (QAM, m even): the real-valued representation, d_points
+ * [2^(m/2)] real PAM levels by label. k: paths kept per layer (at most num_points^K are ever kept). output 0 bit /
+ * 1 symbol (symbol needs hard_out = 1); d_out: LLRs or hard bits [num, K, m] (float) or symbol indices [num, K]
+ * (int32). LLRs are clipped to +-llr_clip (INFINITY allowed). d_workspace: device memory of at least
+ * sb_kbest_workspace_bytes(num, K, real_rep) bytes, 8-byte aligned (SB_ENOMEM if it is missing or smaller).
+ * Malformed arguments return SB_EINVAL (K < 1, M < K, k < 1, num_points not a power of two >= 2, flags outside {0, 1},
+ * real_rep with odd m, soft symbol output, llr_clip < 0 or NaN). Limits, counted in the detection domain (S = K or 2 K
+ * layers of num_points or 2^(m/2) points): S <= 16, k <= 256, points <= 256, k * points <= 16384, and a whitening
+ * scratch of 8 (M^2 + M K + M) (+ 8 (4 M K + 2 M) with real_rep) bytes per problem within 200 KB; beyond them
+ * SB_EUNSUPPORTED with a message. */
+int sb_mimo_kbest(const float* d_y, const float* d_h, const float* d_s, const float* d_points, void* d_out,
+                  void* d_workspace, size_t workspace_bytes, int64_t num, int32_t M, int32_t K, int32_t num_points,
+                  int32_t k, int32_t real_rep, int32_t output, int32_t hard_out, float llr_clip, void* stream);
+/* Workspace bytes sb_mimo_kbest / sb_ofdm_kbest need for num_problems problems of K streams: with S = K << real_rep,
+ * 8 (S^2 + S + 1) + 8 K + 4 S per problem (sb_ofdm_kbest: num_problems = batch * num_rx * num_symbols *
+ * num_subcarriers); 0 for K << real_rep outside 1 ... 16 or real_rep outside {0, 1}. */
+size_t sb_kbest_workspace_bytes(int64_t num_problems, int32_t K, int32_t real_rep);
+/* K-Best detection per OFDM resource element: sb_ofdm_ml's inputs, strides, tables and output layouts (without priors
+ * and soft symbols), then sb_mimo_kbest's detector with M = num_rx_ant and K = streams_per_rx. */
+int sb_ofdm_kbest(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
+                  const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired, const int32_t* d_undesired,
+                  const int32_t* d_out_stream, const int32_t* d_data_pos, const float* d_points, void* d_out,
+                  void* d_workspace, size_t workspace_bytes, int64_t batch, int32_t num_rx, int32_t num_rx_ant,
+                  int32_t num_tx_streams, int32_t num_symbols, int32_t num_subcarriers, int32_t streams_per_rx,
+                  int32_t interferers_per_rx, int32_t num_data, int32_t num_points, int32_t k, int32_t real_rep,
+                  int32_t output, int32_t hard_out, float llr_clip, void* stream);
+
 /* Fused receive front-end (csrc/frontend.cu): LS estimation at the pilots (+ PUSCH CDM de-spreading) + nearest /
  * linear interpolation + OFDM equaliser glue + LMMSE equalisation + square-QAM demapping in ONE launch, for receivers
  * without interfering streams and 1..4 streams (ofdm/channel_estimation.py:138-285, 364-734, ofdm/equalization.py:126-275,

@@ -73,6 +73,9 @@ SIGNATURES = {
     "sb_mimo_ml": (i32, [vp] * 7 + [sz, i64] + [i32] * 6 + [vp]),
     "sb_ml_workspace_bytes": (sz, [i64, i32]),
     "sb_ofdm_ml": (i32, [vp] * 14 + [sz, i64] + [i32] * 12 + [vp]),
+    "sb_mimo_kbest": (i32, [vp] * 6 + [sz, i64] + [i32] * 7 + [f32, vp]),
+    "sb_kbest_workspace_bytes": (sz, [i64, i32, i32]),
+    "sb_ofdm_kbest": (i32, [vp] * 13 + [sz, i64] + [i32] * 13 + [f32, vp]),
 }
 
 

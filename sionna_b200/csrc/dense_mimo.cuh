@@ -1,9 +1,11 @@
 // dense_mimo.cuh -- per-vector dense linear algebra and the OFDM per-resource-element problem assembly shared by the LMMSE
-// kernels (ofdm_mimo.cu) and the maximum-likelihood detector (mimo_ml.cu), so both whiten with the same arithmetic.
+// kernels (ofdm_mimo.cu) and the maximum-likelihood and K-Best detectors (mimo_ml.cu, mimo_kbest.cu), so all whiten
+// with the same arithmetic.
 //   Scratch          per-thread view of a shared-memory matrix, interleaved by thread (element e of thread t at
 //                    [e * T + t]: conflict-free); scratch_threads sizes the CTA
 //   chol_lower       L = chol(S), in place                                   (utils/linalg.py:28-32)
 //   whiten           y_w = L^-1 y, H_w = L^-1 H                              (mimo/utils.py:343-347)
+//   qr_record        modified Gram-Schmidt of [H_w | y_w] in a given column order: R, Q^H y_w, out-of-span term
 //   OfdmEqParams     OFDMEqualizer's inputs and stream-management tables (ofdm/equalization.py:109-275)
 //   ofdm_re / ofdm_load_re / ofdm_out_index   addressing of one resource element, S = H_u H_u^H + diag(no) +
 //                    diag(sum err_var) assembly (equalization.py:205-218), output position of stream k
@@ -46,6 +48,42 @@ static __device__ void whiten(const Scratch& L, const Scratch& Y, const Scratch&
             H(i * K + c) = make_float2(w.x / d, w.y / d);
         }
     }
+}
+
+// Modified Gram-Schmidt on the whitened [H | y] with the columns of H taken in the order col(0), col(1), ... (H: M x K
+// in scratch, column col(j) overwritten by q_j), record: R [K, K] row-major in that order, yq = Q^H y [K], the
+// out-of-span term c0 = ||y - Q yq||^2 in rec[K^2 + K].x. Columns j >= M (or numerically dependent ones) get R_jj = 0
+// and a zero q_j. col is a functor so that the identity order compiles to plain indexing.
+template <class Col>
+static __device__ void qr_record(const Scratch& Y, const Scratch& H, int M, int K, Col col, float2* __restrict__ rec) {
+    for (int j = 0; j < K; ++j) {
+        const int cj = col(j);
+        for (int r = 0; r < j; ++r) {
+            const int cr = col(r);
+            float2 a = make_float2(0.f, 0.f);
+            for (int m = 0; m < M; ++m) a = cadd(a, cmulc(H(m * K + cj), H(m * K + cr)));   // q_r^H h_j
+            for (int m = 0; m < M; ++m) H(m * K + cj) = csub(H(m * K + cj), cmul(H(m * K + cr), a));
+            rec[r * K + j] = a;
+        }
+        for (int r = j + 1; r < K; ++r) rec[r * K + j] = make_float2(0.f, 0.f);
+        float n2 = 0.f;
+        for (int m = 0; m < M; ++m) { float2 v = H(m * K + cj); n2 += v.x * v.x + v.y * v.y; }
+        const float nrm = sqrtf(n2);
+        const bool keep = j < M && nrm > 0.f;
+        const float inv = keep ? 1.f / nrm : 0.f;
+        rec[j * K + j] = make_float2(keep ? nrm : 0.f, 0.f);
+        for (int m = 0; m < M; ++m) H(m * K + cj) = cscale(H(m * K + cj), inv);
+    }
+    for (int r = 0; r < K; ++r) {
+        const int cr = col(r);
+        float2 a = make_float2(0.f, 0.f);
+        for (int m = 0; m < M; ++m) a = cadd(a, cmulc(Y(m), H(m * K + cr)));
+        for (int m = 0; m < M; ++m) Y(m) = csub(Y(m), cmul(H(m * K + cr), a));
+        rec[K * K + r] = a;
+    }
+    float c0 = 0.f;
+    for (int m = 0; m < M; ++m) { float2 v = Y(m); c0 += v.x * v.x + v.y * v.y; }
+    rec[K * K + K] = make_float2(c0, 0.f);
 }
 
 // Threads per CTA of a thread-per-vector scratch kernel: per_thread bytes of shared memory each and at most cap bytes in

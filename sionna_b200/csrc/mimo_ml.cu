@@ -45,36 +45,6 @@ constexpr size_t kMlSmemCap = 200 * 1024;
 
 __host__ __device__ constexpr int ml_record_size(int K) { return K * K + K + 1; }   // float2 per problem
 
-// Modified Gram-Schmidt on the whitened [H | y] (H: M x K in scratch, overwritten by Q), record: R [K, K] row-major,
-// yq [K], c0 in rec[K^2 + K].x. Columns j >= M (or numerically dependent ones) get R_jj = 0 and a zero q_j.
-__device__ void ml_qr_record(const Scratch& Y, const Scratch& H, int M, int K, float2* __restrict__ rec) {
-    for (int j = 0; j < K; ++j) {
-        for (int r = 0; r < j; ++r) {
-            float2 a = make_float2(0.f, 0.f);
-            for (int m = 0; m < M; ++m) a = cadd(a, cmulc(H(m * K + j), H(m * K + r)));   // q_r^H h_j
-            for (int m = 0; m < M; ++m) H(m * K + j) = csub(H(m * K + j), cmul(H(m * K + r), a));
-            rec[r * K + j] = a;
-        }
-        for (int r = j + 1; r < K; ++r) rec[r * K + j] = make_float2(0.f, 0.f);
-        float n2 = 0.f;
-        for (int m = 0; m < M; ++m) { float2 v = H(m * K + j); n2 += v.x * v.x + v.y * v.y; }
-        const float nrm = sqrtf(n2);
-        const bool keep = j < M && nrm > 0.f;
-        const float inv = keep ? 1.f / nrm : 0.f;
-        rec[j * K + j] = make_float2(keep ? nrm : 0.f, 0.f);
-        for (int m = 0; m < M; ++m) H(m * K + j) = cscale(H(m * K + j), inv);
-    }
-    for (int r = 0; r < K; ++r) {
-        float2 a = make_float2(0.f, 0.f);
-        for (int m = 0; m < M; ++m) a = cadd(a, cmulc(Y(m), H(m * K + r)));
-        for (int m = 0; m < M; ++m) Y(m) = csub(Y(m), cmul(H(m * K + r), a));
-        rec[K * K + r] = a;
-    }
-    float c0 = 0.f;
-    for (int m = 0; m < M; ++m) { float2 v = Y(m); c0 += v.x * v.x + v.y * v.y; }
-    rec[K * K + K] = make_float2(c0, 0.f);
-}
-
 // One thread per problem. Dense: y [P, M], h [P, M, K], s [P, M, M]; output position of stream k = p K + k.
 // OFDM (is_ofdm): problem = resource element (b, rx, symbol, subcarrier), output positions from the stream
 // tables (-1: no data; elements without data for any stream are skipped).
@@ -103,7 +73,7 @@ __global__ void ml_prologue_kernel(const float2* __restrict__ y, const float2* _
         }
         sb_dense::chol_lower(S, M);
         sb_dense::whiten(S, Y, H, M, K);
-        ml_qr_record(Y, H, M, K, recs + i * ml_record_size(K));
+        sb_dense::qr_record(Y, H, M, K, [](int j) { return j; }, recs + i * ml_record_size(K));
     }
 }
 

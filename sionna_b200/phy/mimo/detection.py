@@ -1,10 +1,13 @@
-"""MIMO detection (mirror of /root/reference/src/sionna/phy/mimo/detection.py:24-537): linear and maximum-likelihood."""
+"""MIMO detection (mirror of /root/reference/src/sionna/phy/mimo/detection.py:24-1037): linear, maximum-likelihood and
+K-Best."""
+import warnings
+
 import numpy as np
 import torch
 
 from ..._lib import lib, check, ptr, current_stream
 from ..block import Block
-from ..mapping import Constellation, Demapper
+from ..mapping import Constellation, Demapper, pam
 from .equalization import lmmse_equalizer
 
 
@@ -134,4 +137,171 @@ class MaximumLikelihoodDetector(Block):
         check(lib().sb_mimo_ml(ptr(y), ptr(h), ptr(s), ptr(pr), ptr(pts), ptr(out), ptr(ws), ws.numel(), num, mm, k, npts,
                                self._method, int(self._output == "symbol"), int(self._hard_out), current_stream()),
               "sb_mimo_ml")
+        return out
+
+
+KB_MAX_LAYERS = 16
+KB_MAX_K = 256
+KB_MAX_POINTS = 256
+KB_MAX_CHILDREN = 16384
+
+
+def kbest_check_limits(num_layers, k, num_points):
+    """ValueError unless the detection domain (``num_layers`` = streams, or twice that in the real-valued
+    representation, of ``num_points`` points) is within the limits of ``sb_mimo_kbest`` / ``sb_ofdm_kbest``: at most 16
+    layers, k <= 256, 256 points and k * num_points <= 16384."""
+    if num_layers > KB_MAX_LAYERS:
+        raise ValueError(f"KBestDetector: {num_layers} detection layers, supported are at most {KB_MAX_LAYERS} "
+                         f"(16 streams, or 8 with use_real_rep=True)")
+    if k > KB_MAX_K or num_points > KB_MAX_POINTS or k * num_points > KB_MAX_CHILDREN:
+        raise ValueError(f"KBestDetector: k = {k} paths of a {num_points}-point detection constellation; supported are "
+                         f"k <= {KB_MAX_K}, at most {KB_MAX_POINTS} points and k * points <= {KB_MAX_CHILDREN}")
+
+
+def kbest_workspace(num_problems, num_streams, real_rep, device):
+    """Workspace of ``sb_mimo_kbest`` / ``sb_ofdm_kbest`` from PyTorch's caching allocator (sorted triangular records,
+    column orders and output positions, ``sb_kbest_workspace_bytes``)."""
+    n = int(lib().sb_kbest_workspace_bytes(int(num_problems), int(num_streams), int(real_rep)))
+    return torch.empty(max(n, 8), dtype=torch.uint8, device=device)
+
+
+class List2LLR(Block):
+    """Base class of the rules that turn a K-Best candidate list into LLRs (mimo/utils.py:365-418). Only
+    ``List2LLRSimple`` is provided: it runs inside the K-Best kernel, which never materialises the list."""
+
+    def call(self, y, r, dists, path_inds, path_syms):
+        raise NotImplementedError("List2LLR rules run inside KBestDetector's kernel; only List2LLRSimple is provided")
+
+
+class List2LLRSimple(List2LLR):
+    """List2LLRSimple(num_bits_per_symbol, llr_clip_val=20.0, precision=None)
+
+    LLR(k, i) = min metric over the paths whose bit i of stream k is 0 minus the min over those where it is 1 (an empty
+    set counts as +inf), clipped to +-``llr_clip_val`` (mimo/utils.py:420-577; ``np.inf`` disables the clipping). Used
+    as ``KBestDetector``'s ``list2llr``, which reads ``llr_clip_val`` at every call."""
+
+    def __init__(self, num_bits_per_symbol, llr_clip_val=20.0, precision=None, **kwargs):
+        super().__init__(precision=precision, **kwargs)
+        self._num_bits_per_symbol = int(num_bits_per_symbol)
+        self.llr_clip_val = llr_clip_val
+
+    @property
+    def llr_clip_val(self):
+        """Absolute value to which the LLRs are clipped."""
+        return self._llr_clip_val
+
+    @llr_clip_val.setter
+    def llr_clip_val(self, value):
+        self._llr_clip_val = value
+
+
+class KBestDetector(Block):
+    """KBestDetector(output, num_streams, k, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, use_real_rep=False, list2llr=None, precision=None)
+
+    MIMO K-Best detection (detection.py:539-1037) on the fused ``sb_mimo_kbest`` kernel: whitening with S, columns
+    sorted by descending norm, QR, then a breadth-first tree search from the last sorted stream that keeps the k paths
+    with the smallest metrics per layer (ties: lower candidate index first, as ``tf.math.top_k``). ``use_real_rep``
+    detects the real-valued equivalent channel (QAM only) on PAM layers. ``call(y [..., M], h [..., M, num_streams],
+    s [..., M, M])`` -> LLRs / hard bits ``[..., num_streams, num_bits_per_symbol]`` (``output="bit"``; LLRs from
+    ``List2LLRSimple``) or int32 symbol indices ``[..., num_streams]`` (``output="symbol"``, needs ``hard_out=True``).
+    ``k`` is clipped to the number of candidate vectors with a warning. Limits, in the detection domain: at most 16
+    layers (streams, or twice the streams with ``use_real_rep``), k <= 256, at most 256 points and k * points <= 16384
+    (ValueError otherwise)."""
+
+    def __init__(self, output, num_streams, k, constellation_type=None, num_bits_per_symbol=None, constellation=None,
+                 hard_out=False, use_real_rep=False, list2llr=None, precision=None, **kwargs):
+        super().__init__(precision=precision, **kwargs)
+        # same argument checks and error types as the reference (detection.py:691-800)
+        assert output in ("bit", "symbol"), "Unknown output"
+        err_msg = "You must provide either constellation or constellation_type and num_bits_per_symbol."
+        if constellation is None:
+            assert constellation_type is not None and num_bits_per_symbol is not None, err_msg
+        else:
+            assert constellation_type is None and num_bits_per_symbol is None, err_msg
+            assert constellation.precision == self.precision, "Constellation has wrong precision."
+        self._output = output
+        self._hard_out = bool(hard_out)
+        self._use_real_rep = bool(use_real_rep)
+        self._num_tx_streams = int(num_streams)
+        if self._use_real_rep:
+            err_msg = "Only QAM can be used for the real-valued representation"
+            if constellation_type is not None:
+                assert constellation_type == "qam", err_msg
+            else:
+                assert constellation.constellation_type == "qam", err_msg
+            self._num_streams = 2 * self._num_tx_streams
+            n = (constellation.num_bits_per_symbol if num_bits_per_symbol is None else num_bits_per_symbol) // 2
+            self._num_bits_per_symbol = n
+            c = pam(n, normalize=False, precision=precision)       # PAM scaled to energy 0.5, as the reference builds it
+            c = c / (np.std(c) * np.sqrt(2)).astype(c.dtype)
+            self._constellation = np.real(c)
+            self._num_bits_out = 2 * n
+        else:
+            self._num_streams = self._num_tx_streams
+            c = Constellation.check_or_create(constellation_type=constellation_type,
+                                              num_bits_per_symbol=num_bits_per_symbol, constellation=constellation,
+                                              precision=precision)
+            self._constellation = c().cpu().numpy()
+            self._num_bits_per_symbol = c.num_bits_per_symbol
+            self._num_bits_out = c.num_bits_per_symbol
+        self._num_symbols = self._constellation.shape[0]
+        self._k = min(int(k), self._num_symbols ** self._num_streams)
+        if self._k < k:
+            warnings.warn(f"KBestDetector: The provided value of k={k} is larger than the possible maximum number of "
+                          f"paths. It has been set to k={self._k}.")
+        kbest_check_limits(self._num_streams, self._k, self._num_symbols)
+        self._list2llr = None
+        if self._output == "bit":
+            if not self._hard_out:
+                self.list2llr = List2LLRSimple(self._num_bits_per_symbol) if list2llr is None else list2llr
+        else:
+            assert self._hard_out is True, "Soft-symbols are not supported for this detector."
+        self._points_dev = None
+
+    @property
+    def list2llr(self):
+        """``List2LLRSimple`` used for soft outputs; its ``llr_clip_val`` is read at every call."""
+        return self._list2llr
+
+    @list2llr.setter
+    def list2llr(self, value):
+        assert isinstance(value, List2LLR)
+        if not isinstance(value, List2LLRSimple):
+            raise NotImplementedError("KBestDetector computes LLRs inside its kernel: only List2LLRSimple is provided")
+        self._list2llr = value
+
+    def build(self, *input_shapes):
+        assert input_shapes[1][-2] >= input_shapes[1][-1], \
+            "The number of receive antennas cannot be smaller than the number of streams"
+
+    def _kernel_args(self, dev):
+        """(device points, k, real_rep, output, hard_out, llr_clip) of the C-ABI call."""
+        if self._points_dev is None or self._points_dev.device != dev:
+            dt = torch.float32 if self._use_real_rep else torch.complex64
+            self._points_dev = torch.as_tensor(self._constellation).to(device=dev, dtype=dt).contiguous()
+        clip = float(self._list2llr.llr_clip_val) if self._list2llr is not None else float("inf")
+        return (self._points_dev, self._k, int(self._use_real_rep), int(self._output == "symbol"), int(self._hard_out),
+                clip)
+
+    def call(self, y, h, s):
+        dev = self.device
+        k, m = self._num_tx_streams, self._num_bits_out
+        h = torch.as_tensor(h).to(device=dev, dtype=torch.complex64)
+        mm = h.shape[-2]
+        if h.shape[-1] != k:
+            raise ValueError(f"h must have num_streams = {k} as last dimension")
+        batch = torch.broadcast_shapes(tuple(torch.as_tensor(y).shape[:-1]), tuple(h.shape[:-2]),
+                                       tuple(torch.as_tensor(s).shape[:-2]))
+        y = torch.as_tensor(y).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm]).contiguous()
+        h = h.expand(list(batch) + [mm, k]).contiguous()
+        s = torch.as_tensor(s).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm, mm]).contiguous()
+        num = int(np.prod(batch)) if len(batch) else 1
+        if self._output == "bit":
+            out = torch.empty(list(batch) + [k, m], dtype=torch.float32, device=dev)
+        else:
+            out = torch.empty(list(batch) + [k], dtype=torch.int32, device=dev)
+        pts, kk, real_rep, symbol, hard, clip = self._kernel_args(dev)
+        ws = kbest_workspace(num, k, real_rep, dev)
+        check(lib().sb_mimo_kbest(ptr(y), ptr(h), ptr(s), ptr(pts), ptr(out), ptr(ws), ws.numel(), num, mm, k, 2 ** m,
+                                  kk, real_rep, symbol, hard, clip, current_stream()), "sb_mimo_kbest")
         return out

@@ -1,14 +1,15 @@
 """OFDM MIMO detection (mirror of /root/reference/src/sionna/phy/ofdm/detection.py:20-847): ``LinearDetector``
 = fused LMMSE equalisation (``sb_ofdm_lmmse``) + demapping with the per-symbol effective noise variance (``sb_demap``);
 ``MaximumLikelihoodDetector`` / ``MaximumLikelihoodDetectorWithPrior`` = fused covariance assembly + ML detection
-(``sb_ofdm_ml``)."""
+(``sb_ofdm_ml``); ``KBestDetector`` = the same assembly + K-Best detection (``sb_ofdm_kbest``)."""
 import numpy as np
 import torch
 
 from ..._lib import lib, check, ptr, current_stream
 from ..block import Block
 from ..mapping import Constellation, Demapper
-from ..mimo.detection import llrs_to_symbol_logits, ml_check_limits, ml_workspace
+from ..mimo.detection import (llrs_to_symbol_logits, ml_check_limits, ml_workspace, KBestDetector as _MimoKBest,
+                              kbest_workspace)
 from .equalization import LMMSEEqualizer, OFDMEqualizer
 
 
@@ -119,3 +120,61 @@ class MaximumLikelihoodDetectorWithPrior(MaximumLikelihoodDetector):
 
     def call(self, y, h_hat, prior, err_var, no):
         return self._detect(y, h_hat, prior, err_var, no)
+
+
+class KBestDetector(Block):
+    """KBestDetector(output, num_streams, k, resource_grid, stream_management, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, use_real_rep=False, list2llr=None, precision=None)
+
+    K-Best detection for OFDM MIMO (detection.py:849-967) on the fused ``sb_ofdm_kbest`` kernel: the
+    interference-plus-noise covariance of every resource element is assembled on chip from ``OFDMEqualizer``'s stream
+    tables, then the receiver's streams are detected as in ``mimo.KBestDetector`` (same arguments, checks and limits).
+    ``call(y, h_hat, err_var, no)`` -> ``[batch, num_tx, num_streams, num_data_symbols*num_bits_per_symbol]`` LLRs / hard
+    bits (``output="bit"``) or ``[batch, num_tx, num_streams, num_data_symbols]`` int32 indices (``output="symbol"``,
+    ``hard_out=True``). ``num_streams`` must equal ``stream_management.num_streams_per_rx`` (ValueError)."""
+
+    def __init__(self, output, num_streams, k, resource_grid, stream_management, constellation_type=None,
+                 num_bits_per_symbol=None, constellation=None, hard_out=False, use_real_rep=False, list2llr=None,
+                 precision=None, **kwargs):
+        super().__init__(precision=precision, **kwargs)
+        if int(num_streams) != stream_management.num_streams_per_rx:
+            raise ValueError(f"KBestDetector: num_streams = {num_streams}, but every receiver detects "
+                             f"stream_management.num_streams_per_rx = {stream_management.num_streams_per_rx} streams")
+        self._detector = _MimoKBest(output, num_streams, k, constellation_type=constellation_type,
+                                    num_bits_per_symbol=num_bits_per_symbol, constellation=constellation,
+                                    hard_out=hard_out, use_real_rep=use_real_rep, list2llr=list2llr,
+                                    precision=precision)
+        self._output = output
+        self._eq = OFDMEqualizer("lmmse", resource_grid, stream_management, precision=precision)
+
+    @property
+    def list2llr(self):
+        """The wrapped detector's ``List2LLRSimple`` (soft bit outputs)."""
+        return self._detector.list2llr
+
+    def call(self, y, h_hat, err_var, no):
+        eq, det = self._eq, self._detector
+        rg, sm = eq._resource_grid, eq._stream_management
+        dev = self.device
+        y_eff, h, ev, ev_st, no_t, no_st = eq._kernel_inputs(y, h_hat, err_var, no)
+        b, rx, ant, s_, f_ = y_eff.shape
+        if ant < sm.num_streams_per_rx:
+            raise AssertionError("The number of receive antennas cannot be smaller than the number of streams")
+        txs = sm.num_tx * sm.num_streams_per_tx
+        des, und, out_ts, data_pos = eq._tables(dev)
+        nd = rg.pilot_pattern.num_data_symbols
+        m = det._num_bits_out
+        shp = [b, sm.num_tx, sm.num_streams_per_tx]
+        if self._output == "bit":
+            out = torch.zeros(shp + [nd * m], dtype=torch.float32, device=dev)
+        else:
+            out = torch.zeros(shp + [nd], dtype=torch.int32, device=dev)
+        pts, kk, real_rep, symbol, hard, clip = det._kernel_args(dev)
+        ev_arr = np.asarray(ev_st, np.int64)                    # host stride arrays: alive until the call returns
+        no_arr = np.asarray(no_st, np.int64)
+        ws = kbest_workspace(b * rx * s_ * f_, sm.num_streams_per_rx, real_rep, dev)
+        check(lib().sb_ofdm_kbest(ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
+                                  ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos), ptr(pts), ptr(out),
+                                  ptr(ws), ws.numel(), b, rx, ant, txs, s_, f_, sm.num_streams_per_rx,
+                                  sm.num_interfering_streams_per_rx, nd, 2 ** m, kk, real_rep, symbol, hard, clip,
+                                  current_stream()), "sb_ofdm_kbest")
+        return out
