@@ -281,17 +281,17 @@ int sb_tdl_sos(const float* d_doppler, const float* d_theta, const float* d_phi,
  * sb_phase_table: d_e [n_tab, paths, cols] complex; mode 0: exp(-j 2 pi x_j tau[tab, p]) (x = subcarrier frequencies,
  *   cir_to_ofdm_channel :232-244); mode 1: sinc(x_j - tau[tab, p] * scale) (x = tap lags l, scale = bandwidth,
  *   cir_to_time_channel :318-338). n_tab = 1 when all links share the delays (every TDL model), else one table per link.
- * sb_cir_gram: d_g [n_tab, paths, paths] = sum_j e[p, j] conj(e[q, j]).
+ * sb_cir_gram: d_g [n_tab, paths, paths] complex double = sum_j e[p, j] conj(e[q, j]), accumulated in double.
  * sb_cir_link_scale: normalisation of :246-251 / :341-348 per link (batch, rx, tx) from the taps d_a [batch, rx, rx_ant,
  *   tx, tx_ant, paths, time] and the Gram matrix (g_link_stride = 0: shared, else paths*paths): d_scale [batch*rx*tx] =
- *   1 / sqrt(link energy / (rx_ant * tx_ant * time * denom)), 0 for an all-zero link; denom = cols (OFDM: mean over
- *   subcarriers) or 1 (time channel: sum over taps).
+ *   1 / sqrt(link energy / (rx_ant * tx_ant * time * denom)), 0 only for a link of zero energy; denom = cols (OFDM: mean over
+ *   subcarriers) or 1 (time channel: sum over taps). The quadratic form is evaluated in double; paths <= 96 as in sb_cir_apply.
  * sb_cir_apply: d_h [batch, rx, rx_ant, tx, tx_ant, time, cols] = scale[link] * sum_p a[..., p, t] e[tab, p, col]
  *   (d_scale may be NULL; e_link_stride = 0: shared table, else paths*cols). */
 int sb_phase_table(const float* d_tau, const float* d_x, float scale, int32_t mode, float* d_e, int64_t n_tab,
                    int32_t num_paths, int32_t num_cols, void* stream);
-int sb_cir_gram(const float* d_e, float* d_g, int64_t n_tab, int32_t num_paths, int32_t num_cols, void* stream);
-int sb_cir_link_scale(const float* d_a, const float* d_g, int64_t g_link_stride, float* d_scale, int64_t batch,
+int sb_cir_gram(const float* d_e, double* d_g, int64_t n_tab, int32_t num_paths, int32_t num_cols, void* stream);
+int sb_cir_link_scale(const float* d_a, const double* d_g, int64_t g_link_stride, float* d_scale, int64_t batch,
                       int32_t num_rx, int32_t num_rx_ant, int32_t num_tx, int32_t num_tx_ant, int32_t num_paths,
                       int32_t num_time_steps, float denom, void* stream);
 int sb_cir_apply(const float* d_a, const float* d_e, int64_t e_link_stride, const float* d_scale, float* d_h,

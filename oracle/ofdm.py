@@ -307,45 +307,53 @@ def _ofdm_lmmse(y_eff, h_hat, err_var, no, mask, sm, cdt, rdt, equalizer):
 
 
 # ---- on-device channel generation (SURVEY.md 8(f3)) ------------------------------------------------------------------
-def tdl_sos(doppler, theta, phi, phi0, powers, los_power, los_aoa, num_time_steps, fs):
-    """Sum-of-sinusoids tap gains (channel/tr38901/tdl.py:374-456), float64: doppler [B], theta [B, P, Ns],
-    phi [B, A, P, Ns], phi0 [B] | None, powers [P] -> a [B, A, P, T]."""
+def tdl_sos(doppler, theta, phi, phi0, powers, los_power, los_aoa, num_time_steps, fs, dtype=np.float64):
+    """Sum-of-sinusoids tap gains (channel/tr38901/tdl.py:374-456): doppler [B], theta [B, P, Ns], phi [B, A, P, Ns],
+    phi0 [B] | None, powers [P] -> a [B, A, P, T], evaluated in the real type ``dtype`` (float64, or float32 for the
+    reference's own single-precision evaluation)."""
+    rd = np.dtype(dtype).type
     ns = theta.shape[-1]
-    t = np.arange(num_time_steps, dtype=np.float64) / fs                               # :374-376
-    alpha = 2 * np.pi / ns * np.arange(1, ns + 1) + theta.astype(np.float64)           # :286-288, :403
-    arg = (doppler.astype(np.float64)[:, None, None, None, None] * t[None, None, None, :, None]
-           * np.cos(alpha)[:, None, :, None, :] + phi.astype(np.float64)[:, :, :, None, :])          # :415
-    h = np.exp(1j * arg).sum(-1) / np.sqrt(ns)                                           # :417-421
-    h = np.sqrt(np.asarray(powers, np.float64))[None, None, :, None] * h                 # :423-424
+    t = np.arange(num_time_steps, dtype=rd) / rd(fs)                                    # :374-376
+    alpha = rd(2 * np.pi / ns) * np.arange(1, ns + 1, dtype=rd) + theta.astype(rd)      # :286-288, :403
+    arg = (doppler.astype(rd)[:, None, None, None, None] * t[None, None, None, :, None]
+           * np.cos(alpha)[:, None, :, None, :] + phi.astype(rd)[:, :, :, None, :])               # :415
+    h = np.exp(1j * arg).sum(-1) / np.sqrt(rd(ns))                                       # :417-421
+    h = np.sqrt(np.asarray(powers, rd))[None, None, :, None] * h                         # :423-424
     if phi0 is not None:                                                                 # :426-448
-        spec = np.exp(1j * (doppler.astype(np.float64)[:, None] * t[None, :] * np.cos(los_aoa)
-                            + phi0.astype(np.float64)[:, None]))
-        h[:, :, 0, :] += np.sqrt(los_power) * spec[:, None, :]
+        spec = np.exp(1j * (doppler.astype(rd)[:, None] * t[None, :] * np.cos(rd(los_aoa))
+                            + phi0.astype(rd)[:, None]))
+        h[:, :, 0, :] += np.sqrt(rd(los_power)) * spec[:, None, :]
     return h
 
 
-def cir_to_ofdm(frequencies, a, tau):
-    """h[..., t, f] = sum_p a[..., p, t] exp(-j 2 pi f tau_p) (channel/utils.py:180-253); a [..., P, T], tau [P]."""
-    e = np.exp(-2j * np.pi * np.asarray(tau, np.float64)[:, None] * np.asarray(frequencies, np.float64)[None, :])
-    return np.einsum("...pt,pf->...tf", a, e)
+def _contract(a, e):
+    if e.ndim == 2:                                                                      # shared table [P, C]
+        return np.einsum("...pt,pf->...tf", a, e)
+    return np.einsum("brmtnpl,brtpf->brmtnlf", a, e)                                     # per-link [B, RX, TX, P, C]
 
 
-def cir_to_time(bandwidth, a, tau, l_min, l_max):
-    """hm[..., t, l] = sum_p a[..., p, t] sinc(l - tau_p W) (channel/utils.py:320-336); a [..., P, T], tau [P]."""
+def cir_to_ofdm(frequencies, a, tau, dtype=np.complex128):
+    """h[..., t, f] = sum_p a[..., p, t] exp(-j 2 pi f tau_p) (channel/utils.py:180-253); a [B, RX, RA, TX, TA, P, T],
+    tau [P] or per link [B, RX, TX, P]. In ``dtype``: complex128, or complex64 (the phases still exact in float64 and
+    then rounded, as the kernel's table is; the contraction in complex64)."""
+    e = np.exp(-2j * np.pi * np.asarray(tau, np.float64)[..., None] * np.asarray(frequencies, np.float64))
+    return _contract(np.asarray(a).astype(dtype), e.astype(dtype))
+
+
+def cir_to_time(bandwidth, a, tau, l_min, l_max, dtype=np.complex128):
+    """hm[..., t, l] = sum_p a[..., p, t] sinc(l - tau_p W) (channel/utils.py:320-336); shapes and ``dtype`` as
+    cir_to_ofdm."""
     l = np.arange(l_min, l_max + 1, dtype=np.float64)
-    g = np.sinc(l[None, :] - np.asarray(tau, np.float64)[:, None] * bandwidth)           # [P, L]
-    return np.einsum("...pt,pl->...tl", a, g)
+    g = np.sinc(l - np.asarray(tau, np.float64)[..., None] * bandwidth)                  # [..., P, L]
+    return _contract(np.asarray(a).astype(dtype), g.astype(dtype))
 
 
-def apply_time_channel(x, h):
+def apply_time_channel(x, h, dtype=np.complex128):
     """y[b, r, n] = sum_t sum_l h[b, r, t, n, l] x[b, t, n - l], x zero outside [0, N) (apply_time_channel.py:115-133).
-    x [B, Tt, N], h [B, R, Tt, N + L - 1, L] -> [B, R, N + L - 1]."""
+    x [B, Tt, N], h [B, R, Tt, N + L - 1, L] -> [B, R, N + L - 1], in ``dtype``."""
     b, r, tt, no, l_tot = h.shape
     n = x.shape[-1]
-    xp = np.concatenate([x, np.zeros(x.shape[:-1] + (l_tot,), x.dtype)], -1)
-    y = np.zeros((b, r, no), complex)
-    for nn in range(no):
-        for l in range(l_tot):
-            if 0 <= nn - l < n:
-                y[:, :, nn] += np.einsum("brt,bt->br", h[:, :, :, nn, l], xp[:, :, nn - l])
-    return y
+    idx = np.arange(no)[:, None] - np.arange(l_tot)[None, :]                             # [NO, L]: n - l
+    xp = np.concatenate([np.asarray(x).astype(dtype), np.zeros(x.shape[:-1] + (1,), dtype)], -1)
+    xs = xp[..., np.where((idx >= 0) & (idx < n), idx, n)]                              # [B, Tt, NO, L], 0 outside
+    return np.einsum("brtnl,btnl->brn", np.asarray(h).astype(dtype), xs)

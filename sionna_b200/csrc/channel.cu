@@ -47,8 +47,9 @@ __global__ void phase_table_kernel(const float* __restrict__ tau, const float* _
     }
 }
 
-// G[tab, p, q] = sum_j e[tab, p, j] conj(e[tab, q, j]); one warp per (tab, p, q), lanes stride j, fixed shuffle tree.
-__global__ void cir_gram_kernel(const float2* __restrict__ e, float2* __restrict__ g, long long n_tab, int P, int F) {
+// G[tab, p, q] = sum_j e[tab, p, j] conj(e[tab, q, j]) in double (every fp32 x fp32 product is exact there); one warp per
+// (tab, p, q), lanes stride j, fixed shuffle tree.
+__global__ void cir_gram_kernel(const float2* __restrict__ e, double2* __restrict__ g, long long n_tab, int P, int F) {
     const int lane = threadIdx.x & 31;
     const long long warps = ((long long)gridDim.x * blockDim.x) >> 5;
     const long long total = n_tab * P * (long long)P;
@@ -58,17 +59,17 @@ __global__ void cir_gram_kernel(const float2* __restrict__ e, float2* __restrict
         const long long tab = w / ((long long)P * P);
         const float2* ep = e + (tab * P + p) * (long long)F;
         const float2* eq = e + (tab * P + q) * (long long)F;
-        float re = 0.f, im = 0.f;
+        double re = 0.0, im = 0.0;
         for (int j = lane; j < F; j += 32) {
             const float2 a = ep[j], b = eq[j];
-            re += a.x * b.x + a.y * b.y;
-            im += a.y * b.x - a.x * b.y;
+            re += (double)a.x * b.x + (double)a.y * b.y;
+            im += (double)a.y * b.x - (double)a.x * b.y;
         }
         for (int o = 16; o > 0; o >>= 1) {
             re += __shfl_down_sync(0xffffffffu, re, o);
             im += __shfl_down_sync(0xffffffffu, im, o);
         }
-        if (lane == 0) g[w] = make_float2(re, im);
+        if (lane == 0) g[w] = make_double2(re, im);
     }
 }
 
@@ -77,41 +78,45 @@ struct CirDims { long long B; int RX, RA, TX, TA, P, T; };
 
 // scale[link] = 1 / sqrt( (sum over the link's antenna pairs and time steps of a^H G a) / (RA * TA * T * denom) ), 0 if
 // the energy is 0. One CTA per link: thread k takes (pair, t) items k, k + blockDim, ... in order; fixed tree afterwards.
-__global__ void cir_link_scale_kernel(const float2* __restrict__ a, const float2* __restrict__ g, long long g_link_stride,
-                                      float* __restrict__ scale, CirDims d, float denom) {
-    extern __shared__ float2 s_g[];                              // P x P
-    __shared__ float s_part[32];
+// Everything in double: on a nearly flat channel (delays close against 1 / bandwidth) G is almost rank one, and on a link
+// in a deep fade the diagonal and the off-diagonal terms cancel to a small fraction of either; in fp32 that left
+// errors of up to a few percent in the factor and could even drive the energy of a non-zero link to <= 0. In double
+// the taps' fp32 products are exact and the rounding of the sum stays ~1e-16 of the terms.
+__global__ void cir_link_scale_kernel(const float2* __restrict__ a, const double2* __restrict__ g, long long g_link_stride,
+                                      float* __restrict__ scale, CirDims d, double denom) {
+    extern __shared__ double2 s_g[];                             // P x P
+    __shared__ double s_part[32];
     const long long links = d.B * d.RX * d.TX;
     for (long long link = blockIdx.x; link < links; link += gridDim.x) {
         const int tx = (int)(link % d.TX);
         const int rx = (int)((link / d.TX) % d.RX);
         const long long b = link / ((long long)d.TX * d.RX);
-        const float2* gp = g + link * g_link_stride;
+        const double2* gp = g + link * g_link_stride;
         __syncthreads();
         for (int i = threadIdx.x; i < d.P * d.P; i += blockDim.x) s_g[i] = gp[i];
         __syncthreads();
         const int items = d.RA * d.TA * d.T;
-        float acc = 0.f;
+        double acc = 0.0;
         for (int it = threadIdx.x; it < items; it += blockDim.x) {
             const int t = it % d.T;
             const int pair = it / d.T;
             const int ta = pair % d.TA, ra = pair / d.TA;
             const long long row = (((b * d.RX + rx) * d.RA + ra) * d.TX + tx) * d.TA + ta;
             const float2* ap = a + row * (long long)d.P * d.T + t;
-            float e = 0.f;
+            double e = 0.0;
             for (int p = 0; p < d.P; ++p) {
                 const float2 x = ap[(size_t)p * d.T];
                 // diagonal term + 2 Re of the strictly lower triangle (G is Hermitian)
-                e += (x.x * x.x + x.y * x.y) * s_g[p * d.P + p].x;
-                float2 s = make_float2(0.f, 0.f);
+                e += ((double)x.x * x.x + (double)x.y * x.y) * s_g[p * d.P + p].x;
+                double s = 0.0;
                 for (int q = 0; q < p; ++q) {
                     const float2 y = ap[(size_t)q * d.T];
-                    const float2 gq = s_g[p * d.P + q];             // sum_f e_p conj(e_q)
-                    // terms (p, q) and (q, p) together: 2 Re( a_p conj(a_q) G[p, q] )
-                    const float2 cy = cmul(x, make_float2(y.x, -y.y));
-                    s.x += cy.x * gq.x - cy.y * gq.y;
+                    const double2 gq = s_g[p * d.P + q];            // sum_f e_p conj(e_q)
+                    // terms (p, q) and (q, p) together: 2 Re( a_p conj(a_q) G[p, q] ); a_p conj(a_q) is exact in double
+                    const double cr = (double)x.x * y.x + (double)x.y * y.y, ci = (double)x.y * y.x - (double)x.x * y.y;
+                    s += cr * gq.x - ci * gq.y;
                 }
-                e += 2.f * s.x;
+                e += 2.0 * s;
             }
             acc += e;
         }
@@ -119,10 +124,10 @@ __global__ void cir_link_scale_kernel(const float2* __restrict__ a, const float2
         if ((threadIdx.x & 31) == 0) s_part[threadIdx.x >> 5] = acc;
         __syncthreads();
         if (threadIdx.x == 0) {
-            float tot = 0.f;
+            double tot = 0.0;
             for (int w = 0; w < (int)(blockDim.x >> 5); ++w) tot += s_part[w];
-            const float mean = tot / ((float)items * denom);
-            scale[link] = mean > 0.f ? 1.0f / sqrtf(mean) : 0.f;
+            const double mean = tot / ((double)items * denom);
+            scale[link] = mean > 0.0 ? (float)(1.0 / sqrt(mean)) : 0.f;
         }
     }
 }
@@ -378,31 +383,36 @@ extern "C" int sb_phase_table(const float* d_tau, const float* d_x, float scale,
     return SB_OK;
 }
 
-extern "C" int sb_cir_gram(const float* d_e, float* d_g, int64_t n_tab, int32_t num_paths, int32_t num_cols, void* stream) {
+extern "C" int sb_cir_gram(const float* d_e, double* d_g, int64_t n_tab, int32_t num_paths, int32_t num_cols, void* stream) {
     if (n_tab == 0) return SB_OK;
     SB_CHECK_ARG(d_e && d_g && n_tab > 0 && num_paths > 0 && num_cols > 0, "sb_cir_gram: bad arguments");
     const long long warps = n_tab * num_paths * (long long)num_paths;
-    cir_gram_kernel<<<sb_grid(warps, 8, 16), 256, 0, (cudaStream_t)stream>>>((const float2*)d_e, (float2*)d_g, n_tab,
+    cir_gram_kernel<<<sb_grid(warps, 8, 16), 256, 0, (cudaStream_t)stream>>>((const float2*)d_e, (double2*)d_g, n_tab,
                                                                                 num_paths, num_cols);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
 
+constexpr int kMaxCirPaths = 96;                   // sb_cir_apply and sb_cir_link_scale
+
 static int check_dims(int64_t batch, int32_t rx, int32_t ra, int32_t tx, int32_t ta, int32_t p, int32_t t) {
     return batch > 0 && rx > 0 && ra > 0 && tx > 0 && ta > 0 && p > 0 && t > 0;
 }
 
-extern "C" int sb_cir_link_scale(const float* d_a, const float* d_g, int64_t g_link_stride, float* d_scale, int64_t batch,
+extern "C" int sb_cir_link_scale(const float* d_a, const double* d_g, int64_t g_link_stride, float* d_scale, int64_t batch,
                                  int32_t num_rx, int32_t num_rx_ant, int32_t num_tx, int32_t num_tx_ant, int32_t num_paths,
                                  int32_t num_time_steps, float denom, void* stream) {
     if (batch == 0) return SB_OK;
     SB_CHECK_ARG(d_a && d_g && d_scale && check_dims(batch, num_rx, num_rx_ant, num_tx, num_tx_ant, num_paths, num_time_steps) &&
-                     g_link_stride >= 0 && denom > 0.f && num_paths <= 64, "sb_cir_link_scale: bad arguments");
+                     g_link_stride >= 0 && denom > 0.f, "sb_cir_link_scale: bad arguments");
+    SB_CHECK_ARG(num_paths <= kMaxCirPaths, "sb_cir_link_scale: more than 96 paths are not supported");
     CirDims d{batch, num_rx, num_rx_ant, num_tx, num_tx_ant, num_paths, num_time_steps};
     const long long links = batch * num_rx * (long long)num_tx;
-    const size_t smem = sizeof(float2) * (size_t)num_paths * num_paths;
-    cir_link_scale_kernel<<<sb_grid(links, 1, 16), 256, smem, (cudaStream_t)stream>>>((const float2*)d_a, (const float2*)d_g,
-                                                                                g_link_stride, d_scale, d, denom);
+    const size_t smem = sizeof(double2) * (size_t)num_paths * num_paths;     // 96 paths: 144 KB, opt-in above 48 KB
+    if (smem > 48 * 1024)
+        SB_CUDA(cudaFuncSetAttribute(cir_link_scale_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    cir_link_scale_kernel<<<sb_grid(links, 1, 16), 256, smem, (cudaStream_t)stream>>>((const float2*)d_a, (const double2*)d_g,
+                                                                                g_link_stride, d_scale, d, (double)denom);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -414,7 +424,7 @@ extern "C" int sb_cir_apply(const float* d_a, const float* d_e, int64_t e_link_s
     SB_CHECK_ARG(d_a && d_e && d_h && check_dims(batch, num_rx, num_rx_ant, num_tx, num_tx_ant, num_paths, num_time_steps) &&
                      num_cols > 0 && e_link_stride >= 0, "sb_cir_apply: bad arguments");
     CirDims d{batch, num_rx, num_rx_ant, num_tx, num_tx_ant, num_paths, num_time_steps};
-    SB_CHECK_ARG(num_paths <= 96, "sb_cir_apply: more than 96 paths are not supported");
+    SB_CHECK_ARG(num_paths <= kMaxCirPaths, "sb_cir_apply: more than 96 paths are not supported");
     int rc;
     if (num_cols > 48)          // OFDM-like: wide rows
         rc = launch_cir_apply<16, 2, 256, 8>((const float2*)d_a, (const float2*)d_e, e_link_stride, d_scale, (float2*)d_h, d,

@@ -87,7 +87,7 @@ def _cir_convert(a, tau, x, mode, scale, normalize, denom):
               "sb_phase_table")
         g = None
         if normalize:
-            g = torch.empty((n_tab, p, p), dtype=torch.complex64, device=dev)
+            g = torch.empty((n_tab, p, p), dtype=torch.complex128, device=dev)
             check(lib().sb_cir_gram(ptr(e), ptr(g), n_tab, p, n_col, current_stream()), "sb_cir_gram")
         return e, g
 
