@@ -409,6 +409,49 @@ int sb_ofdm_kbest(const float* d_y, const float* d_h_hat, const float* d_err_var
                   int32_t interferers_per_rx, int32_t num_data, int32_t num_points, int32_t k, int32_t real_rep,
                   int32_t output, int32_t hard_out, float llr_clip, void* stream);
 
+/* EPDetector.call (mimo/detection.py:1039-1312, complex2real_channel mimo/utils.py:194-242, SymbolLogits2LLRs
+ * mapping.py:927-967, PAM2QAM mapping.py:1234-1316), complex64: d_y [num, M], d_h [num, M, K], d_s [num, M, M].
+ * num_points = |C| of the transmitted QAM (m = log2 num_points, even); d_levels [2^(m/2)]: the real PAM levels by
+ * label, scaled to energy 1/2. l >= 1 iterations, damping 0 <= beta <= 1. output 0 bit / 1 symbol; d_out: LLRs or hard
+ * bits [num, K, m] (float; real PAM on the even bit positions), QAM logits [num, K, num_points] (float) or QAM indices
+ * [num, K] (int32). One launch, no workspace. Malformed arguments return SB_EINVAL (M < 1, K < 1, num_points not a
+ * power of two >= 2 or with odd m, l < 1, beta outside [0, 1] or NaN, flags outside {0, 1}). Limits: K <= 16,
+ * num_points <= 256, and 8 (M^2 + M K + M + K^2 + K) + 4 (4 K^2 + 14 K) bytes of shared-memory scratch per problem
+ * within 200 KB; beyond them SB_EUNSUPPORTED with a message. M < K is accepted. */
+int sb_mimo_ep(const float* d_y, const float* d_h, const float* d_s, const float* d_levels, void* d_out, int64_t num,
+               int32_t M, int32_t K, int32_t num_points, int32_t l, float beta, int32_t output, int32_t hard_out,
+               void* stream);
+/* EP per OFDM resource element: sb_ofdm_ml's inputs, strides, tables and output layouts (without priors), then
+ * sb_mimo_ep's detector with M = num_rx_ant and K = streams_per_rx. */
+int sb_ofdm_ep(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
+               const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired, const int32_t* d_undesired,
+               const int32_t* d_out_stream, const int32_t* d_data_pos, const float* d_levels, void* d_out,
+               int64_t batch, int32_t num_rx, int32_t num_rx_ant, int32_t num_tx_streams, int32_t num_symbols,
+               int32_t num_subcarriers, int32_t streams_per_rx, int32_t interferers_per_rx, int32_t num_data,
+               int32_t num_points, int32_t l, float beta, int32_t output, int32_t hard_out, void* stream);
+
+/* MMSEPICDetector.call (mimo/detection.py:1314-1643) with output "bit", complex64: d_y [num, M], d_h [num, M, K],
+ * d_s [num, M, M], d_prior [num, K, m] a-priori bit LLRs (NULL: zero prior), d_points [num_points] complex (any
+ * constellation, m = log2 num_points). num_iter >= 1 self-iterations, method 0 app / 1 maxlog demapping. d_out
+ * [num, K, m]: extrinsic LLRs llr_d - llr_a of the last iteration, or their hard decisions (hard_out = 1). Symbol priors
+ * and outputs are converted by the caller (SymbolLogits2LLRs, LLRs2SymbolLogits). One launch, no workspace. Malformed
+ * arguments return SB_EINVAL (M < 1, K < 1, num_points not a power of two >= 2, num_iter < 1, method or hard_out outside
+ * {0, 1}). Limits: K <= 16, num_points <= 1024, and 8 (M^2 + M K + M + 2 K^2 + 6 K) + 4 K m bytes of shared-memory
+ * scratch per problem within 200 KB - 8 num_points; beyond them SB_EUNSUPPORTED with a message. M < K is accepted. */
+int sb_mimo_mmse_pic(const float* d_y, const float* d_h, const float* d_s, const float* d_prior, const float* d_points,
+                     float* d_out, int64_t num, int32_t M, int32_t K, int32_t num_points, int32_t num_iter,
+                     int32_t method, int32_t hard_out, void* stream);
+/* MMSE-PIC per OFDM resource element: sb_ofdm_ml's inputs, strides and tables, then sb_mimo_mmse_pic's detector with
+ * M = num_rx_ant and K = streams_per_rx. d_prior (optional) and d_out: bit LLRs in the output layout
+ * [batch, num_tx_streams, num_data * m]; a stream without data at an element has a zero prior there. */
+int sb_ofdm_mmse_pic(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
+                     const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired,
+                     const int32_t* d_undesired, const int32_t* d_out_stream, const int32_t* d_data_pos,
+                     const float* d_prior, const float* d_points, float* d_out, int64_t batch, int32_t num_rx,
+                     int32_t num_rx_ant, int32_t num_tx_streams, int32_t num_symbols, int32_t num_subcarriers,
+                     int32_t streams_per_rx, int32_t interferers_per_rx, int32_t num_data, int32_t num_points,
+                     int32_t num_iter, int32_t method, int32_t hard_out, void* stream);
+
 /* Fused receive front-end (csrc/frontend.cu): LS estimation at the pilots (+ PUSCH CDM de-spreading) + nearest /
  * linear interpolation + OFDM equaliser glue + LMMSE equalisation + square-QAM demapping in ONE launch, for receivers
  * without interfering streams and 1..4 streams (ofdm/channel_estimation.py:138-285, 364-734, ofdm/equalization.py:126-275,

@@ -76,6 +76,10 @@ SIGNATURES = {
     "sb_mimo_kbest": (i32, [vp] * 6 + [sz, i64] + [i32] * 7 + [f32, vp]),
     "sb_kbest_workspace_bytes": (sz, [i64, i32, i32]),
     "sb_ofdm_kbest": (i32, [vp] * 13 + [sz, i64] + [i32] * 13 + [f32, vp]),
+    "sb_mimo_ep": (i32, [vp] * 5 + [i64] + [i32] * 4 + [f32, i32, i32, vp]),
+    "sb_ofdm_ep": (i32, [vp] * 12 + [i64] + [i32] * 10 + [f32, i32, i32, vp]),
+    "sb_mimo_mmse_pic": (i32, [vp] * 6 + [i64] + [i32] * 6 + [vp]),
+    "sb_ofdm_mmse_pic": (i32, [vp] * 13 + [i64] + [i32] * 12 + [vp]),
 }
 
 

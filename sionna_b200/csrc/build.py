@@ -18,10 +18,11 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "..", "libsionna_b200.so")
 OBJ_DIR = os.path.join(HERE, "..", "..", "build", "obj")
 EXACT = ["common.cu", "ldpc_bp.cu", "ldpc_bp_qc.cu", "ldpc_bp_flat.cu", "ldpc_enc.cu", "phy_kernels.cu"]   # -fmad=false
-FAST = ["ofdm_mimo.cu", "channel.cu", "frontend.cu", "mimo_ml.cu", "mimo_kbest.cu"]                       # -fmad=true
+FAST = ["ofdm_mimo.cu", "channel.cu", "frontend.cu", "mimo_ml.cu", "mimo_kbest.cu",
+        "mimo_iterative.cu"]                                                                     # -fmad=true
 SOURCES = EXACT + FAST
 HEADERS = ["sb_common.h", "sb_math.h", "sb_math2.cuh", "sb_logtab.h", "rng.cuh", "ldpc_graph.h", "ldpc_rules.cuh",
-           "lmmse_diag.cuh", "dense_mimo.cuh", "demap_qam.cuh", os.path.join("..", "..", "include", "sionna_b200.h")]
+           "lmmse_diag.cuh", "dense_mimo.cuh", "demap_qam.cuh", "demap_prior.cuh", os.path.join("..", "..", "include", "sionna_b200.h")]
 COMMON_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
     "-Xcompiler", "-fPIC", "-Xcompiler", "-O2", "-Xcompiler", "-ffp-contract=off", "-Xptxas", "-v",

@@ -12,6 +12,7 @@
 #include "sb_math2.cuh"
 #include "rng.cuh"
 #include "demap_qam.cuh"
+#include "demap_prior.cuh"
 
 namespace {
 
@@ -51,21 +52,6 @@ __global__ void qam_map_kernel(const float* __restrict__ bits, const float2* __r
 }
 
 // ---------------------------------------------------------------------------------------------------------
-// log_sigmoid(x) = -softplus(-x) with TensorFlow's softplus branches (threshold = log(eps) + 2)
-__device__ __forceinline__ float log1p_pos(float u) {   // u >= 0
-    float w = __fadd_rn(1.f, u);
-    if (w == 1.f) return u;
-    return __fmul_rn(sb_logf(w), __fdiv_rn(u, __fsub_rn(w, 1.f)));
-}
-__device__ __forceinline__ float softplusf(float x) {
-    const float threshold = -13.942385f;   // logf(FLT_EPSILON) + 2
-    if (x > -threshold) return x;
-    float ex = sb_expf(x);
-    if (x < threshold) return ex;
-    return log1p_pos(ex);
-}
-__device__ __forceinline__ float log_sigmoidf(float x) { return -softplusf(-x); }
-
 // Stores the M LLRs of the symbols base + threadIdx.x (those < n_sym) through the warp's own tile of 32 * M floats of
 // shared memory (s_out: 32 * M floats per warp of the CTA), so that a warp's global stores are contiguous; no CTA barrier.
 template <int M>
@@ -84,27 +70,8 @@ __device__ __forceinline__ void store_llrs_warp(float* s_out, const float* out, 
     for (int q = lane; q < cnt; q += 32) llr[wfirst * M + q] = s_out[wbase + q];
 }
 
-// One thread per symbol, M = bits per symbol at compile time. Exponents e_j = -|y - c_j|^2 / max(no, tiny) (+ prior
-// term) are evaluated once per pass and feed all 2M groups {points with bit i = v} at the same time:
-//   pass 1: group maxima (maxlog: done);  pass 2 (app): sum_j exp(e_j - max_group) per group, two groups per packed
-//   FP32x2 exp (sb_math2.cuh, bit-identical to sb_expf); LLR_i = logsumexp(bit i = 1) - logsumexp(bit i = 0).
-// Per group the operation order is the one of tf.reduce_logsumexp over the points in ascending label order, which is
-// what the CPU oracle (oracle/mapping_ref.c) evaluates. The LLRs leave through store_llrs_warp.
-template <int M>
-__device__ __forceinline__ float demap_exponent(float2 yy, float2 c, float n0, const float* ls1, const float* ls0, int j,
-                                                bool with_prior) {
-    float dr = __fsub_rn(yy.x, c.x), di = __fsub_rn(yy.y, c.y);
-    float a = __fsqrt_rn(__fmaf_rn(dr, dr, __fmul_rn(di, di)));     // |y - c|  (tf.abs)
-    float e = __fdiv_rn(-__fmul_rn(a, a), n0);                       // -|.|^2 / no
-    if (with_prior) {
-        float ps = 0.f;
-#pragma unroll
-        for (int k = 0; k < M; ++k) ps = __fadd_rn(ps, ((j >> (M - 1 - k)) & 1) ? ls1[k] : ls0[k]);
-        e = __fadd_rn(ps, e);
-    }
-    return e;
-}
-
+// One thread per symbol, M = bits per symbol at compile time: demap_symbol (demap_prior.cuh) with the noise variance
+// max(no, tiny), the LLRs leave through store_llrs_warp.
 template <int METHOD, int M>   // METHOD 0 = app, 1 = maxlog
 __global__ void __launch_bounds__(128) demap_kernel(const float2* __restrict__ y, const float* __restrict__ no,
                                                     long long no_inner, const float2* __restrict__ points,
@@ -133,60 +100,7 @@ __global__ void __launch_bounds__(128) demap_kernel(const float2* __restrict__ y
                     ls0[k] = log_sigmoidf(__fmul_rn(-1.f, pk));
                 }
             }
-            float mx0[M], mx1[M];
-#pragma unroll
-            for (int i = 0; i < M; ++i) { mx0[i] = -INFINITY; mx1[i] = -INFINITY; }
-#pragma unroll 4
-            for (int j = 0; j < NPTS; ++j) {
-                const float e = demap_exponent<M>(yy, s_pts[j], n0, ls1, ls0, j, with_prior);
-#pragma unroll
-                for (int i = 0; i < M; ++i) {                        // label bit i, MSB first (mapping.py:894-907)
-                    if ((j >> (M - 1 - i)) & 1) mx1[i] = fmaxf(mx1[i], e);
-                    else mx0[i] = fmaxf(mx0[i], e);
-                }
-            }
-            if (METHOD == 1) {
-#pragma unroll
-                for (int i = 0; i < M; ++i) out[i] = __fsub_rn(mx1[i], mx0[i]);
-            } else {
-                // tf.reduce_logsumexp: log(sum(exp(x - max))) + max, max replaced by 0 if not finite
-                float sm0[M], sm1[M];
-#pragma unroll
-                for (int i = 0; i < M; ++i) {
-                    mx0[i] = (mx0[i] > -INFINITY && mx0[i] < INFINITY) ? mx0[i] : 0.f;
-                    mx1[i] = (mx1[i] > -INFINITY && mx1[i] < INFINITY) ? mx1[i] : 0.f;
-                    sm0[i] = 0.f; sm1[i] = 0.f;
-                }
-#pragma unroll 2
-                for (int j = 0; j < NPTS; ++j) {
-                    const float e = demap_exponent<M>(yy, s_pts[j], n0, ls1, ls0, j, with_prior);
-                    float t[M + 1];
-#pragma unroll
-                    for (int i = 0; i < M; ++i) t[i] = __fsub_rn(e, ((j >> (M - 1 - i)) & 1) ? mx1[i] : mx0[i]);
-                    t[M] = 0.f;
-#pragma unroll
-                    for (int i = 0; i < M; i += 2) {                 // exp of two groups at a time (sb_math2.cuh)
-                        float2 a = make_float2(fmaxf(t[i], -87.3f), fmaxf(t[i + 1], -87.3f));
-                        float2 r = sb_expf2_inrange(a);
-                        if (t[i] < -87.3f) r.x = 0.f;                // sb_expf: exact 0 below -87.3
-                        if (t[i + 1] < -87.3f) r.y = 0.f;
-                        t[i] = r.x;
-                        t[i + 1] = r.y;
-                    }
-#pragma unroll
-                    for (int i = 0; i < M; ++i) {
-                        if ((j >> (M - 1 - i)) & 1) sm1[i] = __fadd_rn(sm1[i], t[i]);
-                        else sm0[i] = __fadd_rn(sm0[i], t[i]);
-                    }
-                }
-#pragma unroll
-                for (int i = 0; i < M; ++i) {
-                    const float2 lg = sb_logf2(make_float2(fmaxf(sm0[i], 1.17549435e-38f), fmaxf(sm1[i], 1.17549435e-38f)));
-                    float a1 = __fadd_rn(sm1[i] > 0.f ? lg.y : -INFINITY, mx1[i]);
-                    float a0 = __fadd_rn(sm0[i] > 0.f ? lg.x : -INFINITY, mx0[i]);
-                    out[i] = __fsub_rn(a1, a0);
-                }
-            }
+            demap_symbol<METHOD, M>(yy, n0, s_pts, ls1, ls0, with_prior, out);
 #pragma unroll
             for (int i = 0; i < M; ++i) out[i] = hard_out ? (out[i] > 0.f ? 1.f : 0.f) : out[i];   // utils/misc.py:270
         }

@@ -1,5 +1,5 @@
-"""MIMO detection (mirror of /root/reference/src/sionna/phy/mimo/detection.py:24-1037): linear, maximum-likelihood and
-K-Best."""
+"""MIMO detection (mirror of /root/reference/src/sionna/phy/mimo/detection.py:24-1643): linear, maximum-likelihood,
+K-Best, EP and MMSE-PIC."""
 import warnings
 
 import numpy as np
@@ -305,3 +305,169 @@ class KBestDetector(Block):
         check(lib().sb_mimo_kbest(ptr(y), ptr(h), ptr(s), ptr(pts), ptr(out), ptr(ws), ws.numel(), num, mm, k, 2 ** m,
                                   kk, real_rep, symbol, hard, clip, current_stream()), "sb_mimo_kbest")
         return out
+
+
+IT_MAX_STREAMS = 16
+EP_MAX_POINTS = 256
+PIC_MAX_POINTS = 1024
+
+
+def iterative_check_limits(name, num_streams, num_points, max_points):
+    """ValueError unless 1 <= num_streams <= 16 and num_points <= max_points (the limits of ``sb_mimo_ep`` /
+    ``sb_mimo_mmse_pic`` and their OFDM variants: 256 points for EP, 1024 for MMSE-PIC)."""
+    if not 1 <= int(num_streams) <= IT_MAX_STREAMS:
+        raise ValueError(f"{name}: {num_streams} streams, supported are 1 ... {IT_MAX_STREAMS}")
+    if num_points > max_points:
+        raise ValueError(f"{name}: a {num_points}-point constellation, supported are at most {max_points} points")
+
+
+def symbol_logits_to_llrs(logits, num_bits_per_symbol, method):
+    """SymbolLogits2LLRs (mapping.py:927-967): ``[..., 2**m]`` point logits -> ``[..., m]`` LLRs, logsumexp (``"app"``)
+    or max (``"maxlog"``) over the points whose label bit i (MSB first) is 1, minus the same over bit i = 0."""
+    m = num_bits_per_symbol
+    lab = ((torch.arange(2 ** m, device=logits.device)[:, None] >> torch.arange(m - 1, -1, -1, device=logits.device))
+           & 1).bool()
+    x = logits[..., :, None]
+    ninf = torch.tensor(-float("inf"), dtype=logits.dtype, device=logits.device)
+    red = (lambda v: torch.logsumexp(v, dim=-2)) if method == "app" else (lambda v: torch.amax(v, dim=-2))
+    return red(torch.where(lab, x, ninf)) - red(torch.where(~lab, x, ninf))
+
+
+def _dense_inputs(y, h, s, k, dev):
+    """(y [B, M], h [B, M, K], s [B, M, M] complex64 contiguous, batch shape, M, number of problems) after broadcasting
+    the batch dimensions of the three inputs."""
+    h = torch.as_tensor(h).to(device=dev, dtype=torch.complex64)
+    mm = h.shape[-2]
+    if h.shape[-1] != k:
+        raise ValueError(f"h must have num_streams = {k} as last dimension")
+    batch = torch.broadcast_shapes(tuple(torch.as_tensor(y).shape[:-1]), tuple(h.shape[:-2]),
+                                   tuple(torch.as_tensor(s).shape[:-2]))
+    y = torch.as_tensor(y).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm]).contiguous()
+    h = h.expand(list(batch) + [mm, k]).contiguous()
+    s = torch.as_tensor(s).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm, mm]).contiguous()
+    return y, h, s, list(batch), mm, int(np.prod(batch)) if len(batch) else 1
+
+
+class EPDetector(Block):
+    """EPDetector(output, num_bits_per_symbol, hard_out=False, l=10, beta=0.9, precision=None)
+
+    MIMO expectation-propagation detection (detection.py:1039-1312) on the fused ``sb_mimo_ep`` kernel: whitening with
+    S, the real-valued equivalent channel, ``l`` EP iterations with damping ``beta`` over the PAM levels of the QAM
+    (scaled to energy 1/2). ``call(y [..., M], h [..., M, K], s [..., M, M])`` -> LLRs / hard bits ``[..., K, m]``
+    (``output="bit"``: maxlog per PAM, real part on the even bit positions) or QAM logits ``[..., K, 2**m]`` / int32
+    indices ``[..., K]`` (``output="symbol"``, PAM2QAM). QAM only; limits: K <= 16 streams, at most 256 points
+    (ValueError otherwise). M < K is accepted."""
+
+    def __init__(self, output, num_bits_per_symbol, hard_out=False, l=10, beta=0.9, precision=None, **kwargs):
+        super().__init__(precision=precision, **kwargs)
+        # same argument checks and error types as the reference (detection.py:1134-1153)
+        assert output in ("bit", "symbol"), "Unknown output"
+        assert l >= 1, "l must be a positive integer"
+        assert 0.0 <= beta <= 1.0, "beta must be in [0,1]"
+        m = int(num_bits_per_symbol)
+        assert m >= 2 and m % 2 == 0, "EPDetector needs a QAM constellation (an even number of bits per symbol)"
+        if 2 ** m > EP_MAX_POINTS:
+            raise ValueError(f"EPDetector: {2 ** m}-QAM, supported are at most {EP_MAX_POINTS} points")
+        self._output = output
+        self._hard_out = bool(hard_out)
+        self._l = int(l)
+        self._beta = float(beta)
+        self._num_bits_per_symbol = m
+        self._levels = (np.real(pam(m // 2, precision="single")) / np.sqrt(2.0)).astype(np.float32)
+        self._levels_dev = None
+
+    def _kernel_args(self, dev):
+        """(device PAM levels, num_points, l, beta, output, hard_out) of the C-ABI call."""
+        if self._levels_dev is None or self._levels_dev.device != dev:
+            self._levels_dev = torch.as_tensor(self._levels).to(dev).contiguous()
+        return (self._levels_dev, 2 ** self._num_bits_per_symbol, self._l, self._beta, int(self._output == "symbol"),
+                int(self._hard_out))
+
+    def _out(self, shape, dev):
+        m = self._num_bits_per_symbol
+        if self._output == "bit":
+            return torch.empty(shape + [m], dtype=torch.float32, device=dev)
+        if self._hard_out:
+            return torch.empty(shape, dtype=torch.int32, device=dev)
+        return torch.empty(shape + [2 ** m], dtype=torch.float32, device=dev)
+
+    def call(self, y, h, s):
+        dev = self.device
+        k = torch.as_tensor(h).shape[-1]
+        iterative_check_limits("EPDetector", k, 2 ** self._num_bits_per_symbol, EP_MAX_POINTS)
+        y, h, s, batch, mm, num = _dense_inputs(y, h, s, k, dev)
+        out = self._out(batch + [k], dev)
+        lev, npts, l, beta, symbol, hard = self._kernel_args(dev)
+        check(lib().sb_mimo_ep(ptr(y), ptr(h), ptr(s), ptr(lev), ptr(out), num, mm, k, npts, l, beta, symbol, hard,
+                               current_stream()), "sb_mimo_ep")
+        return out
+
+
+class MMSEPICDetector(Block):
+    """MMSEPICDetector(output, demapping_method="maxlog", num_iter=1, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None)
+
+    MIMO MMSE detection with parallel interference cancellation (detection.py:1314-1643) on the fused
+    ``sb_mimo_mmse_pic`` kernel: whitening with S, then ``num_iter`` self-iterations of soft symbols from the a-priori
+    LLRs, the unbiased PIC-MMSE estimate of every stream and demapping with the prior (``"app"`` or ``"maxlog"``); the
+    output is the extrinsic information ``llr_d - llr_a``. ``call(y [..., M], h [..., M, K], s [..., M, M], prior)``:
+    ``output="bit"``: prior = bit LLRs ``[..., K, m]`` -> LLRs / hard bits ``[..., K, m]``; ``output="symbol"``: prior =
+    point logits ``[..., K, |C|]`` (converted to LLRs with the demapping method) -> logits ``[..., K, |C|]``
+    (LLRs2SymbolLogits of the extrinsic LLRs) or their int32 argmax ``[..., K]``. Limits: K <= 16 streams, at most 1024
+    points (ValueError otherwise). M < K is accepted."""
+
+    def __init__(self, output, demapping_method="maxlog", num_iter=1, constellation_type=None, num_bits_per_symbol=None,
+                 constellation=None, hard_out=False, precision=None, **kwargs):
+        super().__init__(precision=precision, **kwargs)
+        # same argument checks and error types as the reference (detection.py:1456-1458)
+        assert isinstance(num_iter, int), "num_iter must be an integer"
+        assert output in ("bit", "symbol"), "Unknown output"
+        assert demapping_method in ("app", "maxlog"), "Unknown demapping method"
+        if num_iter < 1:
+            raise ValueError(f"MMSEPICDetector: num_iter = {num_iter}, at least one self-iteration is needed")
+        self._output = output
+        self._method = demapping_method
+        self._num_iter = num_iter
+        self._hard_out = bool(hard_out)
+        self._constellation = Constellation.check_or_create(constellation_type=constellation_type,
+                                                            num_bits_per_symbol=num_bits_per_symbol,
+                                                            constellation=constellation, precision=precision)
+        if self._constellation.num_points > PIC_MAX_POINTS:
+            raise ValueError(f"MMSEPICDetector: a {self._constellation.num_points}-point constellation, supported are "
+                             f"at most {PIC_MAX_POINTS} points")
+
+    @property
+    def constellation(self):
+        return self._constellation
+
+    def _prior_llrs(self, prior, shape, dev):
+        """Bit LLRs [*shape, m] (float32, contiguous) of a prior given in the output's kind."""
+        m = self._constellation.num_bits_per_symbol
+        pr = torch.as_tensor(prior).to(device=dev, dtype=torch.float32)
+        if self._output == "symbol":
+            pr = symbol_logits_to_llrs(pr, m, self._method)
+        return pr.expand(shape + [m]).contiguous()
+
+    def _finish(self, llr):
+        """The kernel's extrinsic LLRs [..., m] (or hard bits) in the output's kind."""
+        if self._output == "bit":
+            return llr
+        logits = llrs_to_symbol_logits(llr, self._constellation.num_bits_per_symbol)
+        return torch.argmax(logits, dim=-1).to(torch.int32) if self._hard_out else logits
+
+    def _kernel_args(self, dev):
+        """(device points, num_points, num_iter, method, hard_out) of the C-ABI call."""
+        pts = self._constellation().to(device=dev, dtype=torch.complex64).contiguous()
+        return (pts, self._constellation.num_points, self._num_iter, 0 if self._method == "app" else 1,
+                int(self._hard_out and self._output == "bit"))
+
+    def call(self, y, h, s, prior):
+        dev = self.device
+        k, m = torch.as_tensor(h).shape[-1], self._constellation.num_bits_per_symbol
+        iterative_check_limits("MMSEPICDetector", k, self._constellation.num_points, PIC_MAX_POINTS)
+        y, h, s, batch, mm, num = _dense_inputs(y, h, s, k, dev)
+        pr = self._prior_llrs(prior, batch + [k], dev)
+        out = torch.empty(batch + [k, m], dtype=torch.float32, device=dev)
+        pts, npts, num_iter, method, hard = self._kernel_args(dev)
+        check(lib().sb_mimo_mmse_pic(ptr(y), ptr(h), ptr(s), ptr(pr), ptr(pts), ptr(out), num, mm, k, npts, num_iter,
+                                     method, hard, current_stream()), "sb_mimo_mmse_pic")
+        return self._finish(out)

@@ -6,5 +6,6 @@ from .demodulator import OFDMDemodulator
 from .channel_estimation import (BaseChannelEstimator, BaseChannelInterpolator, LSChannelEstimator,
                                  NearestNeighborInterpolator, LinearInterpolator)
 from .equalization import OFDMEqualizer, LMMSEEqualizer
-from .detection import LinearDetector, MaximumLikelihoodDetector, MaximumLikelihoodDetectorWithPrior, KBestDetector
+from .detection import (LinearDetector, MaximumLikelihoodDetector, MaximumLikelihoodDetectorWithPrior, KBestDetector,
+                        EPDetector, MMSEPICDetector)
 from .frontend import FusedLSLinearDetector, fusable, frontend_tables
