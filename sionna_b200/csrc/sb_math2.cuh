@@ -37,6 +37,22 @@ __device__ __forceinline__ float2 sb_expf2_inrange(float2 x) {
               i2f_mov((int)((unsigned)f2i_mov(p.y) + ((unsigned)f2i_mov(t.y) << 23))));
 }
 
+// e^x for x in [-87.3, 88.7], one element: sb_expf's operation sequence without its range tests
+__device__ __forceinline__ float sb_expf_inrange(float x) {
+    float t = __fmaf_rn(x, 1.44269504088896341f, 12582912.0f);
+    float nf = __fadd_rn(t, -12582912.0f);
+    float r = __fmaf_rn(nf, -0.693145751953125f, x);
+    r = __fmaf_rn(nf, -1.42860677e-06f, r);
+    float g = __fmaf_rn(0x1.a124e4p-13f, r, 0x1.6d4316p-10f);
+    g = __fmaf_rn(g, r, 0x1.1110e0p-7f);
+    g = __fmaf_rn(g, r, 0x1.5554eap-5f);
+    g = __fmaf_rn(g, r, 0x1.555556p-3f);
+    g = __fmaf_rn(g, r, 0.5f);
+    float s = __fmaf_rn(__fmul_rn(r, r), g, r);
+    float p = __fadd_rn(1.0f, s);
+    return i2f_mov((int)((unsigned)f2i_mov(p) + ((unsigned)f2i_mov(t) << 23)));
+}
+
 // log(y) for positive normal y
 __device__ __forceinline__ float2 sb_logf2(float2 y) {
     int ix0 = f2i_mov(y.x), ix1 = f2i_mov(y.y);
@@ -149,6 +165,6 @@ __device__ __forceinline__ float2 sb_phif2(float2 x, const LT& lt) {
 template <class LT>
 __device__ __forceinline__ float sb_phif_s(float x, const LT& lt) {
     x = fminf(fmaxf(x, 8.5e-8f), 16.635532f);
-    float t = sb_expf(x);
+    float t = sb_expf_inrange(x);
     return __fsub_rn(sb_logf_tab_s(__fadd_rn(t, 1.0f), lt), sb_logf_tab_s(__fadd_rn(t, -1.0f), lt));
 }
