@@ -1,24 +1,32 @@
-// dense_mimo.cuh -- per-vector dense linear algebra and the OFDM per-resource-element problem assembly shared by the LMMSE
-// kernels (ofdm_mimo.cu) and the maximum-likelihood and K-Best detectors (mimo_ml.cu, mimo_kbest.cu), so all whiten
-// with the same arithmetic.
+// dense_mimo.cuh -- per-vector dense linear algebra, the OFDM per-resource-element problem assembly and the front half
+// of the MIMO detectors, shared by the LMMSE kernels (ofdm_mimo.cu) and the ML, K-Best, EP and MMSE-PIC detectors
+// (mimo_ml.cu, mimo_kbest.cu, mimo_iterative.cu), so all whiten with the same arithmetic.
 //   Scratch          per-thread view of a shared-memory matrix, interleaved by thread (element e of thread t at
-//                    [e * T + t]: conflict-free); scratch_threads sizes the CTA
+//                    [e * T + t]: conflict-free; ScratchOf<float> for real matrices); scratch_threads sizes the CTA,
+//                    detector_threads also under kScratchSmemCap with the error message
 //   chol_lower       L = chol(S), in place                                   (utils/linalg.py:28-32)
 //   whiten           y_w = L^-1 y, H_w = L^-1 H                              (mimo/utils.py:343-347)
 //   qr_record        modified Gram-Schmidt of [H_w | y_w] in a given column order: R, Q^H y_w, out-of-span term
+//                    (qr_record_size float2)
+//   pam2qam_index    QAM label of a pair of PAM labels                       (mapping.py:1234-1320)
 //   OfdmEqParams     OFDMEqualizer's inputs and stream-management tables (ofdm/equalization.py:109-275)
 //   ofdm_re / ofdm_load_re / ofdm_out_index   addressing of one resource element, S = H_u H_u^H + diag(no) +
 //                    diag(sum err_var) assembly (equalization.py:205-218), output position of stream k
+//   MimoProblem / load_whitened   a detector's dense or OFDM problem set; problem i loaded, whitened and given its
+//                    output positions. dense_problem / ofdm_problem build the set from the C-ABI arguments,
+//                    ofdm_check tests the OFDM detectors' pointer arguments
 #pragma once
 #include "sb_common.h"
 
 namespace sb_dense {
 
-struct Scratch {
-    float2* p;
+template <class E>
+struct ScratchOf {
+    E* p;
     int T, t;
-    __device__ __forceinline__ float2& operator()(int e) const { return p[(size_t)e * T + t]; }
+    __device__ __forceinline__ E& operator()(int e) const { return p[(size_t)e * T + t]; }
 };
+using Scratch = ScratchOf<float2>;
 
 // A = L L^H (lower, n x n), in place
 static __device__ void chol_lower(const Scratch& A, int n) {
@@ -86,6 +94,19 @@ static __device__ void qr_record(const Scratch& Y, const Scratch& H, int M, int 
     rec[K * K + K] = make_float2(c0, 0.f);
 }
 
+// float2 per qr_record of K columns: R [K, K], yq [K], c0
+__host__ __device__ constexpr int qr_record_size(int K) { return K * K + K + 1; }
+
+// QAM label of the PAM label pair (re, im) of a QAM with m bits per symbol (m even): re on the even label bits, MSB
+// first (PAM2QAM)
+__device__ __forceinline__ int pam2qam_index(int re, int im, int m) {
+    const int h = m >> 1;
+    int idx = 0;
+    for (int j = 0; j < h; ++j)
+        idx |= (((re >> (h - 1 - j)) & 1) << (m - 1 - 2 * j)) | (((im >> (h - 1 - j)) & 1) << (m - 2 - 2 * j));
+    return idx;
+}
+
 // Threads per CTA of a thread-per-vector scratch kernel: per_thread bytes of shared memory each and at most cap bytes in
 // all. At most 128 and a multiple of 32 when a warp fits; otherwise the largest power of two that fits (16 ... 1), so
 // large matrices still run, at low occupancy. 0 if not even one thread fits.
@@ -97,6 +118,20 @@ static inline int scratch_threads(size_t per_thread, size_t cap, size_t* smem) {
     if (t == 0) return 0;
     *smem = per_thread * t;
     return t;
+}
+
+// dynamic shared memory per CTA of the scratch kernels
+constexpr size_t kScratchSmemCap = 200 * 1024;
+
+// CTA size of a detector kernel with per_thread bytes of scratch after fixed bytes per CTA, *smem = its shared memory;
+// 0 (with an error message naming who) if not even one thread fits
+static inline int detector_threads(const char* who, size_t fixed, size_t per_thread, int M, int K, size_t* smem) {
+    const int th = scratch_threads(per_thread, kScratchSmemCap - fixed, smem);
+    if (!th)
+        sb_set_error("%s: M = %d, K = %d needs %zu bytes of shared-memory scratch per problem, the limit is %zu", who, M,
+                     K, per_thread, kScratchSmemCap - fixed);
+    *smem += fixed;
+    return th;
 }
 
 // OFDMEqualizer inputs. Per (b, rx, sym, sc):
@@ -176,6 +211,85 @@ __device__ __forceinline__ void ofdm_load_re(const OfdmEqParams& p, const OfdmRe
             S(m * M + m2) = acc;
         }
     }
+}
+
+// A detector's problem set: P dense problems (y [P, M], h [P, M, K], s [P, M, M]) or, is_ofdm, the P resource elements
+// of an OFDM grid (problem i = element i of the flattened (b, rx, symbol, subcarrier) grid, M = ANT)
+struct MimoProblem {
+    const float2* y; const float2* h; const float2* s;  // dense inputs (is_ofdm = 0)
+    OfdmEqParams ofdm;
+    int is_ofdm;
+    long long P;
+    int M, K;
+};
+
+// Loads problem i into S [M, M], H [M, K], Y [M] and writes the output position of stream k to oi[k] (dense: i K + k;
+// OFDM: ofdm_out_index, -1 where the stream carries no data). False for an OFDM element that carries no data for any
+// stream; otherwise S -> L = chol(S), Y = L^-1 y, H = L^-1 H.
+static __device__ bool load_whitened(const MimoProblem& q, long long i, const Scratch& S, const Scratch& H,
+                                     const Scratch& Y, long long* oi) {
+    const int M = q.M, K = q.K;
+    if (q.is_ofdm) {
+        const OfdmRe e = ofdm_re(q.ofdm, i);
+        bool any = false;
+        for (int k = 0; k < K; ++k) {
+            oi[k] = ofdm_out_index(q.ofdm, e, k);
+            any = any || oi[k] >= 0;
+        }
+        if (!any) return false;
+        ofdm_load_re(q.ofdm, e, Y, H, S);
+    } else {
+        for (int k = 0; k < K; ++k) oi[k] = i * K + k;
+        for (int e = 0; e < M * M; ++e) S(e) = q.s[i * M * M + e];
+        for (int e = 0; e < M * K; ++e) H(e) = q.h[i * M * K + e];
+        for (int e = 0; e < M; ++e) Y(e) = q.y[i * M + e];
+    }
+    chol_lower(S, M);
+    whiten(S, Y, H, M, K);
+    return true;
+}
+
+static inline MimoProblem dense_problem(const float* y, const float* h, const float* s, long long num, int M, int K) {
+    MimoProblem pb{};
+    pb.y = (const float2*)y; pb.h = (const float2*)h; pb.s = (const float2*)s;
+    pb.is_ofdm = 0; pb.P = num; pb.M = M; pb.K = K;
+    return pb;
+}
+
+// The OFDM C-ABI arguments (sb_ofdm_lmmse and the sb_ofdm_* detectors) as a problem set; ofdm.xh and ofdm.ne are unset
+static inline MimoProblem ofdm_problem(const float* d_y, const float* d_h_hat, const float* d_err_var,
+                                       const int64_t* h_ev_stride, const float* d_no, const int64_t* h_no_stride,
+                                       const int32_t* d_desired, const int32_t* d_undesired,
+                                       const int32_t* d_out_stream, const int32_t* d_data_pos, int64_t batch,
+                                       int num_rx, int num_rx_ant, int num_tx_streams, int num_symbols,
+                                       int num_subcarriers, int streams_per_rx, int interferers_per_rx, int num_data) {
+    MimoProblem pb{};
+    OfdmEqParams& p = pb.ofdm;
+    p.y = (const float2*)d_y; p.hhat = (const float2*)d_h_hat; p.ev = d_err_var; p.no = d_no;
+    for (int i = 0; i < 6; ++i) p.ev_stride[i] = h_ev_stride[i];
+    for (int i = 0; i < 3; ++i) p.no_stride[i] = h_no_stride[i];
+    p.des = d_desired; p.und = d_undesired; p.out_ts = d_out_stream; p.data_pos = d_data_pos;
+    p.B = batch; p.RX = num_rx; p.ANT = num_rx_ant; p.TXS = num_tx_streams;
+    p.S = num_symbols; p.F = num_subcarriers; p.K = streams_per_rx; p.KU = interferers_per_rx; p.ND = num_data;
+    pb.is_ofdm = 1;
+    pb.P = batch * num_rx * (long long)num_symbols * num_subcarriers;
+    pb.M = num_rx_ant;
+    pb.K = streams_per_rx;
+    return pb;
+}
+
+// Pointer arguments of an sb_ofdm_* detector with a non-empty batch: SB_EINVAL ("who: bad arguments") unless every input,
+// table, the constellation and the output are given (d_undesired only with interferers) and num_rx_ant >= 1
+static inline int ofdm_check(const char* who, const float* d_y, const float* d_h_hat, const float* d_err_var,
+                             const int64_t* h_ev_stride, const float* d_no, const int64_t* h_no_stride,
+                             const int32_t* d_desired, const int32_t* d_undesired, const int32_t* d_out_stream,
+                             const int32_t* d_data_pos, const float* d_points, const void* d_out, int64_t batch,
+                             int num_rx_ant, int interferers_per_rx) {
+    SB_CHECK_ARG(d_y && d_h_hat && d_err_var && h_ev_stride && d_no && h_no_stride && d_desired && d_out_stream &&
+                     d_data_pos && d_points && d_out && batch > 0 && num_rx_ant >= 1 &&
+                     (interferers_per_rx == 0 || d_undesired),
+                 "%s: bad arguments", who);
+    return SB_OK;
 }
 
 }  // namespace sb_dense

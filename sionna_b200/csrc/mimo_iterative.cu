@@ -9,8 +9,8 @@
 // and [..., 2K, |C|] logits per iteration; here one thread keeps a whole problem in shared-memory scratch (one launch
 // per call, no workspace).
 //
-// Shared prologue (it_prologue): S -> L = chol(S), y_w = L^-1 y, H_w = L^-1 H (the arithmetic of the other dense
-// detectors), then G = H_w^H H_w and y_mf = H_w^H y_w, K x K complex. Both detectors work on (G, y_mf) only.
+// Shared prologue (it_prologue): y_w and H_w from the detectors' shared loader (load_whitened, dense_mimo.cuh), then
+// G = H_w^H H_w and y_mf = H_w^H y_w, K x K complex. Both detectors work on (G, y_mf) only.
 //
 // EP (ep_kernel): realify(G) and [Re y_mf; Im y_mf] are exactly the reference's H^T H and H^T y of the whitened real
 // channel, whose noise variance is 1/2. Per iteration, A = realify(G) + diag(lam) / 2 is symmetric positive definite
@@ -34,55 +34,23 @@
 namespace {
 
 using sb_dense::Scratch;
-using sb_dense::OfdmEqParams;
+using sb_dense::MimoProblem;
+using sb_dense::ScratchOf;
 
 constexpr int kItMaxStreams = 16;
 constexpr int kEpMaxPoints = 256;                      // 16 PAM levels per real dimension
 constexpr int kPicMaxPoints = 1024;
-constexpr size_t kItSmemCap = 200 * 1024;
-
-// real-valued per-thread scratch, interleaved by thread as Scratch
-struct RScratch {
-    float* p;
-    int T, t;
-    __device__ __forceinline__ float& operator()(int e) const { return p[(size_t)e * T + t]; }
-};
 
 // Scratch of the prologue, in float2 per thread: S [M, M], H [M, K], Y [M], G [K, K], y_mf [K]
 __host__ __device__ constexpr size_t it_base_size(int M, int K) {
     return (size_t)M * M + (size_t)M * K + M + (size_t)K * K + K;
 }
 
-struct ItProblem {
-    const float2* y; const float2* h; const float2* s;  // dense inputs (is_ofdm = 0)
-    OfdmEqParams ofdm;
-    int is_ofdm;
-    long long P;
-    int M, K;
-};
-
-// Loads problem i, whitens it and leaves G and y_mf in scratch; oi[k] = output position of stream k (-1: no data).
-// False for an OFDM element that carries no data.
-__device__ bool it_prologue(const ItProblem& q, long long i, const Scratch& Sc, const Scratch& H, const Scratch& Y,
+// load_whitened, then G and y_mf in scratch. False for an OFDM element that carries no data.
+__device__ bool it_prologue(const MimoProblem& q, long long i, const Scratch& Sc, const Scratch& H, const Scratch& Y,
                             const Scratch& G, const Scratch& YM, long long* oi) {
     const int M = q.M, K = q.K;
-    if (q.is_ofdm) {
-        const sb_dense::OfdmRe e = sb_dense::ofdm_re(q.ofdm, i);
-        bool any = false;
-        for (int k = 0; k < K; ++k) {
-            oi[k] = sb_dense::ofdm_out_index(q.ofdm, e, k);
-            any = any || oi[k] >= 0;
-        }
-        if (!any) return false;
-        sb_dense::ofdm_load_re(q.ofdm, e, Y, H, Sc);
-    } else {
-        for (int k = 0; k < K; ++k) oi[k] = i * K + k;
-        for (int e = 0; e < M * M; ++e) Sc(e) = q.s[i * M * M + e];
-        for (int e = 0; e < M * K; ++e) H(e) = q.h[i * M * K + e];
-        for (int e = 0; e < M; ++e) Y(e) = q.y[i * M + e];
-    }
-    sb_dense::chol_lower(Sc, M);
-    sb_dense::whiten(Sc, Y, H, M, K);
+    if (!sb_dense::load_whitened(q, i, Sc, H, Y, oi)) return false;
     for (int a = 0; a < K; ++a) {
         for (int b = 0; b < K; ++b) {
             float2 g = make_float2(0.f, 0.f);
@@ -99,7 +67,7 @@ __device__ bool it_prologue(const ItProblem& q, long long i, const Scratch& Sc, 
 // ---------------------------------------------------------------------------------------------------------------------
 // EP
 struct EpParams {
-    ItProblem pb;
+    MimoProblem pb;
     const float* levels;                                // [L] PAM levels by label, energy 1/2
     void* out;
     int L, hb, l, output, hard;                         // hb = bits per PAM
@@ -135,14 +103,6 @@ __device__ __forceinline__ int ep_pam_argmax(const float* lev, int L, float xo, 
     return best;
 }
 
-// QAM index of the PAM pair (re, im): re on the even label bits, MSB first (PAM2QAM)
-__device__ __forceinline__ int ep_qam_index(int re, int im, int hb) {
-    int idx = 0;
-    for (int j = 0; j < hb; ++j)
-        idx |= (((re >> (hb - 1 - j)) & 1) << (2 * hb - 1 - 2 * j)) | (((im >> (hb - 1 - j)) & 1) << (2 * hb - 2 - 2 * j));
-    return idx;
-}
-
 // One thread per problem. Shared memory: levels [L] float, then the prologue's float2 scratch and EP's float scratch.
 __global__ void ep_kernel(const EpParams q) {
     extern __shared__ float2 smem[];
@@ -164,9 +124,9 @@ __global__ void ep_kernel(const EpParams q) {
     const Scratch Sc{base, T, t}, H{base + o_h * T, T, t}, Y{base + o_y * T, T, t};
     const Scratch G{base + o_g * T, T, t}, YM{base + o_ym * T, T, t};
     float* rb = reinterpret_cast<float*>(base + it_base_size(M, K) * T);
-    const RScratch A{rb, T, t};
+    const ScratchOf<float> A{rb, T, t};
     const size_t nn = (size_t)n * n;
-    const RScratch lam{rb + nn * T, T, t}, gam{rb + (nn + n) * T, T, t}, sig{rb + (nn + 2 * n) * T, T, t},
+    const ScratchOf<float> lam{rb + nn * T, T, t}, gam{rb + (nn + n) * T, T, t}, sig{rb + (nn + 2 * n) * T, T, t},
         mu{rb + (nn + 3 * n) * T, T, t}, z{rb + (nn + 4 * n) * T, T, t}, xo{rb + (nn + 5 * n) * T, T, t},
         vo{rb + (nn + 6 * n) * T, T, t};
     const float prec = 1e-6f, beta = q.beta;
@@ -261,13 +221,14 @@ __global__ void ep_kernel(const EpParams q) {
                     out[2 * u + 1] = q.hard ? (l2 > 0.f ? 1.f : 0.f) : l2;
                 }
             } else if (q.hard) {
-                static_cast<int*>(q.out)[o] = ep_qam_index(ep_pam_argmax(lev, L, xr, vr), ep_pam_argmax(lev, L, xi, vi), hb);
+                static_cast<int*>(q.out)[o] =
+                    sb_dense::pam2qam_index(ep_pam_argmax(lev, L, xr, vr), ep_pam_argmax(lev, L, xi, vi), 2 * hb);
             } else {
                 // PAM2QAM's gather (mapping.py:1307-1314): output c takes the flattened (re, im) pair at the QAM index
                 // of the pair (c / L, c % L)
                 float* out = static_cast<float*>(q.out) + o * L * L;
                 for (int c = 0; c < L * L; ++c) {
-                    const int g = ep_qam_index(c / L, c % L, hb);
+                    const int g = sb_dense::pam2qam_index(c / L, c % L, 2 * hb);
                     out[c] = ep_logit(xr, vr, lev[g / L]) + ep_logit(xi, vi, lev[g % L]);
                 }
             }
@@ -278,7 +239,7 @@ __global__ void ep_kernel(const EpParams q) {
 // ---------------------------------------------------------------------------------------------------------------------
 // MMSE-PIC
 struct PicParams {
-    ItProblem pb;
+    MimoProblem pb;
     const float2* points;                               // [2^MB]
     const float* prior;                                 // bit LLRs in the output layout, or null (zero prior)
     float* out;
@@ -307,7 +268,7 @@ __global__ void pic_kernel(const PicParams q) {
     const size_t kk = (size_t)K * K;
     const Scratch A{pb, T, t}, XB{pb + kk * T, T, t}, V{pb + (kk + K) * T, T, t}, TG{pb + (kk + 2 * K) * T, T, t},
         XT{pb + (kk + 3 * K) * T, T, t}, NE{pb + (kk + 4 * K) * T, T, t};
-    const RScratch LA{reinterpret_cast<float*>(pb + pic_size(K) * T), T, t};
+    const ScratchOf<float> LA{reinterpret_cast<float*>(pb + pic_size(K) * T), T, t};
     const float tiny = 1.17549435e-38f;                 // np.finfo(float32).tiny, as sb_demap
     long long oi[kItMaxStreams];
     for (long long i = (long long)blockIdx.x * T + t; i < q.pb.P; i += (long long)gridDim.x * T) {
@@ -446,22 +407,12 @@ int pic_check(const char* who, int M, int K, int num_points, int num_iter, int m
     return rc;
 }
 
-// CTA size for per_thread bytes of scratch after fixed bytes per CTA; 0 (with an error message) if none fits
-int it_threads(const char* who, size_t fixed, size_t per_thread, int M, int K, size_t* smem) {
-    const int th = sb_dense::scratch_threads(per_thread, kItSmemCap - fixed, smem);
-    if (!th)
-        sb_set_error("%s: M = %d, K = %d needs %zu bytes of shared-memory scratch per problem, the limit is %zu", who, M,
-                     K, per_thread, kItSmemCap - fixed);
-    *smem += fixed;
-    return th;
-}
-
-int ep_run(const char* who, const ItProblem& pb, const float* levels, int num_points, int l, float beta, int output,
+int ep_run(const char* who, const MimoProblem& pb, const float* levels, int num_points, int l, float beta, int output,
            int hard_out, void* out, cudaStream_t stream) {
     const int m = 31 - __builtin_clz((unsigned)num_points), hb = m / 2;
     const size_t per = sizeof(float2) * it_base_size(pb.M, pb.K) + sizeof(float) * ep_real_size(pb.K);
     size_t smem = 0;
-    const int th = it_threads(who, 16 * sizeof(float), per, pb.M, pb.K, &smem);
+    const int th = sb_dense::detector_threads(who, 16 * sizeof(float), per, pb.M, pb.K, &smem);
     if (!th) return SB_EUNSUPPORTED;
     EpParams q{pb, levels, out, 1 << hb, hb, l, output, hard_out, beta};
     SB_CUDA(cudaFuncSetAttribute(ep_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -470,12 +421,12 @@ int ep_run(const char* who, const ItProblem& pb, const float* levels, int num_po
     return SB_OK;
 }
 
-int pic_run(const char* who, const ItProblem& pb, const float* prior, const float* points, int num_points, int num_iter,
+int pic_run(const char* who, const MimoProblem& pb, const float* prior, const float* points, int num_points, int num_iter,
             int method, int hard_out, float* out, cudaStream_t stream) {
     const int m = 31 - __builtin_clz((unsigned)num_points);
     const size_t per = sizeof(float2) * (it_base_size(pb.M, pb.K) + pic_size(pb.K)) + sizeof(float) * pb.K * m;
     size_t smem = 0;
-    const int th = it_threads(who, sizeof(float2) * num_points, per, pb.M, pb.K, &smem);
+    const int th = sb_dense::detector_threads(who, sizeof(float2) * num_points, per, pb.M, pb.K, &smem);
     if (!th) return SB_EUNSUPPORTED;
     PicParams q{pb, (const float2*)points, prior, out, num_iter, hard_out};
     return sb_dispatch<0, 1>(method, [&](auto METHOD) {
@@ -489,33 +440,6 @@ int pic_run(const char* who, const ItProblem& pb, const float* prior, const floa
     });
 }
 
-ItProblem dense_problem(const float* y, const float* h, const float* s, long long num, int M, int K) {
-    ItProblem pb{};
-    pb.y = (const float2*)y; pb.h = (const float2*)h; pb.s = (const float2*)s;
-    pb.is_ofdm = 0; pb.P = num; pb.M = M; pb.K = K;
-    return pb;
-}
-
-ItProblem ofdm_problem(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
-                       const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired,
-                       const int32_t* d_undesired, const int32_t* d_out_stream, const int32_t* d_data_pos,
-                       int64_t batch, int num_rx, int num_rx_ant, int num_tx_streams, int num_symbols,
-                       int num_subcarriers, int streams_per_rx, int interferers_per_rx, int num_data) {
-    ItProblem pb{};
-    OfdmEqParams& p = pb.ofdm;
-    p.y = (const float2*)d_y; p.hhat = (const float2*)d_h_hat; p.ev = d_err_var; p.no = d_no;
-    for (int i = 0; i < 6; ++i) p.ev_stride[i] = h_ev_stride[i];
-    for (int i = 0; i < 3; ++i) p.no_stride[i] = h_no_stride[i];
-    p.des = d_desired; p.und = d_undesired; p.out_ts = d_out_stream; p.data_pos = d_data_pos;
-    p.B = batch; p.RX = num_rx; p.ANT = num_rx_ant; p.TXS = num_tx_streams;
-    p.S = num_symbols; p.F = num_subcarriers; p.K = streams_per_rx; p.KU = interferers_per_rx; p.ND = num_data;
-    pb.is_ofdm = 1;
-    pb.P = batch * num_rx * (long long)num_symbols * num_subcarriers;
-    pb.M = num_rx_ant;
-    pb.K = streams_per_rx;
-    return pb;
-}
-
 }  // namespace
 
 extern "C" int sb_mimo_ep(const float* d_y, const float* d_h, const float* d_s, const float* d_levels, void* d_out,
@@ -525,7 +449,7 @@ extern "C" int sb_mimo_ep(const float* d_y, const float* d_h, const float* d_s, 
     if (rc != SB_OK) return rc;
     if (num == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_y && d_h && d_s && d_levels && d_out && num > 0, "sb_mimo_ep: bad arguments");
-    return ep_run("sb_mimo_ep", dense_problem(d_y, d_h, d_s, num, M, K), d_levels, num_points, l, beta, output,
+    return ep_run("sb_mimo_ep", sb_dense::dense_problem(d_y, d_h, d_s, num, M, K), d_levels, num_points, l, beta, output,
                   hard_out, d_out, (cudaStream_t)stream);
 }
 
@@ -539,12 +463,14 @@ extern "C" int sb_ofdm_ep(const float* d_y, const float* d_h_hat, const float* d
     const int rc = ep_check("sb_ofdm_ep", num_rx_ant, streams_per_rx, num_points, l, beta, output, hard_out);
     if (rc != SB_OK) return rc;
     if (batch == 0) return SB_OK;                       // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_y && d_h_hat && d_err_var && h_ev_stride && d_no && h_no_stride && d_desired && d_out_stream &&
-                     d_data_pos && d_levels && d_out && batch > 0 && (interferers_per_rx == 0 || d_undesired),
-                 "sb_ofdm_ep: bad arguments");
-    const ItProblem pb = ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired, d_undesired,
-                                      d_out_stream, d_data_pos, batch, num_rx, num_rx_ant, num_tx_streams, num_symbols,
-                                      num_subcarriers, streams_per_rx, interferers_per_rx, num_data);
+    const int ac = sb_dense::ofdm_check("sb_ofdm_ep", d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired,
+                                        d_undesired, d_out_stream, d_data_pos, d_levels, d_out, batch, num_rx_ant,
+                                        interferers_per_rx);
+    if (ac != SB_OK) return ac;
+    const MimoProblem pb = sb_dense::ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired,
+                                                  d_undesired, d_out_stream, d_data_pos, batch, num_rx, num_rx_ant,
+                                                  num_tx_streams, num_symbols, num_subcarriers, streams_per_rx,
+                                                  interferers_per_rx, num_data);
     return ep_run("sb_ofdm_ep", pb, d_levels, num_points, l, beta, output, hard_out, d_out, (cudaStream_t)stream);
 }
 
@@ -555,7 +481,7 @@ extern "C" int sb_mimo_mmse_pic(const float* d_y, const float* d_h, const float*
     if (rc != SB_OK) return rc;
     if (num == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_y && d_h && d_s && d_points && d_out && num > 0, "sb_mimo_mmse_pic: bad arguments");
-    return pic_run("sb_mimo_mmse_pic", dense_problem(d_y, d_h, d_s, num, M, K), d_prior, d_points, num_points, num_iter,
+    return pic_run("sb_mimo_mmse_pic", sb_dense::dense_problem(d_y, d_h, d_s, num, M, K), d_prior, d_points, num_points, num_iter,
                    method, hard_out, d_out, (cudaStream_t)stream);
 }
 
@@ -570,12 +496,14 @@ extern "C" int sb_ofdm_mmse_pic(const float* d_y, const float* d_h_hat, const fl
     const int rc = pic_check("sb_ofdm_mmse_pic", num_rx_ant, streams_per_rx, num_points, num_iter, method, hard_out);
     if (rc != SB_OK) return rc;
     if (batch == 0) return SB_OK;                       // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_y && d_h_hat && d_err_var && h_ev_stride && d_no && h_no_stride && d_desired && d_out_stream &&
-                     d_data_pos && d_points && d_out && batch > 0 && (interferers_per_rx == 0 || d_undesired),
-                 "sb_ofdm_mmse_pic: bad arguments");
-    const ItProblem pb = ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired, d_undesired,
-                                      d_out_stream, d_data_pos, batch, num_rx, num_rx_ant, num_tx_streams, num_symbols,
-                                      num_subcarriers, streams_per_rx, interferers_per_rx, num_data);
+    const int ac = sb_dense::ofdm_check("sb_ofdm_mmse_pic", d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride,
+                                        d_desired, d_undesired, d_out_stream, d_data_pos, d_points, d_out, batch,
+                                        num_rx_ant, interferers_per_rx);
+    if (ac != SB_OK) return ac;
+    const MimoProblem pb = sb_dense::ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired,
+                                                  d_undesired, d_out_stream, d_data_pos, batch, num_rx, num_rx_ant,
+                                                  num_tx_streams, num_symbols, num_subcarriers, streams_per_rx,
+                                                  interferers_per_rx, num_data);
     return pic_run("sb_ofdm_mmse_pic", pb, d_prior, d_points, num_points, num_iter, method, hard_out, d_out,
                    (cudaStream_t)stream);
 }

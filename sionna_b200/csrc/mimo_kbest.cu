@@ -7,10 +7,10 @@
 // warp keeps a problem's whole path list in shared memory and nothing per path leaves the chip.
 //
 // Two launches per call (as mimo_ml.cu: the prologue's scratch would otherwise cap the search's occupancy):
-//   1. kbest_prologue_kernel, one thread per problem: S -> L = chol(S), y_w = L^-1 y, H_w = L^-1 H, the squared norm of
-//      every whitened column, the column order (descending norm, ties: lower index first, an insertion sort), then the
-//      modified Gram-Schmidt of the sorted [H_w | y_w] (qr_record): R (upper triangular, R_jj real >= 0) and
-//      ybar = Q^H y_w. The out-of-span term is dropped: every path metric shares it.
+//   1. kbest_prologue_kernel, one thread per problem: y_w and H_w from the detectors' shared loader (load_whitened,
+//      dense_mimo.cuh), the squared norm of every whitened column, the column order (descending norm, ties: lower index
+//      first, an insertion sort), then the modified Gram-Schmidt of the sorted [H_w | y_w] (qr_record): R (upper
+//      triangular, R_jj real >= 0) and ybar = Q^H y_w. The out-of-span term is dropped: every path metric shares it.
 //      Real representation (real_rep = 1, QAM only): realify(S) / 2 = F F^T with F = realify(L) / sqrt(2), so the
 //      whitened real channel is sqrt(2) [[Re H_w, -Im H_w], [Im H_w, Re H_w]] with y = sqrt(2) [Re y_w; Im y_w]. It is
 //      the reference's whitened channel up to an orthogonal factor, which leaves every metric unchanged. Columns k and
@@ -38,53 +38,31 @@
 namespace {
 
 using sb_dense::Scratch;
-using sb_dense::OfdmEqParams;
+using sb_dense::MimoProblem;
+using sb_dense::qr_record_size;
 
 constexpr int kKbMaxLayers = 16;
 constexpr int kKbMaxK = 256;
 constexpr int kKbMaxPoints = 256;
 constexpr int kKbMaxChildren = 16384;
-constexpr size_t kKbSmemCap = 200 * 1024;
-
-__host__ __device__ constexpr int kb_record_size(int S) { return S * S + S + 1; }   // float2 per problem
 
 size_t kb_workspace_bytes(long long P, int K, int real_rep) {
     const int S = K << real_rep;
-    return (sizeof(float2) * kb_record_size(S) + sizeof(long long) * K + sizeof(int) * S) * (size_t)P;
+    return (sizeof(float2) * qr_record_size(S) + sizeof(long long) * K + sizeof(int) * S) * (size_t)P;
 }
 
-// One thread per problem. Dense: y [P, M], h [P, M, K], s [P, M, M]; output position of stream k = p K + k.
-// OFDM (is_ofdm): problem = resource element, output positions from the stream tables (-1: no data; elements without
-// data for any stream are skipped). Scratch per thread: S [M, M], H [M, K], Y [M] and, real_rep, H_r [2M, 2K], Y_r [2M].
-__global__ void kbest_prologue_kernel(const float2* __restrict__ y, const float2* __restrict__ h,
-                                      const float2* __restrict__ s, int is_ofdm, const OfdmEqParams ofdm, long long P,
-                                      int M, int K, int real_rep, float2* __restrict__ recs, long long* __restrict__ oidx,
-                                      int* __restrict__ orders) {
+// One thread per problem (load_whitened, then the column order and qr_record); output positions to oidx [P, K].
+// Scratch per thread: S [M, M], H [M, K], Y [M] and, real_rep, H_r [2M, 2K], Y_r [2M].
+__global__ void kbest_prologue_kernel(const MimoProblem pb, int real_rep, float2* __restrict__ recs,
+                                      long long* __restrict__ oidx, int* __restrict__ orders) {
     extern __shared__ float2 smem[];
-    const int T = blockDim.x, t = threadIdx.x;
+    const int T = blockDim.x, t = threadIdx.x, M = pb.M, K = pb.K;
     const int S = K << real_rep, MR = M << real_rep;
     const size_t o_h = (size_t)M * M, o_y = o_h + (size_t)M * K, o_hr = o_y + M, o_yr = o_hr + (size_t)MR * S;
     const Scratch Sc{smem, T, t}, H{smem + o_h * T, T, t}, Y{smem + o_y * T, T, t};
     const Scratch HR{smem + o_hr * T, T, t}, YR{smem + o_yr * T, T, t};
-    for (long long i = (long long)blockIdx.x * T + t; i < P; i += (long long)gridDim.x * T) {
-        if (is_ofdm) {
-            const sb_dense::OfdmRe e = sb_dense::ofdm_re(ofdm, i);
-            bool any = false;
-            for (int k = 0; k < K; ++k) {
-                const long long o = sb_dense::ofdm_out_index(ofdm, e, k);
-                oidx[i * K + k] = o;
-                any = any || o >= 0;
-            }
-            if (!any) continue;
-            sb_dense::ofdm_load_re(ofdm, e, Y, H, Sc);
-        } else {
-            for (int k = 0; k < K; ++k) oidx[i * K + k] = i * K + k;
-            for (int e = 0; e < M * M; ++e) Sc(e) = s[i * M * M + e];
-            for (int e = 0; e < M * K; ++e) H(e) = h[i * M * K + e];
-            for (int e = 0; e < M; ++e) Y(e) = y[i * M + e];
-        }
-        sb_dense::chol_lower(Sc, M);
-        sb_dense::whiten(Sc, Y, H, M, K);
+    for (long long i = (long long)blockIdx.x * T + t; i < pb.P; i += (long long)gridDim.x * T) {
+        if (!sb_dense::load_whitened(pb, i, Sc, H, Y, oidx + i * K)) continue;
         float nrm[kKbMaxLayers];
         for (int k = 0; k < K; ++k) {
             float n2 = 0.f;
@@ -99,7 +77,7 @@ __global__ void kbest_prologue_kernel(const float2* __restrict__ y, const float2
             ord[j] = d;
         }
         for (int d = 0; d < S; ++d) orders[i * S + d] = ord[d];
-        float2* rec = recs + i * kb_record_size(S);
+        float2* rec = recs + i * qr_record_size(S);
         if (real_rep) {
             const float r2 = 1.41421356237309515f;
             for (int m = 0; m < M; ++m) {
@@ -174,7 +152,7 @@ __global__ void __launch_bounds__(256) kbest_search_kernel(const KbParams q) {
         bool any = false;
         for (int k = 0; k < K; ++k) any = any || oi[k] >= 0;
         if (!any) continue;
-        const float2* rec = q.rec + p * kb_record_size(S);
+        const float2* rec = q.rec + p * qr_record_size(S);
         const int* ord = q.order + p * S;
         __syncwarp();                                   // the previous problem's finish step has read the path list
         if (lane == 0) {
@@ -295,12 +273,7 @@ __global__ void __launch_bounds__(256) kbest_search_kernel(const KbParams q) {
                     if (ord[s2] == K + ks) pos_im = s2;
                 }
                 int idx = cur[pos_re];
-                if (q.real_rep) {                       // PAM2QAM: real part on the even bit positions
-                    const int mh = m >> 1, re = cur[pos_re], im = cur[pos_im];
-                    idx = 0;
-                    for (int j = 0; j < mh; ++j)
-                        idx |= (((re >> (mh - 1 - j)) & 1) << (m - 1 - 2 * j)) | (((im >> (mh - 1 - j)) & 1) << (m - 2 - 2 * j));
-                }
+                if (q.real_rep) idx = sb_dense::pam2qam_index(cur[pos_re], cur[pos_im], m);
                 if (q.symbol) {
                     reinterpret_cast<int*>(q.out)[o] = idx;
                 } else {
@@ -367,10 +340,11 @@ int kb_check(const char* who, int M, int K, int num_points, int k, int real_rep,
     return SB_OK;
 }
 
-// Both launches on the caller's workspace of P records; ofdm == nullptr for dense problems.
-int kb_run(const char* who, const float2* y, const float2* h, const float2* s, const OfdmEqParams* ofdm, long long P,
-           int M, int K, const float* points, int num_points, int k, int real_rep, int output, int hard_out, float clip,
-           void* out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+// Both launches on the caller's workspace of P records.
+int kb_run(const char* who, const MimoProblem& pb, const float* points, int num_points, int k, int real_rep, int output,
+           int hard_out, float clip, void* out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+    const long long P = pb.P;
+    const int M = pb.M, K = pb.K;
     if (!ws || ws_bytes < kb_workspace_bytes(P, K, real_rep)) {
         sb_set_error("%s: the workspace needs %zu bytes (sb_kbest_workspace_bytes), %zu given", who,
                      kb_workspace_bytes(P, K, real_rep), ws ? ws_bytes : (size_t)0);
@@ -382,24 +356,19 @@ int kb_run(const char* who, const float2* y, const float2* h, const float2* s, c
     size_t psmem = 0;
     const size_t p_thread = sizeof(float2) * ((size_t)M * M + (size_t)M * K + M +
                                               (real_rep ? (size_t)MR * S + MR : 0));
-    const int pthreads = sb_dense::scratch_threads(p_thread, kKbSmemCap, &psmem);
-    if (!pthreads) {
-        sb_set_error("%s: M = %d, K = %d needs %zu bytes of shared-memory scratch per problem, the limit is %zu", who, M,
-                     K, p_thread, kKbSmemCap);
-        return SB_EUNSUPPORTED;
-    }
+    const int pthreads = sb_dense::detector_threads(who, 0, p_thread, M, K, &psmem);
+    if (!pthreads) return SB_EUNSUPPORTED;
     int kpad = 1;
     while (kpad < k) kpad <<= 1;
     const size_t per_warp = (sizeof(unsigned long long) * kpad + sizeof(float2) * k + sizeof(float) * k +
                              sizeof(unsigned) * 256 + 2 * (size_t)k * S + 7) / 8 * 8;
-    const int warps = (int)std::min<size_t>(8, (kKbSmemCap - NP * sizeof(float2)) / per_warp);
+    const int warps = (int)std::min<size_t>(8, (sb_dense::kScratchSmemCap - NP * sizeof(float2)) / per_warp);
     const size_t esmem = NP * sizeof(float2) + per_warp * warps;
     float2* recs = (float2*)ws;
-    long long* oidx = (long long*)((char*)ws + sizeof(float2) * kb_record_size(S) * (size_t)P);
+    long long* oidx = (long long*)((char*)ws + sizeof(float2) * qr_record_size(S) * (size_t)P);
     int* orders = (int*)((char*)oidx + sizeof(long long) * K * (size_t)P);
     SB_CUDA(cudaFuncSetAttribute(kbest_prologue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-    kbest_prologue_kernel<<<sb_grid(P, pthreads, 16), pthreads, psmem, stream>>>(
-        y, h, s, ofdm != nullptr, ofdm ? *ofdm : OfdmEqParams{}, P, M, K, real_rep, recs, oidx, orders);
+    kbest_prologue_kernel<<<sb_grid(P, pthreads, 16), pthreads, psmem, stream>>>(pb, real_rep, recs, oidx, orders);
     SB_LAUNCH_CHECK();
     KbParams q{recs, oidx, orders, points, out, P, S, K, NP, 31 - __builtin_clz((unsigned)NP), bits, k, kpad, real_rep,
                output, hard_out, clip, (int)per_warp};
@@ -425,9 +394,8 @@ extern "C" int sb_mimo_kbest(const float* d_y, const float* d_h, const float* d_
     if (rc != SB_OK) return rc;
     if (num == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_y && d_h && d_s && d_points && d_out && num > 0, "sb_mimo_kbest: bad arguments");
-    return kb_run("sb_mimo_kbest", (const float2*)d_y, (const float2*)d_h, (const float2*)d_s, nullptr, num, M, K,
-                  d_points, num_points, k, real_rep, output, hard_out, llr_clip, d_out, d_workspace, workspace_bytes,
-                  (cudaStream_t)stream);
+    return kb_run("sb_mimo_kbest", sb_dense::dense_problem(d_y, d_h, d_s, num, M, K), d_points, num_points, k, real_rep,
+                  output, hard_out, llr_clip, d_out, d_workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int sb_ofdm_kbest(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
@@ -442,17 +410,14 @@ extern "C" int sb_ofdm_kbest(const float* d_y, const float* d_h_hat, const float
                             llr_clip);
     if (rc != SB_OK) return rc;
     if (batch == 0) return SB_OK;                       // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_y && d_h_hat && d_err_var && h_ev_stride && d_no && h_no_stride && d_desired && d_out_stream &&
-                     d_data_pos && d_points && d_out && batch > 0 && (interferers_per_rx == 0 || d_undesired),
-                 "sb_ofdm_kbest: bad arguments");
-    OfdmEqParams p{};
-    p.y = (const float2*)d_y; p.hhat = (const float2*)d_h_hat; p.ev = d_err_var; p.no = d_no;
-    for (int i = 0; i < 6; ++i) p.ev_stride[i] = h_ev_stride[i];
-    for (int i = 0; i < 3; ++i) p.no_stride[i] = h_no_stride[i];
-    p.des = d_desired; p.und = d_undesired; p.out_ts = d_out_stream; p.data_pos = d_data_pos;
-    p.B = batch; p.RX = num_rx; p.ANT = num_rx_ant; p.TXS = num_tx_streams;
-    p.S = num_symbols; p.F = num_subcarriers; p.K = streams_per_rx; p.KU = interferers_per_rx; p.ND = num_data;
-    const long long P = batch * num_rx * (long long)num_symbols * num_subcarriers;
-    return kb_run("sb_ofdm_kbest", nullptr, nullptr, nullptr, &p, P, num_rx_ant, streams_per_rx, d_points, num_points, k,
-                  real_rep, output, hard_out, llr_clip, d_out, d_workspace, workspace_bytes, (cudaStream_t)stream);
+    const int ac = sb_dense::ofdm_check("sb_ofdm_kbest", d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride,
+                                        d_desired, d_undesired, d_out_stream, d_data_pos, d_points, d_out, batch,
+                                        num_rx_ant, interferers_per_rx);
+    if (ac != SB_OK) return ac;
+    const MimoProblem pb = sb_dense::ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired,
+                                                  d_undesired, d_out_stream, d_data_pos, batch, num_rx, num_rx_ant,
+                                                  num_tx_streams, num_symbols, num_subcarriers, streams_per_rx,
+                                                  interferers_per_rx, num_data);
+    return kb_run("sb_ofdm_kbest", pb, d_points, num_points, k, real_rep, output, hard_out, llr_clip, d_out, d_workspace,
+                  workspace_bytes, (cudaStream_t)stream);
 }

@@ -7,8 +7,8 @@
 // here nothing per candidate leaves the chip.
 //
 // Two launches per call:
-//   1. ml_prologue_kernel, one thread per problem (scratch in shared memory, as the LMMSE kernels): S -> L = chol(S),
-//      whitening y_w = L^-1 y, H_w = L^-1 H, then modified Gram-Schmidt on [H_w | y_w]:
+//   1. ml_prologue_kernel, one thread per problem (scratch in shared memory, as the LMMSE kernels): the detectors'
+//      shared loader (load_whitened, dense_mimo.cuh) gives y_w and H_w, then modified Gram-Schmidt on [H_w | y_w]:
 //        H_w = Q R (R upper trapezoidal K x K, rows >= min(M, K) zero),  yq = Q^H y_w,  c0 = ||y_w - Q yq||^2,
 //      so that ||y_w - H_w x||^2 = c0 + ||yq - R x||^2 for every x. The record (R, yq, c0: 8 (K^2 + K + 1) bytes) and the
 //      K output positions go to the caller's workspace in HBM (sb_ml_workspace_bytes): the prologue needs
@@ -36,44 +36,21 @@
 namespace {
 
 using sb_dense::Scratch;
-using sb_dense::OfdmEqParams;
+using sb_dense::MimoProblem;
+using sb_dense::qr_record_size;
+using sb_dense::kScratchSmemCap;
 
 constexpr int kMlMaxK = 8;
 constexpr long long kMlMaxCandidates = 65536;
 constexpr int kMlMaxPoints = 1024;
-constexpr size_t kMlSmemCap = 200 * 1024;
-
-__host__ __device__ constexpr int ml_record_size(int K) { return K * K + K + 1; }   // float2 per problem
-
-// One thread per problem. Dense: y [P, M], h [P, M, K], s [P, M, M]; output position of stream k = p K + k.
-// OFDM (is_ofdm): problem = resource element (b, rx, symbol, subcarrier), output positions from the stream
-// tables (-1: no data; elements without data for any stream are skipped).
-__global__ void ml_prologue_kernel(const float2* __restrict__ y, const float2* __restrict__ h,
-                                   const float2* __restrict__ s, int is_ofdm, const OfdmEqParams ofdm, long long P, int M, int K, float2* __restrict__ recs,
-                                   long long* __restrict__ oidx) {
+// One thread per problem (load_whitened, then qr_record in the identity order); output positions to oidx [P, K]
+__global__ void ml_prologue_kernel(const MimoProblem pb, float2* __restrict__ recs, long long* __restrict__ oidx) {
     extern __shared__ float2 smem[];
-    const int T = blockDim.x, t = threadIdx.x;
+    const int T = blockDim.x, t = threadIdx.x, M = pb.M, K = pb.K;
     const Scratch S{smem, T, t}, H{smem + (size_t)M * M * T, T, t}, Y{smem + (size_t)(M * M + M * K) * T, T, t};
-    for (long long i = (long long)blockIdx.x * T + t; i < P; i += (long long)gridDim.x * T) {
-        if (is_ofdm) {
-            const sb_dense::OfdmRe e = sb_dense::ofdm_re(ofdm, i);
-            bool any = false;
-            for (int k = 0; k < K; ++k) {
-                const long long o = sb_dense::ofdm_out_index(ofdm, e, k);
-                oidx[i * K + k] = o;
-                any = any || o >= 0;
-            }
-            if (!any) continue;
-            sb_dense::ofdm_load_re(ofdm, e, Y, H, S);
-        } else {
-            for (int k = 0; k < K; ++k) oidx[i * K + k] = i * K + k;
-            for (int e = 0; e < M * M; ++e) S(e) = s[i * M * M + e];
-            for (int e = 0; e < M * K; ++e) H(e) = h[i * M * K + e];
-            for (int e = 0; e < M; ++e) Y(e) = y[i * M + e];
-        }
-        sb_dense::chol_lower(S, M);
-        sb_dense::whiten(S, Y, H, M, K);
-        sb_dense::qr_record(Y, H, M, K, [](int j) { return j; }, recs + i * ml_record_size(K));
+    for (long long i = (long long)blockIdx.x * T + t; i < pb.P; i += (long long)gridDim.x * T) {
+        if (!sb_dense::load_whitened(pb, i, S, H, Y, oidx + i * K)) continue;
+        sb_dense::qr_record(Y, H, M, K, [](int j) { return j; }, recs + i * qr_record_size(K));
     }
 }
 
@@ -213,7 +190,7 @@ __global__ void __launch_bounds__(256) ml_enum_kernel(const MlParams q) {
 #pragma unroll
         for (int k = 0; k < K; ++k) any = any || oi[k] >= 0;
         if (!any) continue;
-        const float2* rec = q.rec + p * ml_record_size(K);
+        const float2* rec = q.rec + p * qr_record_size(K);
         float2 R[K][K], yq[K];
 #pragma unroll
         for (int r = 0; r < K; ++r) {
@@ -337,15 +314,16 @@ int ml_check(const char* who, int K, int num_points, int method, int output, int
     return SB_OK;
 }
 
-// workspace: P records of ml_record_size(K) float2, then P x K output positions (int64)
+// workspace: P records of qr_record_size(K) float2, then P x K output positions (int64)
 size_t ml_workspace_bytes(long long P, int K) {
-    return (sizeof(float2) * ml_record_size(K) + sizeof(long long) * K) * (size_t)P;
+    return (sizeof(float2) * qr_record_size(K) + sizeof(long long) * K) * (size_t)P;
 }
 
-// Both launches on the caller's workspace of P records; ofdm == nullptr for dense problems.
-int ml_run(const char* who, const float2* y, const float2* h, const float2* s, const OfdmEqParams* ofdm, long long P,
-           int M, int K, const float* prior, const float* points, int NP, int method, int output, int hard_out,
-           void* out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+// Both launches on the caller's workspace of P records.
+int ml_run(const char* who, const MimoProblem& pb, const float* prior, const float* points, int NP, int method,
+           int output, int hard_out, void* out, void* ws, size_t ws_bytes, cudaStream_t stream) {
+    const long long P = pb.P;
+    const int M = pb.M, K = pb.K;
     if (!ws || ws_bytes < ml_workspace_bytes(P, K)) {
         sb_set_error("%s: the workspace needs %zu bytes (sb_ml_workspace_bytes), %zu given", who, ml_workspace_bytes(P, K),
                      ws ? ws_bytes : (size_t)0);
@@ -353,12 +331,8 @@ int ml_run(const char* who, const float2* y, const float2* h, const float2* s, c
     }
     size_t psmem = 0;
     const size_t p_thread = sizeof(float2) * ((size_t)M * M + (size_t)M * K + M);
-    const int pthreads = sb_dense::scratch_threads(p_thread, kMlSmemCap, &psmem);
-    if (!pthreads) {
-        sb_set_error("%s: M = %d, K = %d needs %zu bytes of shared-memory scratch per problem, the limit is %zu", who, M,
-                     K, p_thread, kMlSmemCap);
-        return SB_EUNSUPPORTED;
-    }
+    const int pthreads = sb_dense::detector_threads(who, 0, p_thread, M, K, &psmem);
+    if (!pthreads) return SB_EUNSUPPORTED;
     const int AK = K * NP, bits = 31 - __builtin_clz((unsigned)NP);
     long long NO = 1;
     for (int k = 1; k < K; ++k) NO *= NP;
@@ -368,24 +342,23 @@ int ml_run(const char* who, const float2* y, const float2* h, const float2* s, c
     int ethreads = 0;
     if (warp) {
         const size_t per_warp = sizeof(float) * AK * (33 + hp);
-        const int warps = (int)std::min<size_t>(8, (kMlSmemCap - NP * sizeof(float2)) / per_warp);
+        const int warps = (int)std::min<size_t>(8, (kScratchSmemCap - NP * sizeof(float2)) / per_warp);
         ethreads = 32 * warps;
         esmem = NP * sizeof(float2) + per_warp * warps;
     } else {
         const size_t per_thread = sizeof(float) * AK * (2 + hp);
-        ethreads = sb_dense::scratch_threads(per_thread, kMlSmemCap - NP * sizeof(float2), &esmem);
+        ethreads = sb_dense::scratch_threads(per_thread, kScratchSmemCap - NP * sizeof(float2), &esmem);
         esmem += NP * sizeof(float2);
     }
-    if (!ethreads || esmem > kMlSmemCap) {
+    if (!ethreads || esmem > kScratchSmemCap) {
         sb_set_error("%s: %d streams of %d points need more shared memory per problem than %zu bytes", who, K, NP,
-                     kMlSmemCap);
+                     kScratchSmemCap);
         return SB_EUNSUPPORTED;
     }
     float2* recs = (float2*)ws;
-    long long* oidx = (long long*)((char*)ws + sizeof(float2) * ml_record_size(K) * (size_t)P);
+    long long* oidx = (long long*)((char*)ws + sizeof(float2) * qr_record_size(K) * (size_t)P);
     SB_CUDA(cudaFuncSetAttribute(ml_prologue_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)psmem));
-    ml_prologue_kernel<<<sb_grid(P, pthreads, 16), pthreads, psmem, stream>>>(
-        y, h, s, ofdm != nullptr, ofdm ? *ofdm : OfdmEqParams{}, P, M, K, recs, oidx);
+    ml_prologue_kernel<<<sb_grid(P, pthreads, 16), pthreads, psmem, stream>>>(pb, recs, oidx);
     SB_LAUNCH_CHECK();
     MlParams q{recs, oidx, (const float2*)points, prior, out, P, NP, bits, method, output, hard_out};
     return sb_dispatch<1, kMlMaxK>(K, [&](auto KC) -> int {
@@ -416,9 +389,8 @@ extern "C" int sb_mimo_ml(const float* d_y, const float* d_h, const float* d_s, 
     if (rc != SB_OK) return rc;
     if (num == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
     SB_CHECK_ARG(d_y && d_h && d_s && d_points && d_out && num > 0 && M >= 1, "sb_mimo_ml: bad arguments");
-    return ml_run("sb_mimo_ml", (const float2*)d_y, (const float2*)d_h, (const float2*)d_s, nullptr, num, M, K, d_prior,
-                  d_points, num_points, method, output, hard_out, d_out, d_workspace, workspace_bytes,
-                  (cudaStream_t)stream);
+    return ml_run("sb_mimo_ml", sb_dense::dense_problem(d_y, d_h, d_s, num, M, K), d_prior, d_points, num_points,
+                  method, output, hard_out, d_out, d_workspace, workspace_bytes, (cudaStream_t)stream);
 }
 
 extern "C" int sb_ofdm_ml(const float* d_y, const float* d_h_hat, const float* d_err_var, const int64_t* h_ev_stride,
@@ -432,18 +404,14 @@ extern "C" int sb_ofdm_ml(const float* d_y, const float* d_h_hat, const float* d
     const int rc = ml_check("sb_ofdm_ml", streams_per_rx, num_points, method, output, hard_out);
     if (rc != SB_OK) return rc;
     if (batch == 0) return SB_OK;                       // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_y && d_h_hat && d_err_var && h_ev_stride && d_no && h_no_stride && d_desired && d_out_stream &&
-                     d_data_pos && d_points && d_out && batch > 0 && num_rx_ant >= 1 &&
-                     (interferers_per_rx == 0 || d_undesired),
-                 "sb_ofdm_ml: bad arguments");
-    OfdmEqParams p{};
-    p.y = (const float2*)d_y; p.hhat = (const float2*)d_h_hat; p.ev = d_err_var; p.no = d_no;
-    for (int i = 0; i < 6; ++i) p.ev_stride[i] = h_ev_stride[i];
-    for (int i = 0; i < 3; ++i) p.no_stride[i] = h_no_stride[i];
-    p.des = d_desired; p.und = d_undesired; p.out_ts = d_out_stream; p.data_pos = d_data_pos;
-    p.B = batch; p.RX = num_rx; p.ANT = num_rx_ant; p.TXS = num_tx_streams;
-    p.S = num_symbols; p.F = num_subcarriers; p.K = streams_per_rx; p.KU = interferers_per_rx; p.ND = num_data;
-    const long long P = batch * num_rx * (long long)num_symbols * num_subcarriers;
-    return ml_run("sb_ofdm_ml", nullptr, nullptr, nullptr, &p, P, num_rx_ant, streams_per_rx, d_prior, d_points,
-                  num_points, method, output, hard_out, d_out, d_workspace, workspace_bytes, (cudaStream_t)stream);
+    const int ac = sb_dense::ofdm_check("sb_ofdm_ml", d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired,
+                                        d_undesired, d_out_stream, d_data_pos, d_points, d_out, batch, num_rx_ant,
+                                        interferers_per_rx);
+    if (ac != SB_OK) return ac;
+    const MimoProblem pb = sb_dense::ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride, d_desired,
+                                                  d_undesired, d_out_stream, d_data_pos, batch, num_rx, num_rx_ant,
+                                                  num_tx_streams, num_symbols, num_subcarriers, streams_per_rx,
+                                                  interferers_per_rx, num_data);
+    return ml_run("sb_ofdm_ml", pb, d_prior, d_points, num_points, method, output, hard_out, d_out, d_workspace,
+                  workspace_bytes, (cudaStream_t)stream);
 }

@@ -1293,7 +1293,7 @@ extern "C" int sb_pusch_ls_combine(float* d_h, float* d_err_var, int64_t rows, i
 }
 
 using sb_dense::scratch_threads;
-constexpr size_t kLmmseSmemCap = 200 * 1024;
+using sb_dense::kScratchSmemCap;
 
 extern "C" int sb_lmmse_equalize(const float* d_y, const float* d_h, const float* d_s, float* d_x_hat, float* d_no_eff,
                                  int64_t num, int32_t M, int32_t K, void* stream) {
@@ -1302,10 +1302,10 @@ extern "C" int sb_lmmse_equalize(const float* d_y, const float* d_h, const float
                  "sb_lmmse_equalize: bad arguments (need 1 <= K <= 16, K <= M)");
     size_t smem = 0;
     const size_t per_thread = sizeof(float2) * LmmseScratch::elems(M, K);
-    int threads = scratch_threads(per_thread, kLmmseSmemCap, &smem);
+    int threads = scratch_threads(per_thread, kScratchSmemCap, &smem);
     if (!threads) {
         sb_set_error("sb_lmmse_equalize: M = %d, K = %d needs %zu bytes of shared-memory scratch per vector, the limit is %zu",
-                     M, K, per_thread, kLmmseSmemCap);
+                     M, K, per_thread, kScratchSmemCap);
         return SB_EUNSUPPORTED;
     }
     SB_CUDA(cudaFuncSetAttribute(lmmse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -1352,15 +1352,14 @@ extern "C" int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float
                      d_data_pos && d_x_hat && d_no_eff && batch >= 0 && streams_per_rx >= 1 && streams_per_rx <= 16 &&
                      streams_per_rx <= num_rx_ant && (interferers_per_rx == 0 || d_undesired),
                  "sb_ofdm_lmmse: bad arguments (need 1 <= streams_per_rx <= min(16, num_rx_ant))");
-    if (batch == 0) return SB_OK;
-    OfdmEqParams p{};
-    p.y = (const float2*)d_y; p.hhat = (const float2*)d_h_hat; p.ev = d_err_var; p.no = d_no;
-    for (int i = 0; i < 6; ++i) p.ev_stride[i] = h_ev_stride[i];
-    for (int i = 0; i < 3; ++i) p.no_stride[i] = h_no_stride[i];
-    p.des = d_desired; p.und = d_undesired; p.out_ts = d_out_stream; p.data_pos = d_data_pos;
-    p.xh = (float2*)d_x_hat; p.ne = d_no_eff; p.B = batch; p.RX = num_rx; p.ANT = num_rx_ant; p.TXS = num_tx_streams;
-    p.S = num_symbols; p.F = num_subcarriers; p.K = streams_per_rx; p.KU = interferers_per_rx; p.ND = num_data;
-    long long total_re = batch * num_rx * (long long)num_symbols * num_subcarriers;
+    const sb_dense::MimoProblem pb = sb_dense::ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride,
+                                                            d_desired, d_undesired, d_out_stream, d_data_pos, batch,
+                                                            num_rx, num_rx_ant, num_tx_streams, num_symbols,
+                                                            num_subcarriers, streams_per_rx, interferers_per_rx,
+                                                            num_data);
+    OfdmEqParams p = pb.ofdm;
+    p.xh = (float2*)d_x_hat; p.ne = d_no_eff;
+    const long long total_re = pb.P;
     if (interferers_per_rx == 0 && streams_per_rx <= 4) {     // diagonal noise covariance: register kernel
         sb_dispatch<1, 4>(streams_per_rx, [&](auto K) {
             ofdm_lmmse_diag_kernel<K><<<sb_grid(total_re, 128, 16), 128, 0, (cudaStream_t)stream>>>(p);
@@ -1371,10 +1370,10 @@ extern "C" int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float
     }
     size_t smem = 0;
     const size_t per_thread = sizeof(float2) * LmmseScratch::elems(num_rx_ant, streams_per_rx);
-    int threads = scratch_threads(per_thread, kLmmseSmemCap, &smem);
+    int threads = scratch_threads(per_thread, kScratchSmemCap, &smem);
     if (!threads) {
         sb_set_error("sb_ofdm_lmmse: %d receive antennas, %d streams need %zu bytes of shared-memory scratch per resource "
-                     "element, the limit is %zu", num_rx_ant, streams_per_rx, per_thread, kLmmseSmemCap);
+                     "element, the limit is %zu", num_rx_ant, streams_per_rx, per_thread, kScratchSmemCap);
         return SB_EUNSUPPORTED;
     }
     SB_CUDA(cudaFuncSetAttribute(ofdm_lmmse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

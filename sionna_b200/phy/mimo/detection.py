@@ -63,11 +63,21 @@ def ml_check_limits(num_streams, num_points):
                          f"{ML_MAX_CANDIDATES} and constellations of at most {ML_MAX_POINTS} points")
 
 
-def ml_workspace(num_problems, num_streams, device):
-    """Workspace of ``sb_mimo_ml`` / ``sb_ofdm_ml`` from PyTorch's caching allocator (whitened triangular records and
-    output positions, ``sb_ml_workspace_bytes``)."""
-    n = int(lib().sb_ml_workspace_bytes(int(num_problems), int(num_streams)))
-    return torch.empty(max(n, 8), dtype=torch.uint8, device=device)
+def detector_workspace(nbytes, device):
+    """Workspace of ``nbytes`` for the ML and K-Best entry points (``sb_ml_workspace_bytes`` /
+    ``sb_kbest_workspace_bytes``) from PyTorch's caching allocator."""
+    return torch.empty(max(int(nbytes), 8), dtype=torch.uint8, device=device)
+
+
+def detector_out(output, hard_out, num_bits_per_symbol, shape, device):
+    """Uninitialised detector output: LLRs / hard bits ``[*shape, m]`` (``output="bit"``), int32 symbol indices
+    ``[*shape]`` (``output="symbol"`` with ``hard_out``) or symbol logits ``[*shape, 2**m]``."""
+    m = num_bits_per_symbol
+    if output == "bit":
+        return torch.empty(shape + [m], dtype=torch.float32, device=device)
+    if hard_out:
+        return torch.empty(shape, dtype=torch.int32, device=device)
+    return torch.empty(shape + [2 ** m], dtype=torch.float32, device=device)
 
 
 def llrs_to_symbol_logits(llrs, num_bits_per_symbol):
@@ -76,6 +86,21 @@ def llrs_to_symbol_logits(llrs, num_bits_per_symbol):
     m = num_bits_per_symbol
     a = 2.0 * ((torch.arange(2 ** m, device=llrs.device)[:, None] >> torch.arange(m - 1, -1, -1, device=llrs.device)) & 1) - 1.0
     return torch.nn.functional.logsigmoid(llrs[..., None, :] * a.to(llrs.dtype)).sum(-1)
+
+
+def _dense_inputs(y, h, s, k, dev):
+    """(y [B, M], h [B, M, K], s [B, M, M] complex64 contiguous, batch shape, M, number of problems) after broadcasting
+    the batch dimensions of the three inputs."""
+    h = torch.as_tensor(h).to(device=dev, dtype=torch.complex64)
+    mm = h.shape[-2]
+    if h.shape[-1] != k:
+        raise ValueError(f"h must have num_streams = {k} as last dimension")
+    batch = torch.broadcast_shapes(tuple(torch.as_tensor(y).shape[:-1]), tuple(h.shape[:-2]),
+                                   tuple(torch.as_tensor(s).shape[:-2]))
+    y = torch.as_tensor(y).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm]).contiguous()
+    h = h.expand(list(batch) + [mm, k]).contiguous()
+    s = torch.as_tensor(s).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm, mm]).contiguous()
+    return y, h, s, list(batch), mm, int(np.prod(batch)) if len(batch) else 1
 
 
 class MaximumLikelihoodDetector(Block):
@@ -110,30 +135,16 @@ class MaximumLikelihoodDetector(Block):
         dev = self.device
         k, m = self._num_streams, self._constellation.num_bits_per_symbol
         npts = 2 ** m
-        h = torch.as_tensor(h).to(device=dev, dtype=torch.complex64)
-        mm = h.shape[-2]
-        if h.shape[-1] != k:
-            raise ValueError(f"h must have num_streams = {k} as last dimension")
-        batch = torch.broadcast_shapes(tuple(torch.as_tensor(y).shape[:-1]), tuple(h.shape[:-2]),
-                                       tuple(torch.as_tensor(s).shape[:-2]))
-        y = torch.as_tensor(y).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm]).contiguous()
-        h = h.expand(list(batch) + [mm, k]).contiguous()
-        s = torch.as_tensor(s).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm, mm]).contiguous()
-        num = int(np.prod(batch)) if len(batch) else 1
+        y, h, s, batch, mm, num = _dense_inputs(y, h, s, k, dev)
         pr = None
         if prior is not None:
             pr = torch.as_tensor(prior).to(device=dev, dtype=torch.float32)
             if self._output == "bit":
                 pr = llrs_to_symbol_logits(pr, m)
-            pr = pr.expand(list(batch) + [k, npts]).contiguous()
-        if self._output == "bit":
-            out = torch.empty(list(batch) + [k, m], dtype=torch.float32, device=dev)
-        elif self._hard_out:
-            out = torch.empty(list(batch) + [k], dtype=torch.int32, device=dev)
-        else:
-            out = torch.empty(list(batch) + [k, npts], dtype=torch.float32, device=dev)
+            pr = pr.expand(batch + [k, npts]).contiguous()
+        out = detector_out(self._output, self._hard_out, m, batch + [k], dev)
         pts = self._constellation().to(device=dev, dtype=torch.complex64).contiguous()
-        ws = ml_workspace(num, k, dev)
+        ws = detector_workspace(lib().sb_ml_workspace_bytes(num, k), dev)
         check(lib().sb_mimo_ml(ptr(y), ptr(h), ptr(s), ptr(pr), ptr(pts), ptr(out), ptr(ws), ws.numel(), num, mm, k, npts,
                                self._method, int(self._output == "symbol"), int(self._hard_out), current_stream()),
               "sb_mimo_ml")
@@ -156,13 +167,6 @@ def kbest_check_limits(num_layers, k, num_points):
     if k > KB_MAX_K or num_points > KB_MAX_POINTS or k * num_points > KB_MAX_CHILDREN:
         raise ValueError(f"KBestDetector: k = {k} paths of a {num_points}-point detection constellation; supported are "
                          f"k <= {KB_MAX_K}, at most {KB_MAX_POINTS} points and k * points <= {KB_MAX_CHILDREN}")
-
-
-def kbest_workspace(num_problems, num_streams, real_rep, device):
-    """Workspace of ``sb_mimo_kbest`` / ``sb_ofdm_kbest`` from PyTorch's caching allocator (sorted triangular records,
-    column orders and output positions, ``sb_kbest_workspace_bytes``)."""
-    n = int(lib().sb_kbest_workspace_bytes(int(num_problems), int(num_streams), int(real_rep)))
-    return torch.empty(max(n, 8), dtype=torch.uint8, device=device)
 
 
 class List2LLR(Block):
@@ -286,22 +290,10 @@ class KBestDetector(Block):
     def call(self, y, h, s):
         dev = self.device
         k, m = self._num_tx_streams, self._num_bits_out
-        h = torch.as_tensor(h).to(device=dev, dtype=torch.complex64)
-        mm = h.shape[-2]
-        if h.shape[-1] != k:
-            raise ValueError(f"h must have num_streams = {k} as last dimension")
-        batch = torch.broadcast_shapes(tuple(torch.as_tensor(y).shape[:-1]), tuple(h.shape[:-2]),
-                                       tuple(torch.as_tensor(s).shape[:-2]))
-        y = torch.as_tensor(y).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm]).contiguous()
-        h = h.expand(list(batch) + [mm, k]).contiguous()
-        s = torch.as_tensor(s).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm, mm]).contiguous()
-        num = int(np.prod(batch)) if len(batch) else 1
-        if self._output == "bit":
-            out = torch.empty(list(batch) + [k, m], dtype=torch.float32, device=dev)
-        else:
-            out = torch.empty(list(batch) + [k], dtype=torch.int32, device=dev)
+        y, h, s, batch, mm, num = _dense_inputs(y, h, s, k, dev)
+        out = detector_out(self._output, self._hard_out, m, batch + [k], dev)
         pts, kk, real_rep, symbol, hard, clip = self._kernel_args(dev)
-        ws = kbest_workspace(num, k, real_rep, dev)
+        ws = detector_workspace(lib().sb_kbest_workspace_bytes(num, k, real_rep), dev)
         check(lib().sb_mimo_kbest(ptr(y), ptr(h), ptr(s), ptr(pts), ptr(out), ptr(ws), ws.numel(), num, mm, k, 2 ** m,
                                   kk, real_rep, symbol, hard, clip, current_stream()), "sb_mimo_kbest")
         return out
@@ -331,21 +323,6 @@ def symbol_logits_to_llrs(logits, num_bits_per_symbol, method):
     ninf = torch.tensor(-float("inf"), dtype=logits.dtype, device=logits.device)
     red = (lambda v: torch.logsumexp(v, dim=-2)) if method == "app" else (lambda v: torch.amax(v, dim=-2))
     return red(torch.where(lab, x, ninf)) - red(torch.where(~lab, x, ninf))
-
-
-def _dense_inputs(y, h, s, k, dev):
-    """(y [B, M], h [B, M, K], s [B, M, M] complex64 contiguous, batch shape, M, number of problems) after broadcasting
-    the batch dimensions of the three inputs."""
-    h = torch.as_tensor(h).to(device=dev, dtype=torch.complex64)
-    mm = h.shape[-2]
-    if h.shape[-1] != k:
-        raise ValueError(f"h must have num_streams = {k} as last dimension")
-    batch = torch.broadcast_shapes(tuple(torch.as_tensor(y).shape[:-1]), tuple(h.shape[:-2]),
-                                   tuple(torch.as_tensor(s).shape[:-2]))
-    y = torch.as_tensor(y).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm]).contiguous()
-    h = h.expand(list(batch) + [mm, k]).contiguous()
-    s = torch.as_tensor(s).to(device=dev, dtype=torch.complex64).expand(list(batch) + [mm, mm]).contiguous()
-    return y, h, s, list(batch), mm, int(np.prod(batch)) if len(batch) else 1
 
 
 class EPDetector(Block):
@@ -383,20 +360,12 @@ class EPDetector(Block):
         return (self._levels_dev, 2 ** self._num_bits_per_symbol, self._l, self._beta, int(self._output == "symbol"),
                 int(self._hard_out))
 
-    def _out(self, shape, dev):
-        m = self._num_bits_per_symbol
-        if self._output == "bit":
-            return torch.empty(shape + [m], dtype=torch.float32, device=dev)
-        if self._hard_out:
-            return torch.empty(shape, dtype=torch.int32, device=dev)
-        return torch.empty(shape + [2 ** m], dtype=torch.float32, device=dev)
-
     def call(self, y, h, s):
         dev = self.device
         k = torch.as_tensor(h).shape[-1]
         iterative_check_limits("EPDetector", k, 2 ** self._num_bits_per_symbol, EP_MAX_POINTS)
         y, h, s, batch, mm, num = _dense_inputs(y, h, s, k, dev)
-        out = self._out(batch + [k], dev)
+        out = detector_out(self._output, self._hard_out, self._num_bits_per_symbol, batch + [k], dev)
         lev, npts, l, beta, symbol, hard = self._kernel_args(dev)
         check(lib().sb_mimo_ep(ptr(y), ptr(h), ptr(s), ptr(lev), ptr(out), num, mm, k, npts, l, beta, symbol, hard,
                                current_stream()), "sb_mimo_ep")

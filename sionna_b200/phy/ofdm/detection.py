@@ -3,14 +3,13 @@
 ``MaximumLikelihoodDetector`` / ``MaximumLikelihoodDetectorWithPrior`` = fused covariance assembly + ML detection
 (``sb_ofdm_ml``); ``KBestDetector``, ``EPDetector`` and ``MMSEPICDetector`` = the same assembly + K-Best, EP or
 MMSE-PIC detection (``sb_ofdm_kbest``, ``sb_ofdm_ep``, ``sb_ofdm_mmse_pic``)."""
-import numpy as np
 import torch
 
 from ..._lib import lib, check, ptr, current_stream
 from ..block import Block
 from ..mapping import Constellation, Demapper
-from ..mimo.detection import (llrs_to_symbol_logits, ml_check_limits, ml_workspace, KBestDetector as _MimoKBest,
-                              kbest_workspace, EPDetector as _MimoEP, MMSEPICDetector as _MimoPIC,
+from ..mimo.detection import (llrs_to_symbol_logits, ml_check_limits, detector_workspace, detector_out,
+                              KBestDetector as _MimoKBest, EPDetector as _MimoEP, MMSEPICDetector as _MimoPIC,
                               iterative_check_limits, EP_MAX_POINTS, PIC_MAX_POINTS)
 from .equalization import LMMSEEqualizer, OFDMEqualizer
 
@@ -76,14 +75,9 @@ class MaximumLikelihoodDetector(Block):
         return self._detect(y, h_hat, None, err_var, no)
 
     def _detect(self, y, h_hat, prior, err_var, no):
-        eq = self._eq
-        rg, sm = eq._resource_grid, eq._stream_management
-        dev = self.device
-        y_eff, h, ev, ev_st, no_t, no_st = eq._kernel_inputs(y, h_hat, err_var, no)
-        b, rx, ant, s_, f_ = y_eff.shape
-        txs = sm.num_tx * sm.num_streams_per_tx
-        des, und, out_ts, data_pos = eq._tables(dev)
-        nd = rg.pilot_pattern.num_data_symbols
+        dev, sm = self.device, self._eq._stream_management
+        ptrs, sizes, _alive, nd = self._eq._cabi_args(y, h_hat, err_var, no)
+        b, rx, _, txs, s_, f_ = sizes[:6]
         m = self._constellation.num_bits_per_symbol
         npts = 2 ** m
         pr = None
@@ -92,23 +86,12 @@ class MaximumLikelihoodDetector(Block):
             if self._output == "bit":
                 pr = llrs_to_symbol_logits(pr.reshape(b, txs, nd, m), m)
             pr = pr.reshape(b, txs, nd, npts).contiguous()
-        shp = [b, sm.num_tx, sm.num_streams_per_tx]
-        if self._output == "bit":
-            out = torch.zeros(shp + [nd * m], dtype=torch.float32, device=dev)
-        elif self._hard_out:
-            out = torch.zeros(shp + [nd], dtype=torch.int32, device=dev)
-        else:
-            out = torch.zeros(shp + [nd, npts], dtype=torch.float32, device=dev)
+        out = detector_out(self._output, self._hard_out, m, [b, sm.num_tx, sm.num_streams_per_tx, nd], dev).zero_()
         pts = self._constellation().to(device=dev, dtype=torch.complex64).contiguous()
-        ev_arr = np.asarray(ev_st, np.int64)                    # host stride arrays: alive until the call returns
-        no_arr = np.asarray(no_st, np.int64)
-        ws = ml_workspace(b * rx * s_ * f_, sm.num_streams_per_rx, dev)
-        check(lib().sb_ofdm_ml(ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
-                               ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos), ptr(pr), ptr(pts), ptr(out),
-                               ptr(ws), ws.numel(), b, rx, ant, txs, s_, f_,
-                               sm.num_streams_per_rx, sm.num_interfering_streams_per_rx, nd, npts, self._method,
+        ws = detector_workspace(lib().sb_ml_workspace_bytes(b * rx * s_ * f_, sm.num_streams_per_rx), dev)
+        check(lib().sb_ofdm_ml(*ptrs, ptr(pr), ptr(pts), ptr(out), ptr(ws), ws.numel(), *sizes, npts, self._method,
                                int(self._output == "symbol"), int(self._hard_out), current_stream()), "sb_ofdm_ml")
-        return out
+        return out.flatten(-2) if self._output == "bit" else out
 
 
 class MaximumLikelihoodDetectorWithPrior(MaximumLikelihoodDetector):
@@ -154,49 +137,18 @@ class KBestDetector(Block):
         return self._detector.list2llr
 
     def call(self, y, h_hat, err_var, no):
-        eq, det = self._eq, self._detector
-        rg, sm = eq._resource_grid, eq._stream_management
-        dev = self.device
-        y_eff, h, ev, ev_st, no_t, no_st = eq._kernel_inputs(y, h_hat, err_var, no)
-        b, rx, ant, s_, f_ = y_eff.shape
+        dev, det, sm = self.device, self._detector, self._eq._stream_management
+        ptrs, sizes, _alive, nd = self._eq._cabi_args(y, h_hat, err_var, no)
+        b, rx, ant, _, s_, f_ = sizes[:6]
         if ant < sm.num_streams_per_rx:
             raise AssertionError("The number of receive antennas cannot be smaller than the number of streams")
-        txs = sm.num_tx * sm.num_streams_per_tx
-        des, und, out_ts, data_pos = eq._tables(dev)
-        nd = rg.pilot_pattern.num_data_symbols
         m = det._num_bits_out
-        shp = [b, sm.num_tx, sm.num_streams_per_tx]
-        if self._output == "bit":
-            out = torch.zeros(shp + [nd * m], dtype=torch.float32, device=dev)
-        else:
-            out = torch.zeros(shp + [nd], dtype=torch.int32, device=dev)
+        out = detector_out(self._output, det._hard_out, m, [b, sm.num_tx, sm.num_streams_per_tx, nd], dev).zero_()
         pts, kk, real_rep, symbol, hard, clip = det._kernel_args(dev)
-        ev_arr = np.asarray(ev_st, np.int64)                    # host stride arrays: alive until the call returns
-        no_arr = np.asarray(no_st, np.int64)
-        ws = kbest_workspace(b * rx * s_ * f_, sm.num_streams_per_rx, real_rep, dev)
-        check(lib().sb_ofdm_kbest(ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
-                                  ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos), ptr(pts), ptr(out),
-                                  ptr(ws), ws.numel(), b, rx, ant, txs, s_, f_, sm.num_streams_per_rx,
-                                  sm.num_interfering_streams_per_rx, nd, 2 ** m, kk, real_rep, symbol, hard, clip,
-                                  current_stream()), "sb_ofdm_kbest")
-        return out
-
-
-def _ofdm_kernel_inputs(eq, y, h_hat, err_var, no, dev):
-    """(leading C-ABI arguments up to d_data_pos, [batch .. num_data] sizes, host stride arrays kept alive by the
-    caller, num_data) of the OFDM detector entry points."""
-    rg, sm = eq._resource_grid, eq._stream_management
-    y_eff, h, ev, ev_st, no_t, no_st = eq._kernel_inputs(y, h_hat, err_var, no)
-    b, rx, ant, s_, f_ = y_eff.shape
-    txs = sm.num_tx * sm.num_streams_per_tx
-    des, und, out_ts, data_pos = eq._tables(dev)
-    nd = rg.pilot_pattern.num_data_symbols
-    ev_arr = np.asarray(ev_st, np.int64)
-    no_arr = np.asarray(no_st, np.int64)
-    ptrs = [ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
-            ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos)]
-    sizes = [b, rx, ant, txs, s_, f_, sm.num_streams_per_rx, sm.num_interfering_streams_per_rx, nd]
-    return ptrs, sizes, (ev_arr, no_arr, y_eff, h, ev, no_t), nd
+        ws = detector_workspace(lib().sb_kbest_workspace_bytes(b * rx * s_ * f_, sm.num_streams_per_rx, real_rep), dev)
+        check(lib().sb_ofdm_kbest(*ptrs, ptr(pts), ptr(out), ptr(ws), ws.numel(), *sizes, 2 ** m, kk, real_rep, symbol,
+                                  hard, clip, current_stream()), "sb_ofdm_kbest")
+        return out.flatten(-2) if self._output == "bit" else out
 
 
 class EPDetector(Block):
@@ -219,9 +171,10 @@ class EPDetector(Block):
 
     def call(self, y, h_hat, err_var, no):
         dev, det, sm = self.device, self._detector, self._eq._stream_management
-        ptrs, sizes, _alive, nd = _ofdm_kernel_inputs(self._eq, y, h_hat, err_var, no, dev)
+        ptrs, sizes, _alive, nd = self._eq._cabi_args(y, h_hat, err_var, no)
         lev, npts, l, beta, symbol, hard = det._kernel_args(dev)
-        out = det._out([sizes[0], sm.num_tx, sm.num_streams_per_tx, nd], dev).zero_()
+        out = detector_out(det._output, det._hard_out, det._num_bits_per_symbol,
+                           [sizes[0], sm.num_tx, sm.num_streams_per_tx, nd], dev).zero_()
         check(lib().sb_ofdm_ep(*ptrs, ptr(lev), ptr(out), *sizes, npts, l, beta, symbol, hard, current_stream()),
               "sb_ofdm_ep")
         return out.flatten(-2) if det._output == "bit" else out
@@ -255,7 +208,7 @@ class MMSEPICDetector(Block):
 
     def call(self, y, h_hat, prior, err_var, no):
         dev, det, sm = self.device, self._detector, self._eq._stream_management
-        ptrs, sizes, _alive, nd = _ofdm_kernel_inputs(self._eq, y, h_hat, err_var, no, dev)
+        ptrs, sizes, _alive, nd = self._eq._cabi_args(y, h_hat, err_var, no)
         m = det.constellation.num_bits_per_symbol
         shp = [sizes[0], sm.num_tx, sm.num_streams_per_tx, nd]
         pr = torch.as_tensor(prior)

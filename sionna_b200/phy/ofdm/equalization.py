@@ -62,24 +62,32 @@ class OFDMEqualizer(Block):
     def call(self, y, h_hat, err_var, no):
         if self.precision != "single":
             raise NotImplementedError("OFDM equalisation runs complex64 kernels only.")
-        rg, sm = self._resource_grid, self._stream_management
-        dev = self.device
+        if self._equalizer != "lmmse":
+            return self._unfused(*self._kernel_inputs(y, h_hat, err_var, no))
+        sm = self._stream_management
+        ptrs, sizes, _alive, nd = self._cabi_args(y, h_hat, err_var, no)
+        shp = (sizes[0], sm.num_tx, sm.num_streams_per_tx, nd)
+        x_hat = torch.zeros(shp, dtype=torch.complex64, device=self.device)
+        no_eff = torch.zeros(shp, dtype=torch.float32, device=self.device)
+        check(lib().sb_ofdm_lmmse(*ptrs, ptr(x_hat), ptr(no_eff), *sizes, current_stream()), "sb_ofdm_lmmse")
+        return x_hat, no_eff
+
+    def _cabi_args(self, y, h_hat, err_var, no):
+        """The arguments ``sb_ofdm_lmmse`` and the OFDM detector entry points share: (pointers d_y ... d_data_pos,
+        sizes batch ... num_data, the tensors and host stride arrays the caller keeps alive until the call returns,
+        num_data)."""
+        sm = self._stream_management
         y_eff, h, ev, ev_st, no_t, no_st = self._kernel_inputs(y, h_hat, err_var, no)
         b, rx, ant, s_, f_ = y_eff.shape
-        txs = sm.num_tx * sm.num_streams_per_tx
-        des, und, out_ts, data_pos = self._tables(dev)
-        nd = rg.pilot_pattern.num_data_symbols
-        if self._equalizer != "lmmse":
-            return self._unfused(y_eff, h, ev, ev_st, no_t, no_st)
-        x_hat = torch.zeros((b, sm.num_tx, sm.num_streams_per_tx, nd), dtype=torch.complex64, device=dev)
-        no_eff = torch.zeros((b, sm.num_tx, sm.num_streams_per_tx, nd), dtype=torch.float32, device=dev)
-        ev_arr = (np.asarray(ev_st, np.int64))
-        no_arr = (np.asarray(no_st, np.int64))
-        check(lib().sb_ofdm_lmmse(ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
-                                  ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos), ptr(x_hat), ptr(no_eff),
-                                  b, rx, ant, txs, s_, f_, sm.num_streams_per_rx, sm.num_interfering_streams_per_rx, nd,
-                                  current_stream()), "sb_ofdm_lmmse")
-        return x_hat, no_eff
+        des, und, out_ts, data_pos = self._tables(self.device)
+        nd = self._resource_grid.pilot_pattern.num_data_symbols
+        ev_arr = np.asarray(ev_st, np.int64)
+        no_arr = np.asarray(no_st, np.int64)
+        ptrs = [ptr(y_eff), ptr(h), ptr(ev), ptr(ev_arr), ptr(no_t), ptr(no_arr), ptr(des),
+                ptr(und) if und.numel() else None, ptr(out_ts), ptr(data_pos)]
+        sizes = [b, rx, ant, sm.num_tx * sm.num_streams_per_tx, s_, f_, sm.num_streams_per_rx,
+                 sm.num_interfering_streams_per_rx, nd]
+        return ptrs, sizes, (ev_arr, no_arr, y_eff, h, ev, no_t), nd
 
     def _kernel_inputs(self, y, h_hat, err_var, no):
         """The fused kernels' inputs: y [B, rx, ant, S, F] without nulled subcarriers, h [B, rx, ant, txs, S, F] and
