@@ -277,6 +277,24 @@ int sb_apply_time_channel(const float* d_x, const float* d_h, const float* d_no,
 int sb_tdl_sos(const float* d_doppler, const float* d_theta, const float* d_phi, const float* d_phi0,
                const float* d_powers, float los_power, float los_aoa, float* d_a, int64_t batch, int32_t num_ant_pairs,
                int32_t num_paths, int32_t num_sinusoids, int32_t num_time_steps, float sampling_frequency, void* stream);
+/* CDL.__call__ (channel/tr38901/cdl.py:258-332 and channel_coefficients.py:459-1030, no sub-clustering): cluster
+ * coefficients of TR 38.901 (7.5-22), (7.5-28)..(7.5-30) summed over 20 rays. Draws: d_speed, d_v_phi, d_v_theta
+ * [batch]; d_coupling [batch, 4, clusters, 20] normals whose per-cluster argsort permutes the arrival azimuth, departure
+ * azimuth, arrival zenith and departure zenith of the rays (in that order); d_phases [batch, clusters, 20, 4] initial
+ * phases. Per-instance tables over the rows c * 400 + zenith_index * 20 + azimuth_index (c in table order) plus one LoS
+ * row at clusters * 400: d_rx_dir [rows, 3] arrival unit vectors, d_rx_field / d_tx_field [rows, 4] GCS fields (pol 1
+ * theta, phi, pol 2 theta, phi), d_rx_phase [rows, num_rx_ant] / d_tx_phase [rows, num_tx_ant] complex antenna phases;
+ * d_rx_pol / d_tx_pol [ant] polarization index 0 / 1; d_cluster_scale [clusters] = sqrt(P_c / 20) (times sqrt(1 / (K +
+ * 1)) for LoS models); d_order [clusters]: table cluster of output cluster o (ascending delay); d_los_field [4] LoS gains
+ * (rx pol major, times sqrt(K / (K + 1))) or NULL for NLoS models; xpr_scale = sqrt(1 / XPR); wavenumber = 2 pi / lambda.
+ * -> d_a [batch, num_rx_ant, num_tx_ant, clusters, time_steps] complex, written once, no atomics. clusters <= 24. */
+int sb_cdl_coefficients(const float* d_speed, const float* d_v_phi, const float* d_v_theta, const float* d_coupling,
+                        const float* d_phases, const float* d_rx_dir, const float* d_rx_field, const float* d_rx_phase,
+                        const int32_t* d_rx_pol, const float* d_tx_field, const float* d_tx_phase,
+                        const int32_t* d_tx_pol, const float* d_cluster_scale, const int32_t* d_order,
+                        const float* d_los_field, float xpr_scale, float wavenumber, float* d_a, int64_t batch,
+                        int32_t num_clusters, int32_t num_rx_ant, int32_t num_tx_ant, int32_t num_time_steps,
+                        float sampling_frequency, void* stream);
 /* CIR -> channel conversion without eager tensor expressions (channel/utils.py:180-350), csrc/channel.cu.
  * sb_phase_table: d_e [n_tab, paths, cols] complex; mode 0: exp(-j 2 pi x_j tau[tab, p]) (x = subcarrier frequencies,
  *   cir_to_ofdm_channel :232-244); mode 1: sinc(x_j - tau[tab, p] * scale) (x = tap lags l, scale = bandwidth,

@@ -59,6 +59,7 @@ SIGNATURES = {
     "sb_apply_time_channel": (i32, [vp, vp, vp, i64, vp, i64, i32, i32, i32, i32, i32, u64, u64, vp]),
     "sb_uniform": (i32, [vp, i64, f32, f32, u64, u64, vp]),
     "sb_tdl_sos": (i32, [vp, vp, vp, vp, vp, f32, f32, vp, i64, i32, i32, i32, i32, f32, vp]),
+    "sb_cdl_coefficients": (i32, [vp] * 15 + [f32, f32, vp, i64, i32, i32, i32, i32, f32, vp]),
     "sb_phase_table": (i32, [vp, vp, f32, i32, vp, i64, i32, i32, vp]),
     "sb_cir_gram": (i32, [vp, vp, i64, i32, i32, vp]),
     "sb_cir_link_scale": (i32, [vp, vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, f32, vp]),

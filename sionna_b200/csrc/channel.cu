@@ -292,6 +292,165 @@ __global__ void tdl_sos_kernel(const float* __restrict__ doppler, const float* _
     }
 }
 
+// CDL cluster coefficients (TR 38.901 (7.5-22), (7.5-28)..(7.5-30) without sub-clustering):
+//   a[b, u, v, o, t] = sum_r g_r[pol(u), pol(v)] A_rx[rx_r, u] A_tx[tx_r, v] exp(j w_r t)   (+ the LoS ray on o = 0)
+// for output cluster o = table cluster c = order[o]. Ray r of cluster c takes the arrival angles (zenith index
+// perm_zoa[r], azimuth index perm_aoa[r]) and the departure angles likewise, perm = argsort of the coupling normals; rx_r
+// and tx_r are the rows c * 400 + zenith * 20 + azimuth of the per-instance tables. g_r = F_rx^T M_r F_tx scaled by
+// sqrt(P_c / 20) (and sqrt(1 / (K + 1))), M_r = [[e^{j p0}, x e^{j p1}], [x e^{j p2}, e^{j p3}]], x = sqrt(1 / XPR);
+// w_r = k (r_rx . v) / fs is the Doppler phase per sample with the arrival unit vector r_rx.
+// A CTA owns one batch element and a tile of up to kCdlTile time steps:
+//   1. ranks the 4 x C x 20 coupling normals (comparison counts, ties broken by index as a stable argsort does);
+//   2. builds the per-ray record (table rows, 4 polarization gains, Doppler rate) in shared memory;
+//   3. evaluates the C x 20 (+ 1) Doppler phasors of the tile once, for every antenna pair;
+//   4. thread = (antenna pair, output cluster): the 20 (21) ray coefficients in registers, one complex MAC per ray and
+//      time step; the tile goes through shared memory so that the stores are contiguous runs of the
+//      [batch, rx ant, tx ant, cluster, time] output, which is written exactly once.
+// Shared-memory arrays are indexed with the cluster innermost: adjacent lanes read adjacent words.
+constexpr int kCdlRays = 20;
+constexpr int kCdlTile = 16;
+constexpr int kCdlThreads = 256;
+constexpr int kCdlMaxClusters = 24;
+struct CdlArgs {
+    const float *speed, *v_phi, *v_theta, *coupling, *phases, *rx_dir, *rx_field, *tx_field, *cluster_scale, *los_field;
+    const float2 *rx_phase, *tx_phase;
+    const int *rx_pol, *tx_pol, *order;
+    float xpr_scale, wavenumber, fs;
+    float2* out;
+    long long B;
+    int C, NR, NT, T;
+};
+
+__global__ void __launch_bounds__(kCdlThreads) cdl_kernel(CdlArgs p) {
+    extern __shared__ float2 s_cdl[];
+    const int C = p.C, CR = C * kCdlRays;
+    float2* s_dop = s_cdl;                                          // [20][tile][C] + LoS [tile]
+    float2* s_out = s_dop + (size_t)(CR + 1) * kCdlTile;            // [threads][tile + 1]
+    float2* s_g = s_out + (size_t)kCdlThreads * (kCdlTile + 1);     // [20][4][C] + LoS [4]
+    float* s_w = (float*)(s_g + (size_t)4 * CR + 4);                // [20][C] + LoS
+    int* s_rx = (int*)(s_w + CR + 1);                               // [20][C]
+    int* s_tx = s_rx + CR;                                          // [20][C]
+    unsigned char* s_perm = (unsigned char*)(s_tx + CR);            // [4][C][20]
+    const bool los = p.los_field != nullptr;
+    const int tiles = (p.T + kCdlTile - 1) / kCdlTile;
+    const int pairs = p.NR * p.NT, items = pairs * C;
+    for (long long blk = blockIdx.x; blk < p.B * tiles; blk += gridDim.x) {
+        const long long b = blk / tiles;
+        const int t0 = (int)(blk % tiles) * kCdlTile;
+        const int nt = min(kCdlTile, p.T - t0);
+        __syncthreads();
+        for (int i = threadIdx.x; i < 4 * CR; i += blockDim.x) {
+            const float* x = p.coupling + (b * 4 * C + i / kCdlRays) * kCdlRays;
+            const int r = i % kCdlRays;
+            const float v = x[r];
+            int rank = 0;
+            for (int j = 0; j < kCdlRays; ++j) rank += (x[j] < v) || (x[j] == v && j < r);
+            s_perm[i - r + rank] = (unsigned char)r;
+        }
+        __syncthreads();
+        const float sp = p.speed[b], vph = p.v_phi[b], vth = p.v_theta[b];
+        const float vx = sp * cosf(vph) * sinf(vth), vy = sp * sinf(vph) * sinf(vth), vz = sp * cosf(vth);
+        const float kw = p.wavenumber / p.fs;
+        for (int i = threadIdx.x; i < CR + 1; i += blockDim.x) {
+            if (i == CR) {                                          // the LoS ray: fixed gains, LoS arrival direction
+                if (los) {
+                    const float* d = p.rx_dir + (size_t)CR * kCdlRays * 3;
+                    s_w[CR] = kw * (d[0] * vx + d[1] * vy + d[2] * vz);
+                    for (int k = 0; k < 4; ++k) s_g[4 * CR + k] = make_float2(p.los_field[k], 0.f);
+                }
+                continue;
+            }
+            const int c = i / kCdlRays, r = i % kCdlRays;
+            const int ia = s_perm[(0 * C + c) * kCdlRays + r], id = s_perm[(1 * C + c) * kCdlRays + r];
+            const int iz = s_perm[(2 * C + c) * kCdlRays + r], izd = s_perm[(3 * C + c) * kCdlRays + r];
+            const int rx = (c * kCdlRays + iz) * kCdlRays + ia, tx = (c * kCdlRays + izd) * kCdlRays + id;
+            const int k = r * C + c;
+            s_rx[k] = rx;
+            s_tx[k] = tx;
+            const float* d = p.rx_dir + (size_t)rx * 3;
+            s_w[k] = kw * (d[0] * vx + d[1] * vy + d[2] * vz);
+            const float* ph = p.phases + ((b * C + c) * kCdlRays + r) * 4;
+            float2 e[4];
+            for (int q = 0; q < 4; ++q) sincosf(ph[q], &e[q].y, &e[q].x);
+            const float xs = p.xpr_scale, sc = p.cluster_scale[c];
+            const float* fr = p.rx_field + (size_t)rx * 4;
+            const float* ft = p.tx_field + (size_t)tx * 4;
+            for (int pr = 0; pr < 2; ++pr)
+                for (int pt = 0; pt < 2; ++pt) {
+                    const float t_th = ft[2 * pt], t_ph = ft[2 * pt + 1];
+                    // M F_tx, then F_rx^T (M F_tx)
+                    const float2 m0 = make_float2(e[0].x * t_th + xs * e[1].x * t_ph, e[0].y * t_th + xs * e[1].y * t_ph);
+                    const float2 m1 = make_float2(xs * e[2].x * t_th + e[3].x * t_ph, xs * e[2].y * t_th + e[3].y * t_ph);
+                    const float r_th = fr[2 * pr], r_ph = fr[2 * pr + 1];
+                    s_g[(r * 4 + pr * 2 + pt) * C + c] = make_float2(sc * (r_th * m0.x + r_ph * m1.x), sc * (r_th * m0.y + r_ph * m1.y));
+                }
+        }
+        __syncthreads();
+        for (int i = threadIdx.x; i < (CR + 1) * kCdlTile; i += blockDim.x) {
+            const int tt = i / (CR + 1), k = i % (CR + 1);         // k = r * C + c, or CR for the LoS ray
+            if (k == CR && !los) continue;
+            float s, co;
+            sincosf(s_w[k] * (float)(t0 + tt), &s, &co);
+            const int r = k / C, c = k % C;
+            s_dop[k == CR ? (size_t)CR * kCdlTile + tt : ((size_t)r * kCdlTile + tt) * C + c] = make_float2(co, s);
+        }
+        __syncthreads();
+        for (int base = 0; base < items; base += kCdlThreads) {
+            const int item = base + threadIdx.x;
+            if (item < items) {
+                const int o = item % C, pair = item / C;
+                const int c = p.order[o], u = pair / p.NT, v = pair % p.NT;
+                const int pq = p.rx_pol[u] * 2 + p.tx_pol[v];
+                float2 coef[kCdlRays + 1];
+#pragma unroll
+                for (int r = 0; r < kCdlRays; ++r) {
+                    const int k = r * C + c;
+                    const float2 g = s_g[(r * 4 + pq) * C + c];
+                    const float2 ar = __ldg(p.rx_phase + (size_t)s_rx[k] * p.NR + u);
+                    const float2 at = __ldg(p.tx_phase + (size_t)s_tx[k] * p.NT + v);
+                    coef[r] = cmul(cmul(g, ar), at);
+                }
+                const bool los_here = los && o == 0;
+                coef[kCdlRays] = make_float2(0.f, 0.f);
+                if (los_here) {
+                    const size_t row = (size_t)C * kCdlRays * kCdlRays;
+                    coef[kCdlRays] = cmul(cmul(s_g[4 * CR + pq], __ldg(p.rx_phase + row * p.NR + u)),
+                                          __ldg(p.tx_phase + row * p.NT + v));
+                }
+                for (int tt = 0; tt < nt; ++tt) {
+                    float2 acc = make_float2(0.f, 0.f);
+#pragma unroll
+                    for (int r = 0; r < kCdlRays; ++r) {
+                        const float2 z = s_dop[((size_t)r * kCdlTile + tt) * C + c];
+                        acc.x += coef[r].x * z.x - coef[r].y * z.y;
+                        acc.y += coef[r].x * z.y + coef[r].y * z.x;
+                    }
+                    if (los_here) {
+                        const float2 z = s_dop[(size_t)CR * kCdlTile + tt];
+                        acc.x += coef[kCdlRays].x * z.x - coef[kCdlRays].y * z.y;
+                        acc.y += coef[kCdlRays].x * z.y + coef[kCdlRays].y * z.x;
+                    }
+                    s_out[threadIdx.x * (kCdlTile + 1) + tt] = acc;
+                }
+            }
+            __syncthreads();
+            const int n_items = min(kCdlThreads, items - base);
+            float2* op = p.out + ((b * items + base) * (long long)p.T + t0);
+            for (int i = threadIdx.x; i < n_items * nt; i += blockDim.x) {
+                const int li = i / nt, tt = i % nt;
+                op[(size_t)li * p.T + tt] = s_out[li * (kCdlTile + 1) + tt];
+            }
+            __syncthreads();
+        }
+    }
+}
+
+static size_t cdl_smem_bytes(int C) {
+    const size_t cr = (size_t)C * kCdlRays;
+    return sizeof(float2) * ((cr + 1) * kCdlTile + (size_t)kCdlThreads * (kCdlTile + 1) + 4 * cr + 4) +
+           sizeof(float) * (cr + 1) + 2 * sizeof(int) * cr + 4 * cr;
+}
+
 // ApplyOFDMChannel: y[b, r, re] = sum_t h[b, r, t, re] * x[b, t, re] + sqrt(no) CN(0,1)   (r = rx*ant, t = tx*ant)
 __global__ void apply_ofdm_channel_kernel(const float2* __restrict__ x, const float2* __restrict__ h,
                                           const float* __restrict__ no, long long no_inner, float2* __restrict__ y,
@@ -367,6 +526,33 @@ extern "C" int sb_tdl_sos(const float* d_doppler, const float* d_theta, const fl
     tdl_sos_kernel<<<sb_grid(batch * num_ant_pairs * num_paths, 128, 16), 128, 0, (cudaStream_t)stream>>>(
         d_doppler, d_theta, d_phi, d_phi0, d_powers, los_power, los_aoa, (float2*)d_a, batch, num_ant_pairs, num_paths,
         num_sinusoids, num_time_steps, sampling_frequency);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+extern "C" int sb_cdl_coefficients(const float* d_speed, const float* d_v_phi, const float* d_v_theta,
+                                   const float* d_coupling, const float* d_phases, const float* d_rx_dir,
+                                   const float* d_rx_field, const float* d_rx_phase, const int32_t* d_rx_pol,
+                                   const float* d_tx_field, const float* d_tx_phase, const int32_t* d_tx_pol,
+                                   const float* d_cluster_scale, const int32_t* d_order, const float* d_los_field,
+                                   float xpr_scale, float wavenumber, float* d_a, int64_t batch, int32_t num_clusters,
+                                   int32_t num_rx_ant, int32_t num_tx_ant, int32_t num_time_steps,
+                                   float sampling_frequency, void* stream) {
+    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    SB_CHECK_ARG(d_speed && d_v_phi && d_v_theta && d_coupling && d_phases && d_rx_dir && d_rx_field && d_rx_phase &&
+                     d_rx_pol && d_tx_field && d_tx_phase && d_tx_pol && d_cluster_scale && d_order && d_a && batch > 0 &&
+                     num_clusters > 0 && num_clusters <= kCdlMaxClusters && num_rx_ant > 0 && num_tx_ant > 0 &&
+                     num_time_steps > 0 && sampling_frequency > 0.f && xpr_scale >= 0.f,
+                 "sb_cdl_coefficients: bad arguments (1 <= num_clusters <= 24)");
+    SB_CHECK_ARG((long long)num_rx_ant * num_tx_ant * num_clusters <= INT32_MAX,
+                 "sb_cdl_coefficients: too many antenna pairs");
+    CdlArgs p{d_speed, d_v_phi, d_v_theta, d_coupling, d_phases, d_rx_dir, d_rx_field, d_tx_field, d_cluster_scale,
+              d_los_field, (const float2*)d_rx_phase, (const float2*)d_tx_phase, d_rx_pol, d_tx_pol, d_order, xpr_scale,
+              wavenumber, sampling_frequency, (float2*)d_a, batch, num_clusters, num_rx_ant, num_tx_ant, num_time_steps};
+    const size_t smem = cdl_smem_bytes(num_clusters);
+    SB_CUDA(cudaFuncSetAttribute(cdl_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const long long ctas = batch * ((num_time_steps + kCdlTile - 1) / kCdlTile);
+    cdl_kernel<<<sb_grid(ctas, 1, 16), kCdlThreads, smem, (cudaStream_t)stream>>>(p);
     SB_LAUNCH_CHECK();
     return SB_OK;
 }

@@ -43,3 +43,23 @@ for m in ("A", "B", "C", "D", "E", "A30", "B100", "C300"):   # the last three: T
     tdl[f"{m}_scale_delays"] = np.array(int(d["scale_delays"]))
     print("TDL-" + m, d["num_clusters"], "taps, los", d["los"])
 np.savez_compressed(os.path.join(os.path.dirname(__file__), "..", "sionna_b200", "phy", "channel", "tdl_models.npz"), **tdl)
+
+# ---- TR 38.901 Tables 7.7.1-1..5 CDL clusters (normalised delays, powers in dB, angles in degrees) -------------------
+# Written as text (JSON, one object per model). Rows stay in table order (not delay order); for the LoS models D and E
+# row 0 is the specular component.
+cdl = {}
+for m in ("A", "B", "C", "D", "E"):
+    with open(os.path.join(mdir, f"CDL-{m}.json")) as f:
+        d = json.load(f)
+    t = {"los": int(d["los"]), "num_clusters": int(d["num_clusters"]),
+         "delays": [float(v) for v in d["delays"]], "powers_db": [float(v) for v in d["powers"]]}
+    for k in ("aod", "aoa", "zod", "zoa"):
+        t[k] = [float(v) for v in d[k]]
+    for k in ("cASD", "cASA", "cZSD", "cZSA"):
+        t[k] = float(d[k])
+    t["xpr_db"] = float(d["xpr"])
+    cdl[m] = t
+    print("CDL-" + m, d["num_clusters"], "clusters,", len(d["delays"]), "rows, los", d["los"])
+with open(os.path.join(os.path.dirname(__file__), "..", "sionna_b200", "phy", "channel", "cdl_models.json"), "w") as f:
+    json.dump(cdl, f, indent=1)
+    f.write("\n")
