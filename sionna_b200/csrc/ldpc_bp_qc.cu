@@ -6,8 +6,9 @@
 // shifted by s) replaces every index table by arithmetic:
 //   * message slot of base entry `be` and check offset i (CN = r*Z + i):   be*Z + i
 //     - CN (r, i) walks its edges with a constant stride of Z words: no loads of indices at all;
-//     - VN (c, j) reaches the edge of entry (r, c, s) at be*Z + ((j - s) mod Z): one broadcast LDS of a packed
-//       table word + 4 integer ops; 32 consecutive VNs hit 32 consecutive words (mod the wrap): conflict free.
+//     - VN (c, j) reaches the edge of entry (r, c, s) at be*Z + ((j - s) mod Z): one broadcast LDS of a table entry
+//       in address form + 3 integer ops (vn_addr); 32 consecutive VNs hit 32 consecutive words (mod the wrap):
+//       conflict free.
 //   * a warp owns 32 consecutive checks (or variables) of ONE base row (column): degree and table entries are
 //     warp-uniform, so the min-sum update keeps the whole row in registers (fully unrolled degree buckets, one
 //     shared-memory read and one write per edge) and the VN update keeps addresses + messages in registers.
@@ -398,12 +399,25 @@ __device__ __forceinline__ int2 lds_i2(uint32_t a) {
 }
 
 // ---- variable-node update (decoding.py:714-732) for VN (c, j) -------------------------------------------------
-// msg_s / ce_s are 32-bit shared-window addresses of the message array and of the column's first table entry.
-// Returns the unclipped x_tot. MODE 0: normal update; MODE 1: initialisation v2c = llr (decoding.py:571).
-// Branch free: table entries beyond the column's degree are not read (predicate), their slot address points at the
-// VN's own first edge and the accumulate / store are predicated off.
-template <int DMAX, bool CHECK, bool KEEPM, int MODE, bool EXACT = false>   // EXACT: deg == DMAX and !CHECK: no guards
-__device__ __forceinline__ float vn_qc(uint32_t msg_s, uint32_t ce_s, int deg, int j4, int Z4, float llr, float clip) {
+// ce_s is the 32-bit shared-window address of the column's first table entry. The shared-memory copy of the column
+// table holds per edge {x, y}: x = address of message slot be*Z minus 4*s, y = 4*s << 16 | 4*zrow. With j4 = 4*j and
+// jk = j4 << 16 | 0xffff (per thread, the same for every edge) the edge's message is at x + (jk < y ? j4 + 4*Z : j4):
+// jk < y holds exactly when j < s, where (j - s) mod Z wraps. One compare, one select and one add per edge.
+struct VnLane {
+    uint32_t j4, j4w, jk;                                 // j4w = j4 + 4*Z, the offset of a wrapped edge
+};
+__device__ __forceinline__ uint32_t vn_addr(int2 e, const VnLane& v) {
+    return (uint32_t)e.x + (v.jk < (uint32_t)e.y ? v.j4w : v.j4);
+}
+// the edge exists: check offset (j - s) mod Z below the block row's zrow (partial block rows only)
+__device__ __forceinline__ bool vn_in_row(int2 e, uint32_t addr, const VnLane& v) {
+    return addr - (uint32_t)e.x - ((uint32_t)e.y >> 16) < ((uint32_t)e.y & 0xffffu);
+}
+
+// Returns the unclipped x_tot. Branch free: table entries beyond the column's degree are not read (predicate) and their
+// load, accumulate and store are predicated off.
+template <int DMAX, bool CHECK, bool KEEPM, bool EXACT = false>   // EXACT: deg == DMAX and !CHECK: no guards
+__device__ __forceinline__ float vn_qc(uint32_t ce_s, int deg, const VnLane& vl, float llr, float clip) {
     uint32_t addr[DMAX];
     float m[KEEPM ? DMAX : 1];
     bool on[DMAX];
@@ -412,85 +426,77 @@ __device__ __forceinline__ float vn_qc(uint32_t msg_s, uint32_t ce_s, int deg, i
     for (int k = 0; k < DMAX; ++k) {
         int2 e = make_int2(0, 0);
         if (EXACT || k < deg) e = lds_i2(ce_s + 8 * k);   // warp-uniform predicate
-        int t = j4 - (e.y & 0xffff);
-        t += (t >> 31) & Z4;                              // (j - s) mod Z, in bytes
-        bool ok = EXACT || ((k < deg) && (!CHECK || t < (int)((unsigned)e.y >> 16)));   // edge exists
+        addr[k] = vn_addr(e, vl);
+        bool ok = EXACT || ((k < deg) && (!CHECK || vn_in_row(e, addr[k], vl)));
         on[k] = ok;
-        addr[k] = msg_s + e.x + t;
         float v = 0.f;
-        if (MODE == 0) {
-            if (ok) v = lds_f32(addr[k]);
-            if (ok) acc = __fadd_rn(acc, v);              // :715 sequential, ascending CN
-        }
+        if (ok) v = lds_f32(addr[k]);
+        if (ok) acc = __fadd_rn(acc, v);                  // :715 sequential, ascending CN
         if (KEEPM) m[KEEPM ? k : 0] = v;
     }
     float x_tot = __fadd_rn(acc, llr);                    // :716
-    const float init = __fadd_rn(llr, 0.f);               // canonical +0.0 for punctured bits (llr = -0.0)
 #pragma unroll
     for (int k = 0; k < DMAX; ++k) {
-        if (MODE == 1) {
-            if (on[k]) sts_f32(addr[k], init);
-        } else {
-            float v = 0.f;
-            if (KEEPM) v = m[KEEPM ? k : 0];
-            else if (on[k]) v = lds_f32(addr[k]);
-            float y = clipf(__fadd_rn(-v, x_tot), clip);  // :724-729
-            if (on[k]) sts_f32(addr[k], y);
-        }
+        float v = 0.f;
+        if (KEEPM) v = m[KEEPM ? k : 0];
+        else if (on[k]) v = lds_f32(addr[k]);
+        float y = clipf(__fadd_rn(-v, x_tot), clip);      // :724-729
+        if (on[k]) sts_f32(addr[k], y);
     }
     return x_tot;
 }
 
+// Loop form for any degree. MODE 0: the update; MODE 1: initialisation v2c = llr (decoding.py:571), canonical +0.0 for
+// punctured bits (llr = -0.0).
 template <int MODE>
-__device__ __forceinline__ float vn_qc_loop(uint32_t msg_s, uint32_t ce_s, int deg, int j4, int Z4, float llr, float clip) {
+__device__ __forceinline__ float vn_qc_loop(uint32_t ce_s, int deg, const VnLane& vl, float llr, float clip) {
     float acc = 0.f;
     if (MODE == 0)
         for (int k = 0; k < deg; ++k) {
-            int2 e = lds_i2(ce_s + 8 * k);
-            int t = j4 - (e.y & 0xffff);
-            t += (t >> 31) & Z4;
-            if (t < (int)((unsigned)e.y >> 16)) acc = __fadd_rn(acc, lds_f32(msg_s + e.x + t));
+            const int2 e = lds_i2(ce_s + 8 * k);
+            const uint32_t a = vn_addr(e, vl);
+            if (vn_in_row(e, a, vl)) acc = __fadd_rn(acc, lds_f32(a));
         }
     float x_tot = __fadd_rn(acc, llr);
     for (int k = 0; k < deg; ++k) {
-        int2 e = lds_i2(ce_s + 8 * k);
-        int t = j4 - (e.y & 0xffff);
-        t += (t >> 31) & Z4;
-        if (t < (int)((unsigned)e.y >> 16)) {
-            uint32_t a = msg_s + e.x + t;
+        const int2 e = lds_i2(ce_s + 8 * k);
+        const uint32_t a = vn_addr(e, vl);
+        if (vn_in_row(e, a, vl))
             sts_f32(a, (MODE == 1) ? __fadd_rn(llr, 0.f) : clipf(__fadd_rn(-lds_f32(a), x_tot), clip));
-        }
     }
     return x_tot;
 }
 
-// VN update of a column of class CLS (kColMax). EX: exact-degree variants (min-sum kernels; the phi kernels sit at the
-// register cap and keep the guarded buckets).
-template <int MODE, int CLS, bool EX>
-__device__ __forceinline__ float vn_cls(uint32_t msgb, uint32_t ce, int deg, int j4, int Z4, float llr, float clip) {
+// VN update of a column of class CLS (kColMax). EX: exact-degree variants.
+template <int CLS, bool EX>
+__device__ __forceinline__ float vn_cls(uint32_t ce, int deg, const VnLane& vl, float llr, float clip) {
     constexpr int D = kColMax[CLS];
     if constexpr (D == kLoop) {
-        return vn_qc_loop<MODE>(msgb, ce, deg, j4, Z4, llr, clip);
+        return vn_qc_loop<0>(ce, deg, vl, llr, clip);
     } else if constexpr (CLS >= kColCut) {
-        return vn_qc<D, true, true, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
-    } else if constexpr (D > 12) {                        // re-reads its messages instead of keeping them in registers
-        return vn_qc<D, false, false, MODE>(msgb, ce, deg, j4, Z4, llr, clip);
+        return vn_qc<D, true, true>(ce, deg, vl, llr, clip);
+    } else if constexpr (D > 12) {
+        // the punctured columns of base graph 1 at the rates that keep 24 block rows: exact-degree code, each message
+        // read once; the guarded buckets re-read their messages instead of keeping them in registers
+        if (CLS == 2 && EX && deg == 19) return vn_qc<19, false, true, true>(ce, deg, vl, llr, clip);
+        if (CLS == 2 && EX && deg == 17) return vn_qc<17, false, true, true>(ce, deg, vl, llr, clip);
+        return vn_qc<D, false, false>(ce, deg, vl, llr, clip);
     } else {
         // exact-degree code (no guards) for every degree up to 12; deg is warp-uniform
         if constexpr (CLS == 3) {
-            if (EX && deg == 9) return vn_qc<9, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-            if (EX && deg == 10) return vn_qc<10, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-            if (EX && deg == 11) return vn_qc<11, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 9) return vn_qc<9, false, true, true>(ce, deg, vl, llr, clip);
+            if (EX && deg == 10) return vn_qc<10, false, true, true>(ce, deg, vl, llr, clip);
+            if (EX && deg == 11) return vn_qc<11, false, true, true>(ce, deg, vl, llr, clip);
         } else if constexpr (CLS == 4) {
-            if (EX && deg == 5) return vn_qc<5, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-            if (EX && deg == 6) return vn_qc<6, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
-            if (EX && deg == 7) return vn_qc<7, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 5) return vn_qc<5, false, true, true>(ce, deg, vl, llr, clip);
+            if (EX && deg == 6) return vn_qc<6, false, true, true>(ce, deg, vl, llr, clip);
+            if (EX && deg == 7) return vn_qc<7, false, true, true>(ce, deg, vl, llr, clip);
         } else if constexpr (CLS == 5) {
-            if (EX && deg == 3) return vn_qc<3, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 3) return vn_qc<3, false, true, true>(ce, deg, vl, llr, clip);
         } else {
-            if (EX && deg == 1) return vn_qc<1, false, true, MODE, true>(msgb, ce, deg, j4, Z4, llr, clip);
+            if (EX && deg == 1) return vn_qc<1, false, true, true>(ce, deg, vl, llr, clip);
         }
-        return vn_qc<D, false, true, MODE, EX>(msgb, ce, deg, j4, Z4, llr, clip);
+        return vn_qc<D, false, true, EX>(ce, deg, vl, llr, clip);
     }
 }
 
@@ -655,17 +661,17 @@ __device__ __forceinline__ void syndrome_pass(const QcParams& p, const WarpCtx& 
     }
 }
 
-template <int MODE, int CLS, bool EX>
-__device__ __forceinline__ void vn_class(const QcParams& p, const WarpCtx& w, uint32_t msgb, const float* llr_s,
+template <int CLS, bool EX>
+__device__ __forceinline__ void vn_class(const QcParams& p, const WarpCtx& w, const VnLane& vl, const float* llr_s,
                                          const int4* s_col, uint32_t s_ce, int start, int end, float clip,
                                          bool final_pass, long long b, unsigned char* hd) {
     for (int cc = first_of(start, p.col_cls_mod[CLS], w); cc < end; cc += w.G) {
         int4 ci = s_col[cc];
         if (w.lane_i < ci.z) {
             int v = ci.w + w.lane_i;
-            float x_tot = vn_cls<MODE, CLS, EX>(msgb, s_ce + 8 * ci.x, ci.y, 4 * w.lane_i, 4 * p.Z, llr_s[v], clip);
-            if (MODE == 0 && hd) hd[v] = 0.f >= x_tot ? 1 : 0;                                // hard decision (:622-624)
-            if (MODE == 0 && final_pass) {
+            float x_tot = vn_cls<CLS, EX>(s_ce + 8 * ci.x, ci.y, vl, llr_s[v], clip);
+            if (hd) hd[v] = 0.f >= x_tot ? 1 : 0;                                            // hard decision (:622-624)
+            if (final_pass) {
                 int o = p.out_pos[v];
                 if (o >= 0) {
                     x_tot = clipf(x_tot, clip);                                              // :730
@@ -676,22 +682,33 @@ __device__ __forceinline__ void vn_class(const QcParams& p, const WarpCtx& w, ui
     }
 }
 
-template <int MODE, bool EX>
-__device__ __forceinline__ void vn_all(const QcParams& p, const WarpCtx& w, uint32_t msgb, const float* llr_s,
+template <bool EX>
+__device__ __forceinline__ void vn_all(const QcParams& p, const WarpCtx& w, const VnLane& vl, const float* llr_s,
                                        const int4* s_col, uint32_t s_ce, float clip, bool final_pass,
-                                       bool with_fused, long long b, unsigned char* hd = nullptr) {
+                                       bool with_fused, long long b, unsigned char* hd) {
     const int* ce = p.col_cls_end;
-    vn_class<MODE, 0, EX>(p, w, msgb, llr_s, s_col, s_ce, 0, ce[0], clip, final_pass, b, hd);
-    vn_class<MODE, 1, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[0], ce[1], clip, final_pass, b, hd);
-    vn_class<MODE, 2, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[1], ce[2], clip, final_pass, b, hd);
-    vn_class<MODE, 3, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[2], ce[3], clip, final_pass, b, hd);
-    vn_class<MODE, 4, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[3], ce[4], clip, final_pass, b, hd);
-    vn_class<MODE, 5, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[4], ce[5], clip, final_pass, b, hd);
-    vn_class<MODE, 6, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[5], ce[6], clip, final_pass, b, hd);
-    vn_class<MODE, 7, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[6], ce[7], clip, final_pass, b, hd);
-    vn_class<MODE, 8, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[7], ce[8], clip, final_pass, b, hd);
-    vn_class<MODE, 9, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[8], ce[9], clip, final_pass, b, hd);
-    if (with_fused) vn_class<MODE, 10, EX>(p, w, msgb, llr_s, s_col, s_ce, ce[9], ce[10], clip, final_pass, b, hd);
+    vn_class<0, EX>(p, w, vl, llr_s, s_col, s_ce, 0, ce[0], clip, final_pass, b, hd);
+    vn_class<1, EX>(p, w, vl, llr_s, s_col, s_ce, ce[0], ce[1], clip, final_pass, b, hd);
+    vn_class<2, EX>(p, w, vl, llr_s, s_col, s_ce, ce[1], ce[2], clip, final_pass, b, hd);
+    vn_class<3, EX>(p, w, vl, llr_s, s_col, s_ce, ce[2], ce[3], clip, final_pass, b, hd);
+    vn_class<4, EX>(p, w, vl, llr_s, s_col, s_ce, ce[3], ce[4], clip, final_pass, b, hd);
+    vn_class<5, EX>(p, w, vl, llr_s, s_col, s_ce, ce[4], ce[5], clip, final_pass, b, hd);
+    vn_class<6, EX>(p, w, vl, llr_s, s_col, s_ce, ce[5], ce[6], clip, final_pass, b, hd);
+    vn_class<7, EX>(p, w, vl, llr_s, s_col, s_ce, ce[6], ce[7], clip, final_pass, b, hd);
+    vn_class<8, EX>(p, w, vl, llr_s, s_col, s_ce, ce[7], ce[8], clip, final_pass, b, hd);
+    vn_class<9, EX>(p, w, vl, llr_s, s_col, s_ce, ce[8], ce[9], clip, final_pass, b, hd);
+    if (with_fused) vn_class<10, EX>(p, w, vl, llr_s, s_col, s_ce, ce[9], ce[10], clip, final_pass, b, hd);
+}
+
+// v2c = llr on every edge (decoding.py:571), once per codeword. One class-agnostic loop over the warp's columns in loop
+// form: the unrolled classes are the iterations' code, and a second copy of them for this pass only made the kernel
+// larger (it is bound by instruction fetch).
+__device__ __forceinline__ void vn_init(const QcParams& p, const WarpCtx& w, const VnLane& vl, const float* llr_s,
+                                        const int4* s_col, uint32_t s_ce) {
+    for (int cc = w.grp; cc < p.n_cols; cc += w.G) {
+        const int4 ci = s_col[cc];
+        if (w.lane_i < ci.z) vn_qc_loop<1>(s_ce + 8 * ci.x, ci.y, vl, llr_s[ci.w + w.lane_i], 0.f);
+    }
 }
 
 // Threads per CTA. 24 warps (80 registers/thread) for every rule: 30 warps at 64 registers were measured for the min-sum
@@ -728,10 +745,16 @@ __global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_
     w.G = W / Zb;
     w.grp = warp / Zb;
     w.lane_i = (warp - w.grp * Zb) * 32 + lane;
+    VnLane vl{4u * w.lane_i, 4u * (w.lane_i + Z), (4u * w.lane_i) << 16 | 0xffffu};
+    asm("" : "+r"(vl.j4), "+r"(vl.j4w), "+r"(vl.jk));     // three live registers: not rebuilt from lane_i at every edge
 
     for (int i = tid; i < p.n_cols; i += T) s_col[i] = p.col_info[i];
     for (int i = tid; i < p.n_rows; i += T) s_row[i] = p.row_info[i];
-    for (int i = tid; i < p.nnz; i += T) s_ce_p[i] = p.col_edge[i];
+    for (int i = tid; i < p.nnz; i += T) {                // the column table in address form (vn_addr)
+        const int2 e = p.col_edge[i];
+        const uint32_t s4 = (uint32_t)e.y & 0xffffu;
+        s_ce_p[i] = make_int2((int)(msgb + (uint32_t)e.x - s4), (int)(s4 << 16 | (uint32_t)e.y >> 16));
+    }
     const LogTab<REP> lt(lane);
     if (RULE == SB_CN_BOXPLUS_PHI) LogTab<REP>::fill(tid, T);
     if (p.use_tma && tid == 0) mbar_init(bar);
@@ -748,7 +771,7 @@ __global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_
         __syncthreads();
         if (tid == 0) *sat_flag = 0;
         // ---- v2c = llr of the edge's VN (decoding.py:571) ---------------------------------------------------------
-        vn_all<1, true>(p, w, msgb, llr_s, s_col, s_ce, clip, false, true, b);
+        vn_init(p, w, vl, llr_s, s_col, s_ce);
         __syncthreads();
         if (p.num_iter == 0) {                           // x_hat = llr_ch (decoding.py:603-608)
             for (int v = tid; v < N; v += T) {
@@ -783,7 +806,7 @@ __global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_
             }
             __syncthreads();
             // ---- VN phase ---------------------------------------------------------------------------------------
-            vn_all<0, true>(p, w, msgb, llr_s, s_col, s_ce, clip, final_pass, final_pass, b, hd);
+            vn_all<true>(p, w, vl, llr_s, s_col, s_ce, clip, final_pass, final_pass, b, hd);
             __syncthreads();
         }
         if (EARLY && p.iters_out && tid == 0) p.iters_out[b] = limit;
