@@ -100,7 +100,7 @@ struct QcParams {
 #define SB_PHI_HI 16.635532f
 // Least fp32 x above which phi(x) is +0 for every x in this arithmetic: e^x + 1 and e^x - 1 round to the same float
 // and the two logs cancel. Below it phi is not monotone (x = 14.7117338 gives 2^-20). Checked over every fp32 value up
-// to 16.635532 against the oracle and on the device by tests/test_ldpc_phi_union_gpu.py.
+// to 16.635532 against the oracle and on the device by tests/test_ldpc_qc_kernel_gpu.py.
 #define SB_PHI_ZERO 14.7117348f
 // The two passes of the update, written once for every variant below: pass 1 on the edge words b = bits(x), pass 2 on
 // the staged words w = phi(|x|) | sign(x); one edge pair (two independent phi chains, sb_math2.cuh) or one edge.

@@ -19,6 +19,7 @@ import pytest
 import torch
 
 from oracle import ofdm as F
+from oracle.parity import cnormal, envelope
 
 pytestmark = pytest.mark.gpu
 
@@ -29,25 +30,7 @@ BARS = {                                        # (rms, max) bar of a comparison
                                                 # complex exp per sinusoid and step in the float32 evaluation; the worst
                                                 # |a - a64| is 1.6e-6 of the path amplitude at every T, 30 706 included
 }
-FLOOR = 2.0 ** -24
-
-
-def _envelope(what, got, f32, ref, scale, bar=None):
-    """'' if got's error is within bar times f32's, both against ref and relative to scale, else the measurement."""
-    bar = bar or BARS.get(what.split(" ")[0], DEFAULT_BAR)
-    scale = np.maximum(np.broadcast_to(scale, ref.shape), np.finfo(np.float32).tiny)
-    a = np.abs(np.asarray(got, np.complex128) - ref) / scale
-    b = np.abs(np.asarray(f32, np.complex128) - ref) / scale
-    rms_a, max_a = float(np.sqrt(np.mean(a ** 2))), float(a.max())
-    rms_b, max_b = max(float(np.sqrt(np.mean(b ** 2))), FLOOR), max(float(b.max()), FLOOR)
-    line = (f"{what}: kernel rms {rms_a:.2e} max {max_a:.2e} | complex64 numpy rms {rms_b:.2e} max {max_b:.2e} "
-            f"| ratio rms {rms_a / rms_b:.2f} max {max_a / max_b:.2f} (bar {bar[0]:g} / {bar[1]:g})")
-    print(line)
-    return "" if rms_a <= bar[0] * rms_b and max_a <= bar[1] * max_b else line
-
-
-def _c(rng, shape, scale=1.0):
-    return ((rng.normal(size=shape) + 1j * rng.normal(size=shape)) * scale / np.sqrt(2)).astype(np.complex64)
+FLOOR = (2.0 ** -24, 2.0 ** -24)                # least complex64 (rms, max) error, relative to the scale
 
 
 def _dev(x, dev):
@@ -98,7 +81,7 @@ def test_cir_apply_envelope(cuda_device, mode, f, t, p, per_link):
     from sionna_b200.phy.channel import cir_to_ofdm_channel, cir_to_time_channel, subcarrier_frequencies
     rng = np.random.default_rng(1000 * f + 10 * t + p)
     b, rx, ra, tx, ta = (2, 1, 2, 2, 1) if f * t < 50000 else (1, 1, 2, 1, 1)
-    a = _c(rng, (b, rx, ra, tx, ta, p, t))
+    a = cnormal(rng, (b, rx, ra, tx, ta, p, t))
     a[0, 0, 0, 0, 0, :, :1] = 0                                     # one zero time step of one row
     if mode == "ofdm":
         bw, lo, hi = f * 30e3, None, None
@@ -131,7 +114,7 @@ def test_cir_apply_envelope(cuda_device, mode, f, t, p, per_link):
             scale = scale / np.where(c64 > 0, c64, 1)
         assert np.all(np.isfinite(got))
         assert np.all(got[0, 0, 0, 0, 0, 0] == 0)
-        bad.append(_envelope(f"cir {mode} normalize={normalize}", got, f32, ref, scale))
+        bad.append(envelope(f"cir {mode} normalize={normalize}", got, f32, ref, DEFAULT_BAR, FLOOR, scale=scale))
     assert not any(bad), "\n".join(x for x in bad if x)
 
 
@@ -186,7 +169,7 @@ def test_cir_gram_double(cuda_device, f, p):
     from sionna_b200._lib import ptr
     rng = np.random.default_rng(f * 100 + p)
     n_tab = 3
-    e = _c(rng, (n_tab, p, f))
+    e = cnormal(rng, (n_tab, p, f))
     g = torch.empty((n_tab, p, p), dtype=torch.complex128, device=cuda_device)
     _call("sb_cir_gram", _dev(e, cuda_device), ptr(g), n_tab, p, f)
     e64 = e.astype(np.complex128)
@@ -256,15 +239,15 @@ def test_spatial_corr_envelope(cuda_device, n):
     from sionna_b200._lib import ptr
     rng = np.random.default_rng(n)
     bsz, cols = 3, 77
-    m = _c(rng, (n, 2 * n)).astype(np.complex128)
+    m = cnormal(rng, (n, 2 * n)).astype(np.complex128)
     l = np.linalg.cholesky(m @ m.conj().T / (2 * n) + 0.1 * np.eye(n)).astype(np.complex64)
-    v = _c(rng, (bsz, n, cols))
+    v = cnormal(rng, (bsz, n, cols))
     out = torch.empty((bsz, n, cols), dtype=torch.complex64, device=cuda_device)
     _call("sb_spatial_corr", _dev(v, cuda_device), _dev(l, cuda_device), ptr(out), bsz, n, cols)
     ref = np.einsum("ij,bjc->bic", l.astype(np.complex128), v.astype(np.complex128))
     f32 = np.einsum("ij,bjc->bic", l, v)
     scale = np.sqrt(np.einsum("ij,bjc->bic", np.abs(l).astype(np.float64) ** 2, np.abs(v).astype(np.float64) ** 2))
-    bad = _envelope(f"spatial corr n={n}", out.cpu().numpy(), f32, ref, scale)
+    bad = envelope(f"spatial corr n={n}", out.cpu().numpy(), f32, ref, DEFAULT_BAR, FLOOR, scale=scale)
     assert not bad, bad
 
 
@@ -296,7 +279,7 @@ def test_tdl_sos_envelope(cuda_device, model, ns, t, speed):
         pw[0] += tdl._los_power
     scale = np.sqrt(pw)[None, None, :, None]
     print(f"tdl {model} Ns={ns} T={t} speed {speed}: worst |a - a64| = {np.abs(got - ref).max():.2e}")
-    bad = _envelope(f"tdl_sos T={t}", got, f32, ref, scale)
+    bad = envelope(f"tdl_sos T={t}", got, f32, ref, BARS["tdl_sos"], FLOOR, scale=scale)
     assert not bad, bad
 
 
@@ -306,13 +289,13 @@ def test_apply_ofdm_channel_envelope(cuda_device, r, tt, re):
     from sionna_b200.phy.channel import ApplyOFDMChannel
     rng = np.random.default_rng(r * tt + re)
     b, s = 2, 1
-    h = _c(rng, (b, 1, r, 1, tt, s, re))
-    x = _c(rng, (b, 1, tt, s, re))
+    h = cnormal(rng, (b, 1, r, 1, tt, s, re))
+    x = cnormal(rng, (b, 1, tt, s, re))
     got = ApplyOFDMChannel()(_dev(x, cuda_device), _dev(h, cuda_device)).cpu().numpy()
     ref = np.einsum("brmtksf,btksf->brmsf", h.astype(np.complex128), x.astype(np.complex128))
     f32 = np.einsum("brmtksf,btksf->brmsf", h, x)
     scale = np.sqrt(np.einsum("brmtksf,btksf->brmsf", np.abs(h).astype(np.float64) ** 2, np.abs(x).astype(np.float64) ** 2))
-    bad = _envelope(f"apply ofdm R={r} Tt={tt} RE={re}", got, f32, ref, scale)
+    bad = envelope(f"apply ofdm R={r} Tt={tt} RE={re}", got, f32, ref, DEFAULT_BAR, FLOOR, scale=scale)
     assert not bad, bad
 
 
@@ -322,15 +305,15 @@ def test_apply_time_channel_envelope(cuda_device, tt, n, l):
     from sionna_b200.phy.channel import ApplyTimeChannel
     rng = np.random.default_rng(100 * n + l)
     b, r = 2, 3
-    h = _c(rng, (b, 1, r, 1, tt, n + l - 1, l))
-    x = _c(rng, (b, 1, tt, n))
+    h = cnormal(rng, (b, 1, r, 1, tt, n + l - 1, l))
+    x = cnormal(rng, (b, 1, tt, n))
     got = ApplyTimeChannel(n, l)(_dev(x, cuda_device), _dev(h, cuda_device)).cpu().numpy()[:, 0]
     h3, x3 = h[:, 0, :, 0], x[:, 0]
     ref = F.apply_time_channel(x3, h3)
     f32 = F.apply_time_channel(x3, h3, np.complex64)
     scale = np.sqrt(F.apply_time_channel(np.abs(x3) ** 2, np.abs(h3) ** 2).real)
-    bad = _envelope(f"apply time N={n} L={l}", got, f32, ref, scale)
+    bad = envelope(f"apply time N={n} L={l}", got, f32, ref, DEFAULT_BAR, FLOOR, scale=scale)
     edges = np.r_[0:min(l - 1, n + l - 1), max(n, 0):n + l - 1]
-    bad2 = _envelope(f"apply time N={n} L={l} edges", got[..., edges], f32[..., edges], ref[..., edges], scale[..., edges]) \
-        if len(edges) else ""
+    bad2 = envelope(f"apply time N={n} L={l} edges", got[..., edges], f32[..., edges], ref[..., edges], DEFAULT_BAR,
+                    FLOOR, scale=scale[..., edges]) if len(edges) else ""
     assert not bad and not bad2, bad + bad2

@@ -33,6 +33,7 @@ import scipy.fft as sfft
 import torch
 
 from oracle import ofdm as F
+from oracle.parity import cnormal, envelope
 
 pytestmark = pytest.mark.gpu
 
@@ -41,10 +42,6 @@ R16_SIZES = [2048, 4096]
 GENERIC_SIZES = [1025, 1031, 2187, 4095, 5000, 6144, 7264, 7265, 8192]
 DEFAULT_BAR = (2.0, 3.0)                       # (rms, max)
 SIZE_BARS = {2187: (3.0, 3.5), 4095: (3.5, 4.0)}
-
-
-def _c64(rng, shape):
-    return ((rng.normal(size=shape) + 1j * rng.normal(size=shape)) / np.sqrt(2)).astype(np.complex64)
 
 
 def _rms(a):
@@ -62,13 +59,18 @@ def _largest_prime_factor(n):
     return big
 
 
-def _direct_dft_envelope(p, transforms, rng):
-    """(rms, max) error of a length-p DFT summed term by term in complex64 (x_0 w^0 + x_1 w^c + ... in that order,
-    roots rounded to complex64) against complex128, normalised by the rms of the exact output."""
-    x = _c64(rng, (transforms, p))
+def _direct_dft_floor(n, size, rng):
+    """Floor (rms, max) of the fp32 envelope of a size-n transform of `size` outputs: none unless n has a prime factor
+    p > 19, else the error of min(16, size // p) (at least one) length-p DFTs summed term by term in complex64 (x_0 w^0
+    + x_1 w^c + ... in that order, roots rounded to complex64) against complex128, normalised by the rms of the exact
+    output."""
+    p = _largest_prime_factor(n)
+    if p <= 19:
+        return 0.0, 0.0
+    x = cnormal(rng, (max(1, min(16, size // p)), p))
     k = np.arange(p)
     w = np.exp(-2j * np.pi * k / p).astype(np.complex64)
-    out = np.empty((transforms, p), np.complex64)
+    out = np.empty(x.shape, np.complex64)
     for c0 in range(0, p, 64):
         c = np.arange(c0, min(p, c0 + 64))
         terms = x[:, None, :] * w[(c[:, None] * k[None, :]) % p][None]
@@ -78,22 +80,10 @@ def _direct_dft_envelope(p, transforms, rng):
     return _rms(e), float(e.max())
 
 
-def _envelope(n, got, ref, f32, rng, what):
-    """'' if got (kernel) is within the bars of the fp32 envelope, both measured against ref, else the measurement."""
-    scale = _rms(ref)
-    a = np.abs(got - ref) / scale
-    b = np.abs(f32 - ref) / scale
-    rms_b, max_b = _rms(b), float(b.max())
-    p = _largest_prime_factor(n)
-    if p > 19:
-        rms_d, max_d = _direct_dft_envelope(p, max(1, min(16, got.size // p)), rng)
-        rms_b, max_b = max(rms_b, rms_d), max(max_b, max_d)
-    rms_a, max_a = _rms(a), float(a.max())
-    line = (f"{what} N={n}: kernel rms {rms_a:.2e} max {max_a:.2e} | fp32 envelope rms {rms_b:.2e} max {max_b:.2e} "
-            f"| ratio rms {rms_a / max(rms_b, 1e-30):.2f} max {max_a / max(max_b, 1e-30):.2f}")
-    print(line)
-    bar = SIZE_BARS.get(n, DEFAULT_BAR)
-    return "" if rms_a <= bar[0] * rms_b and max_a <= bar[1] * max_b else line
+def _envelope_n(what, n, got, f32, ref, rng):
+    """The envelope of a size-n transform, errors relative to the rms of the whole exact output."""
+    return envelope(f"{what} N={n}", got, f32, ref, SIZE_BARS.get(n, DEFAULT_BAR), _direct_dft_floor(n, got.size, rng),
+                    axis=None)
 
 
 def _modulate_f32(x, cp):
@@ -124,12 +114,12 @@ def _check_ofdm(dev, x, cp, l_mins, rng):
     got_t = t.cpu().numpy()
     ref_t = F.ofdm_modulate(x.astype(np.complex128), cp)
     assert got_t.shape == ref_t.shape
-    bad = [_envelope(n, got_t, ref_t, _modulate_f32(x, cp), rng, "modulate")]
+    bad = [_envelope_n("modulate", n, got_t, _modulate_f32(x, cp), ref_t, rng)]
     for l_min in l_mins:
         xh = OFDMDemodulator(n, l_min, cp)(t).cpu().numpy()
         assert xh.shape == x.shape
         ref = F.ofdm_demodulate(got_t.astype(np.complex128), n, l_min, cp)
-        bad.append(_envelope(n, xh, ref, _demodulate_f32(got_t, n, l_min, cp), rng, f"demodulate l_min={l_min}"))
+        bad.append(_envelope_n(f"demodulate l_min={l_min}", n, xh, _demodulate_f32(got_t, n, l_min, cp), ref, rng))
     back = OFDMDemodulator(n, 0, cp)(t).cpu().numpy()
     assert np.abs(back - x).max() < 3e-5 * np.sqrt(max(n, 72) / 72)
     return [b for b in bad if b]
@@ -141,9 +131,9 @@ def _check_signal_fft(dev, x, rng):
     n = x.shape[-1]
     xd = torch.from_numpy(x).to(dev)
     ref = np.fft.fft(x.astype(np.complex128), axis=-1) / np.sqrt(n)
-    bad = [_envelope(n, fft(xd).cpu().numpy(), ref, sfft.fft(x, axis=-1, norm="ortho"), rng, "fft")]
+    bad = [_envelope_n("fft", n, fft(xd).cpu().numpy(), sfft.fft(x, axis=-1, norm="ortho"), ref, rng)]
     ref = np.fft.ifft(x.astype(np.complex128), axis=-1) * np.sqrt(n)
-    bad.append(_envelope(n, ifft(xd).cpu().numpy(), ref, sfft.ifft(x, axis=-1, norm="ortho"), rng, "ifft"))
+    bad.append(_envelope_n("ifft", n, ifft(xd).cpu().numpy(), sfft.ifft(x, axis=-1, norm="ortho"), ref, rng))
     return [b for b in bad if b]
 
 
@@ -152,7 +142,7 @@ def test_fft_sizes_within_fp32_envelope(cuda_device, n):
     """3 rows x 5 OFDM symbols = 15 transforms, not a multiple of 2 or 4 transforms per warp; per-symbol cyclic
     prefixes (up to the full symbol for small N), l_min = 0 and -7; odd N exercise floor(N/2) in the (i)fftshift."""
     rng = np.random.default_rng(n)
-    x = _c64(rng, (3, 5, n))
+    x = cnormal(rng, (3, 5, n))
     cp = rng.integers(0, min(n, 40) + 1, 5).astype(np.int32)
     cp[0] = min(n, 40)
     bad = _check_ofdm(cuda_device, x, cp, (0, -7), rng) + _check_signal_fft(cuda_device, x.reshape(15, n), rng)
@@ -162,7 +152,7 @@ def test_fft_sizes_within_fp32_envelope(cuda_device, n):
 def test_fft_prime_8191_single_transform(cuda_device):
     """The largest prime the generic kernel accepts: one direct 8191-term DFT per direction, O(N^2) in one thread."""
     rng = np.random.default_rng(8191)
-    x = _c64(rng, (1, 1, 8191))
+    x = cnormal(rng, (1, 1, 8191))
     bad = _check_ofdm(cuda_device, x, np.array([37], np.int32), (-7,), rng)
     assert not bad, "\n".join(bad)
 
@@ -186,7 +176,7 @@ def test_fft_partial_batches(cuda_device, n):
     rng = np.random.default_rng(1000 + n)
     bad = []
     for shape in ((1, 1, n), (1, 3, n), (1, 5, n), (_grid_stride(n, cuda_device) + 1, 1, n)):
-        x = _c64(rng, shape)
+        x = cnormal(rng, shape)
         cp = np.full(shape[1], 11, np.int32)
         bad += _check_ofdm(cuda_device, x, cp, (-3,), rng)
     assert not bad, "\n".join(bad)

@@ -37,6 +37,7 @@ import torch
 from oracle import ofdm as F
 from oracle import nr as ON
 from oracle.mimo import logits_to_llrs
+from oracle.parity import cnormal, envelope
 
 pytestmark = pytest.mark.gpu
 
@@ -62,10 +63,6 @@ ANTS = (1, 2, 3, 5, 7, 8, 13, 16, 17)
 INTERPS = ("nn", "lin", "lin_time_avg")
 
 
-def _c(rng, shape, scale=1.0):
-    return (rng.normal(size=shape) + 1j * rng.normal(size=shape)) * scale / np.sqrt(2)
-
-
 def _grid(k, num_sym, fft, pilots, guards=(0, 0), dc=False):
     from sionna_b200.phy.ofdm import ResourceGrid
     return ResourceGrid(num_sym, fft, 15e3, num_tx=1, num_streams_per_tx=k, cyclic_prefix_length=0,
@@ -73,7 +70,7 @@ def _grid(k, num_sym, fft, pilots, guards=(0, 0), dc=False):
                         pilot_ofdm_symbol_indices=list(pilots))
 
 
-def _constellation(h, kind="qam"):
+def _demapper_constellation(h, kind="qam"):
     """Square QAM with 2^(2h) points, or ("asym") a separable constellation whose imaginary levels are the real ones
     reversed and scaled by 0.75, so that the two dimensions cannot be confused."""
     from sionna_b200.phy.mapping import Constellation, separable_levels_np
@@ -110,10 +107,11 @@ def _received(rng, rg, b, ant, pts, no, rx=1):
     s_, n = rg.num_ofdm_symbols, rg.fft_size
     lead = (b, rx, ant, tx, st, 1, 1)
     ramp = rng.uniform(-0.003, 0.003, lead) * np.arange(n) + rng.uniform(-0.01, 0.01, lead) * np.arange(s_)[:, None]
-    h = _c(rng, lead) * np.exp(2j * np.pi * ramp) + 0.02 * _c(rng, (b, rx, ant, tx, st, s_, n))
+    h = cnormal(rng, lead, dtype=np.complex128) * np.exp(2j * np.pi * ramp) + \
+        0.02 * cnormal(rng, (b, rx, ant, tx, st, s_, n), dtype=np.complex128)
     y = np.einsum("brmtksf,btksf->brmsf", h, grid)
     no_b = np.broadcast_to(np.reshape(no, np.shape(no) + (1,) * (3 - np.ndim(no))), (b, rx, ant))
-    return (y + _c(rng, y.shape) * np.sqrt(no_b)[..., None, None]).astype(np.complex64)
+    return (y + cnormal(rng, y.shape, dtype=np.complex128) * np.sqrt(no_b)[..., None, None]).astype(np.complex64)
 
 
 def _oracle(rg, y, no, interp, pts, method, dtype, pusch=None):
@@ -142,24 +140,6 @@ def _oracle(rg, y, no, interp, pts, method, dtype, pusch=None):
     logits = -np.abs(x[..., None] - c) ** 2 / np.maximum(ne, rdt(TINY))[..., None]
     llr = logits_to_llrs(logits, m, method)
     return x, ne, llr.reshape(llr.shape[:-2] + (-1,))
-
-
-def _rel(got, ref, rows):
-    den = np.sqrt(np.mean(ref ** 2, axis=-1, keepdims=True)) if rows else np.abs(ref)
-    return np.abs(got - ref) / np.maximum(den, 1e-30)
-
-
-def _envelope(what, got, f32, ref, bar=DEFAULT_BAR, rows=False):
-    """'' if got's error is within bar = (rms, max) times f32's, both against ref, else the measurement. rows: errors
-    relative to the rms of ref over the last axis (LLRs of one frame and stream), else per element."""
-    assert np.array_equal(np.isfinite(got), np.isfinite(ref)), f"{what}: kernel finite where the oracle is not (or vice versa)"
-    a, b = _rel(got, ref, rows), _rel(f32, ref, rows)
-    rms_a, max_a = float(np.sqrt(np.mean(a ** 2))), float(a.max())
-    rms_b, max_b = float(np.sqrt(np.mean(b ** 2))), float(b.max())
-    line = (f"{what}: kernel rms {rms_a:.2e} max {max_a:.2e} | complex64 numpy rms {rms_b:.2e} max {max_b:.2e} "
-            f"| ratio rms {rms_a / max(rms_b, 1e-30):.2f} max {max_a / max(max_b, 1e-30):.2f} (bar {bar[0]:g} / {bar[1]:g})")
-    print(line)
-    return "" if rms_a <= bar[0] * rms_b and max_a <= bar[1] * max_b else line
 
 
 def _hard_check(what, hard, soft, ref, f32, m, bar=DEFAULT_BAR):
@@ -197,9 +177,10 @@ def _compare(tag, rg, est_kind, y, no, const, method, soft, eq, pusch=None, ant=
     x32, n32, l32 = _oracle(rg, y, no, est_kind, pts, method, np.complex64, pusch)
     assert soft.shape == l64.shape and eq[0].shape == x64.shape, tag
     low = ant is not None and ant < rg.num_streams_per_tx
-    bad = [_envelope(f"{tag} x_hat", eq[0], x32, x64, BARS["x_hat ANT=1<K" if low and ant == 1 else "x_hat"]),
-           _envelope(f"{tag} no_eff", eq[1], n32, n64, BARS["no_eff ANT<K"] if low else DEFAULT_BAR),
-           _envelope(f"{tag} llr", soft, l32, l64, BARS["llr ANT<K"] if low else DEFAULT_BAR, rows=True)]
+    bad = [envelope(f"{tag} x_hat", eq[0], x32, x64, BARS["x_hat ANT=1<K" if low and ant == 1 else "x_hat"],
+                    scale=np.abs(x64)),
+           envelope(f"{tag} no_eff", eq[1], n32, n64, BARS["no_eff ANT<K"] if low else DEFAULT_BAR, scale=np.abs(n64)),
+           envelope(f"{tag} llr", soft, l32, l64, BARS["llr ANT<K"] if low else DEFAULT_BAR)]
     return bad, l64, l32
 
 
@@ -232,7 +213,7 @@ def test_soft_llrs_all_variants(cuda_device, k, h, method):
     rng = np.random.default_rng(zlib.crc32(f"variant {k} {h} {method}".encode()))
     rg = _grid(k, s_, fft, pilots, guards, dc)
     assert rg.num_effective_subcarriers == 60
-    const = _constellation(h)
+    const = _demapper_constellation(h)
     det = _detector(LSChannelEstimator(rg, interp), rg, k, const, method)
     assert det._sm.num_streams_per_rx == k and const.num_bits_per_symbol == 2 * h and det._method == METHODS.index(method)
     assert det._num_listed == _LISTED[(k, h, method)]             # < 128: one partial tile; else a partial last tile
@@ -260,7 +241,7 @@ def test_high_snr_app(cuda_device, h, kind):
     k, ant, b = 2, 5, 2
     rng = np.random.default_rng(zlib.crc32(f"high snr {h} {kind}".encode()))
     rg = _grid(k, 5, 60, [1])
-    const = _constellation(h, kind)
+    const = _demapper_constellation(h, kind)
     det = _detector(LSChannelEstimator(rg, "lin"), rg, k, const, "app")
     no = rng.uniform(1e-4, 1e-3, (b, 1, ant)).astype(np.float32)
     y = _received(rng, rg, b, ant, const.points.numpy(), no)
@@ -301,7 +282,7 @@ def test_pusch_tables(cuda_device, cfg):
     rg = tx.resource_grid
     est = PUSCHLSChannelEstimator(rg, tx._dmrs_length, tx._dmrs_additional_position, tx._num_cdm_groups_without_data,
                                   interpolation_type=interp)
-    const = _constellation(m // 2)
+    const = _demapper_constellation(m // 2)
     det = _detector(est, rg, layers, const, method)
     if length == 2 and addpos == 1 and interp == "lin":
         assert det._num_terms == 16
@@ -325,7 +306,7 @@ def test_batch_slices(cuda_device):
     from sionna_b200.phy.ofdm import LSChannelEstimator
     k, h, ant, method = 2, 2, 4, "app"
     rg = _grid(k, 14, 600, [2, 11])
-    const = _constellation(h)
+    const = _demapper_constellation(h)
     det = _detector(LSChannelEstimator(rg, "lin"), rg, k, const, method)
     tiles = -(-det._num_listed // 128)
     sms = torch.cuda.get_device_properties(0).multi_processor_count
@@ -350,7 +331,7 @@ def test_noise_shapes(cuda_device):
     from sionna_b200.phy.ofdm import LSChannelEstimator
     k, h, ant, b = 3, 3, 5, 3
     rg = _grid(k, 14, 60, [2, 11])
-    const = _constellation(h)
+    const = _demapper_constellation(h)
     det = _detector(LSChannelEstimator(rg, "nn"), rg, k, const, "app")
     rng = np.random.default_rng(22)
     y = torch.from_numpy(_received(rng, rg, b, ant, const.points.numpy(), 0.003)).to(cuda_device)
@@ -373,7 +354,7 @@ def test_two_receivers_c_abi(cuda_device):
     from sionna_b200.phy.ofdm.equalization import _strides_for
     k_all, k, h, ant, b = 4, 2, 2, 5, 3
     rg = _grid(k_all, 5, 60, [1, 3])
-    const = _constellation(h)
+    const = _demapper_constellation(h)
     det = _detector(LSChannelEstimator(rg, "lin"), rg, k_all, const, "app")
     t = det._tables(cuda_device)
     rng = np.random.default_rng(23)

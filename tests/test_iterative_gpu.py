@@ -17,6 +17,7 @@ from oracle import mapping as MAP
 from oracle import ofdm as F
 from oracle.iterative import ep_detect, mmse_pic_detect, ofdm_ep_detect, ofdm_mmse_pic_detect
 from oracle.mimo import llrs_to_logits, logits_to_llrs
+from oracle.parity import cnormal, constellation, envelope, mimo_problem, ofdm_detection_case
 
 BAR = (2.0, 4.0)
 GAP = 1e-3
@@ -31,51 +32,11 @@ BARS = {                                        # EP cases held to a wider rms b
 }
 
 
-def _c(rng, shape, scale=1.0):
-    return ((rng.normal(size=shape) + 1j * rng.normal(size=shape)) * scale / np.sqrt(2)).astype(np.complex64)
-
-
-def _problem(rng, num, m, k, points, no):
-    """y = h x + n with non-diagonal noise covariances s = no (I + 0.5 A A^H / m); also the transmitted indices."""
-    h = _c(rng, (num, m, k))
-    ind = rng.integers(0, len(points), (num, k))
-    a = _c(rng, (num, m, m))
-    s = (no * (np.eye(m) + 0.5 * a @ np.conj(np.swapaxes(a, -1, -2)) / m)).astype(np.complex64)
-    n = (np.linalg.cholesky(s.astype(np.complex128)) @ _c(rng, (num, m, 1)))[..., 0]
-    return ((h @ points[ind][..., None])[..., 0] + n).astype(np.complex64), h, s, ind
-
-
-def _err(got, ref):
-    fin = np.isfinite(ref)
-    den = np.sqrt(np.mean(np.where(fin, ref, 0) ** 2, axis=-1, keepdims=True))
-    return np.where(fin, np.abs(got - ref), 0) / np.maximum(den, 1e-30)
-
-
-def _envelope(what, got, f32, ref, bar=BAR):
-    """'' if got's error is within bar = (rms, max) times f32's, both against ref, else the measurement."""
-    a, b = _err(got, ref), _err(f32, ref)
-    rms_a, max_a = float(np.sqrt(np.mean(a ** 2))), float(a.max())
-    rms_b, max_b = float(np.sqrt(np.mean(b ** 2))), float(b.max())
-    line = (f"{what}: kernel rms {rms_a:.2e} max {max_a:.2e} | complex64 numpy rms {rms_b:.2e} max {max_b:.2e} "
-            f"| ratio rms {rms_a / max(rms_b, 1e-30):.2f} max {max_a / max(max_b, 1e-30):.2f}")
-    print(line)
-    return "" if rms_a <= bar[0] * rms_b and max_a <= bar[1] * max_b else line
-
-
 def _keep(what, *margins):
     keep = np.all([g > GAP for g in margins], axis=0)
     print(f"{what}: {1 - keep.mean():.3%} of the problems excluded (margin <= {GAP})")
     assert 1 - keep.mean() < EXCLUDED.get(what, 0.01), what
     return keep
-
-
-def _constellation(kind, m):
-    from sionna_b200.phy.mapping import Constellation
-    if kind == "custom":
-        rng = np.random.default_rng(99)
-        pts = (rng.normal(size=2 ** m) + 1j * rng.normal(size=2 ** m)).astype(np.complex64)
-        return Constellation("custom", m, points=pts, normalize=True, center=True)
-    return Constellation(kind, m)
 
 
 def _bits(ind, m):
@@ -100,7 +61,7 @@ def test_dense_ep_against_oracle(cuda_device, case):
     name, ns, m, mm, l, beta, num, no = case
     pts = MAP.qam(m)
     rng = np.random.default_rng(zlib.crc32(name.encode()))
-    y, h, s, _ = _problem(rng, num, mm, ns, pts, no)
+    y, h, s = mimo_problem(rng, num, mm, ns, pts, no)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
     kw = dict(l=l, beta=beta)
     ref, g_soft = ep_detect(y, h, s, m, "bit", **kw)
@@ -111,12 +72,12 @@ def test_dense_ep_against_oracle(cuda_device, case):
     got = EPDetector("bit", m, **kw)(*dev).cpu().numpy()
     assert got.shape == ref.shape == (num, ns, m)
     bar = BARS.get(name, BAR)
-    bad = [_envelope(f"{name} LLRs", got[keep], f32[keep], ref[keep], bar)]
+    bad = [envelope(f"{name} LLRs", got[keep], f32[keep], ref[keep], bar)]
     lref, _ = ep_detect(y, h, s, m, "symbol", **kw)
     l32, _ = ep_detect(y, h, s, m, "symbol", dtype=np.complex64, **kw)
     logits = EPDetector("symbol", m, **kw)(*dev).cpu().numpy()
     assert logits.shape == (num, ns, 2 ** m)
-    bad.append(_envelope(f"{name} logits", logits[keep], l32[keep], lref[keep], bar))
+    bad.append(envelope(f"{name} logits", logits[keep], l32[keep], lref[keep], bar))
     hard_b = EPDetector("bit", m, hard_out=True, **kw)(*dev)
     hard_s = EPDetector("symbol", m, hard_out=True, **kw)(*dev)
     assert hard_b.dtype == torch.float32 and hard_s.dtype == torch.int32
@@ -132,7 +93,7 @@ def test_ep_noiseless_problems_have_no_errors(cuda_device, m):
     from sionna_b200.phy.mimo import EPDetector
     rng = np.random.default_rng(40 + m)
     pts = MAP.qam(m)
-    h = _c(rng, (100, 7, 3))
+    h = cnormal(rng, (100, 7, 3))
     ind = rng.integers(0, len(pts), (100, 3))
     y = (h @ pts[ind][..., None])[..., 0]
     s = (1e-4 * np.eye(7)).astype(np.complex64)
@@ -172,10 +133,10 @@ PIC_DENSE = [("qpsk 4x8 maxlog it1 zero", "qam", 2, 4, 8, "maxlog", 1, "zero", 1
 def test_dense_mmse_pic_against_oracle(cuda_device, case):
     from sionna_b200.phy.mimo import MMSEPICDetector
     name, kind, m, ns, mm, method, it, pk, num, no = case
-    const = _constellation(kind, m)
+    const = constellation(kind, m)
     pts = const().cpu().numpy().astype(np.complex64)
     rng = np.random.default_rng(zlib.crc32(name.encode()))
-    y, h, s, ind = _problem(rng, num, mm, ns, pts, no)
+    y, h, s, ind = mimo_problem(rng, num, mm, ns, pts, no, return_indices=True)
     pr = _prior(rng, pk, ind, m)
     plog = llrs_to_logits(pr, m).astype(np.float32)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
@@ -188,13 +149,13 @@ def test_dense_mmse_pic_against_oracle(cuda_device, case):
     args = dict(demapping_method=method, num_iter=it, constellation=const)
     got = MMSEPICDetector("bit", **args)(*dev, torch.from_numpy(pr).to(cuda_device)).cpu().numpy()
     assert got.shape == ref.shape == (num, ns, m)
-    bad = [_envelope(f"{name} LLRs", got[keep], f32[keep], ref[keep])]
+    bad = [envelope(f"{name} LLRs", got[keep], f32[keep], ref[keep], BAR)]
     lref, _ = mmse_pic_detect(y, h, s, plog, pts, "symbol", **kw)
     l32, _ = mmse_pic_detect(y, h, s, plog, pts, "symbol", dtype=np.complex64, **kw)
     dplog = torch.from_numpy(plog).to(cuda_device)
     logits = MMSEPICDetector("symbol", **args)(*dev, dplog).cpu().numpy()
     assert logits.shape == (num, ns, 2 ** m)
-    bad.append(_envelope(f"{name} logits", logits[keep], l32[keep], lref[keep]))
+    bad.append(envelope(f"{name} logits", logits[keep], l32[keep], lref[keep], BAR))
     hard_b = MMSEPICDetector("bit", hard_out=True, **args)(*dev, torch.from_numpy(pr).to(cuda_device))
     hard_s = MMSEPICDetector("symbol", hard_out=True, **args)(*dev, dplog)
     assert hard_b.dtype == torch.float32 and hard_s.dtype == torch.int32
@@ -210,7 +171,7 @@ def test_zero_prior_single_iteration_is_lmmse(cuda_device):
     from sionna_b200.phy.mimo import MMSEPICDetector, LinearDetector
     rng = np.random.default_rng(3)
     pts = MAP.qam(4)
-    y, h, s, _ = _problem(rng, 2048, 8, 4, pts, 0.05)
+    y, h, s = mimo_problem(rng, 2048, 8, 4, pts, 0.05)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
     xh, ne = F.lmmse_equalizer(y.astype(complex), h.astype(complex), s.astype(complex))
     p64 = pts.astype(complex) / np.sqrt(np.mean(np.abs(pts.astype(complex)) ** 2))
@@ -219,30 +180,9 @@ def test_zero_prior_single_iteration_is_lmmse(cuda_device):
     f32 = logits_to_llrs(-np.abs(x32[..., None] - pts) ** 2 / n32[..., None], 4, "maxlog")
     pic = MMSEPICDetector("bit", "maxlog", 1, "qam", 4)(*dev, torch.zeros(2048, 4, 4, device=cuda_device))
     lin = LinearDetector("lmmse", "bit", "maxlog", "qam", 4)(*dev)
-    bad = [_envelope("MMSE-PIC zero prior", pic.cpu().numpy(), f32, ref),
-           _envelope("LinearDetector", lin.cpu().numpy(), f32, ref)]
+    bad = [envelope("MMSE-PIC zero prior", pic.cpu().numpy(), f32, ref, BAR),
+           envelope("LinearDetector", lin.cpu().numpy(), f32, ref, BAR)]
     assert not any(bad), "\n".join(b for b in bad if b)
-
-
-def _ofdm_case(cfg, rng):
-    """(rg, sm, oracle stream dict, y_eff, h, err_var, no, points) on a 3-symbol Kronecker grid (symbol 1 pilots)."""
-    from sionna_b200.phy.ofdm import ResourceGrid
-    from sionna_b200.phy.mimo import StreamManagement
-    name, b, num_tx, spt, rx, ant, m, assoc = cfg
-    s_ = 3
-    txs = num_tx * spt
-    f_ = txs * max(1, round(12 / txs))
-    rg = ResourceGrid(s_, f_, 15e3, num_tx=num_tx, num_streams_per_tx=spt, pilot_pattern="kronecker",
-                      pilot_ofdm_symbol_indices=[1])
-    sm = StreamManagement(np.array(assoc), spt)
-    pts = MAP.qam(m).astype(np.complex64)
-    h = _c(rng, (b, rx, ant, num_tx, spt, s_, f_))
-    x = pts[rng.integers(0, len(pts), (b, num_tx, spt, s_, f_))]
-    no = rng.uniform(0.02, 0.06, size=(b, rx, ant)).astype(np.float32)
-    y = np.einsum("brmtksf,btksf->brmsf", h.astype(np.complex128), x)
-    y = (y + _c(rng, y.shape) * np.sqrt(no)[..., None, None]).astype(np.complex64)
-    ev = (0.01 * rng.uniform(size=(b, rx, ant, num_tx, spt, s_, f_))).astype(np.float32)
-    return rg, sm, F.stream_management(assoc, spt), y, h, ev, no, pts
 
 
 # (name, batch, num_tx, streams per tx, num_rx, rx antennas, bits per symbol, association)
@@ -256,7 +196,7 @@ OFDM = [("siso", 8, 1, 1, 1, 1, 4, [[1]]),
 def test_ofdm_against_oracle(cuda_device, cfg):
     from sionna_b200.phy.ofdm import EPDetector, MMSEPICDetector
     rng = np.random.default_rng(zlib.crc32(cfg[0].encode()))
-    rg, sm, smr, y, h, ev, no, pts = _ofdm_case(cfg, rng)
+    rg, sm, smr, y, h, ev, no, pts = ofdm_detection_case(cfg, rng, (0.02, 0.06))
     m = cfg[6]
     mask = rg.pilot_pattern.mask.astype(bool)
     args = [torch.as_tensor(v).to(cuda_device) for v in (y, h, ev, no)]
@@ -273,7 +213,8 @@ def test_ofdm_against_oracle(cuda_device, cfg):
     keep = _keep(f"{cfg[0]} EP", g1, g2, g3)
     got = EPDetector("bit", rg, sm, m)(*args).cpu().numpy()
     assert got.shape == ref.shape == (b, tx, st, nd * m)
-    bad.append(_envelope(f"{cfg[0]} EP LLRs", got.reshape(shp)[keep], f32.reshape(shp)[keep], ref.reshape(shp)[keep]))
+    bad.append(envelope(f"{cfg[0]} EP LLRs", got.reshape(shp)[keep], f32.reshape(shp)[keep], ref.reshape(shp)[keep],
+                        BAR))
     assert np.array_equal(EPDetector("bit", rg, sm, m, hard_out=True)(*args).cpu().numpy().reshape(shp)[keep],
                           hb.reshape(shp)[keep])
     assert np.array_equal(EPDetector("symbol", rg, sm, m, hard_out=True)(*args).cpu().numpy()[keep], hs[keep])
@@ -289,8 +230,8 @@ def test_ofdm_against_oracle(cuda_device, cfg):
     det = MMSEPICDetector("bit", "app", rg, sm, 2, "qam", m)
     got = det(args[0], args[1], dpr, args[2], args[3]).cpu().numpy()
     assert got.shape == ref.shape
-    bad.append(_envelope(f"{cfg[0]} MMSE-PIC LLRs", got.reshape(shp)[keep], f32.reshape(shp)[keep],
-                         ref.reshape(shp)[keep]))
+    bad.append(envelope(f"{cfg[0]} MMSE-PIC LLRs", got.reshape(shp)[keep], f32.reshape(shp)[keep],
+                        ref.reshape(shp)[keep], BAR))
     hard = MMSEPICDetector("bit", "app", rg, sm, 2, "qam", m, hard_out=True)(args[0], args[1], dpr, args[2], args[3])
     assert np.array_equal(hard.cpu().numpy().reshape(shp)[keep], hb.reshape(shp)[keep])
     sym = MMSEPICDetector("symbol", "app", rg, sm, 2, "qam", m)(
@@ -306,7 +247,7 @@ def test_batch_dimensions_broadcast(cuda_device):
     from sionna_b200.phy.mimo import EPDetector, MMSEPICDetector
     rng = np.random.default_rng(12)
     pts = MAP.qam(4)
-    y, h, s, ind = _problem(rng, 96, 2, 2, pts, 0.05)
+    y, h, s, ind = mimo_problem(rng, 96, 2, 2, pts, 0.05, return_indices=True)
     s1 = s[0]
     dev = lambda v: torch.from_numpy(np.ascontiguousarray(v)).to(cuda_device)
     pr = _prior(rng, "random", ind, 4)
@@ -345,7 +286,7 @@ def test_constructor_errors(cuda_device):
     with pytest.raises(ValueError):
         MMSEPICDetector("bit", constellation_type="qam", num_bits_per_symbol=12)
     rng = np.random.default_rng(2)
-    y, h, s, _ = _problem(rng, 4, 17, 17, MAP.qam(2), 0.1)
+    y, h, s = mimo_problem(rng, 4, 17, 17, MAP.qam(2), 0.1)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
     with pytest.raises(ValueError):
         EPDetector("bit", 2)(*dev)                                  # 17 streams
@@ -363,7 +304,7 @@ def test_double_precision_falls_back_with_a_warning(cuda_device):
     from sionna_b200.phy.block import PrecisionWarning
     rng = np.random.default_rng(5)
     pts = MAP.qam(2)
-    y, h, s, ind = _problem(rng, 256, 4, 2, pts, 0.1)
+    y, h, s, ind = mimo_problem(rng, 256, 4, 2, pts, 0.1, return_indices=True)
     pr = _prior(rng, "random", ind, 2)
     for cls, args, extra in ((EPDetector, ("bit", 2), ()), (MMSEPICDetector, ("bit", "app", 2, "qam", 2), (pr,))):
         single = cls(*args)(*(torch.from_numpy(v).to(cuda_device) for v in (y, h, s) + extra))

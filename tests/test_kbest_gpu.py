@@ -13,9 +13,9 @@ import pytest
 import torch
 
 from oracle import mapping as MAP
-from oracle import ofdm as F
 from oracle.kbest import kbest_detect, ofdm_kbest_detect
 from oracle.mimo import ml_detect
+from oracle.parity import cnormal, constellation, envelope, mimo_problem, ofdm_detection_case
 
 BAR = (2.0, 4.0)
 GAP = 1e-4
@@ -30,54 +30,11 @@ EXCLUDED = {                                    # cases allowed to exclude more 
 }                                               # (the share depends on the inputs and the oracle only, not the kernel)
 
 
-def _c(rng, shape, scale=1.0):
-    return ((rng.normal(size=shape) + 1j * rng.normal(size=shape)) * scale / np.sqrt(2)).astype(np.complex64)
-
-
-def _problem(rng, num, m, k, points, no):
-    """y = h x + n with non-diagonal noise covariances s = no (I + 0.5 A A^H / m)."""
-    h = _c(rng, (num, m, k))
-    x = points[rng.integers(0, len(points), (num, k))]
-    a = _c(rng, (num, m, m))
-    s = (no * (np.eye(m) + 0.5 * a @ np.conj(np.swapaxes(a, -1, -2)) / m)).astype(np.complex64)
-    n = (np.linalg.cholesky(s.astype(np.complex128)) @ _c(rng, (num, m, 1)))[..., 0]
-    return ((h @ x[..., None])[..., 0] + n).astype(np.complex64), h, s
-
-
-def _err(got, ref):
-    fin = np.isfinite(ref)
-    den = np.sqrt(np.mean(np.where(fin, ref, 0) ** 2, axis=-1, keepdims=True))
-    return np.where(fin, np.abs(got - ref), 0) / np.maximum(den, 1e-30)
-
-
-def _envelope(what, got, f32, ref, bar=BAR):
-    """'' if got's error is within bar = (rms, max) times f32's, both against ref, else the measurement."""
-    fin = np.isfinite(ref)
-    assert np.array_equal(np.isfinite(got), fin), f"{what}: kernel finite where the oracle is not (or vice versa)"
-    assert np.array_equal(np.isfinite(f32), fin), f"{what}: complex64 oracle finite where the oracle is not"
-    a, b = _err(got, ref), _err(f32, ref)
-    rms_a, max_a = float(np.sqrt(np.mean(a ** 2))), float(a.max())
-    rms_b, max_b = float(np.sqrt(np.mean(b ** 2))), float(b.max())
-    line = (f"{what}: kernel rms {rms_a:.2e} max {max_a:.2e} | complex64 numpy rms {rms_b:.2e} max {max_b:.2e} "
-            f"| ratio rms {rms_a / max(rms_b, 1e-30):.2f} max {max_a / max(max_b, 1e-30):.2f}")
-    print(line)
-    return "" if rms_a <= bar[0] * rms_b and max_a <= bar[1] * max_b else line
-
-
 def _keep(what, gap):
     keep = gap > GAP
     print(f"{what}: {1 - keep.mean():.3%} of the problems excluded (decision gap <= {GAP})")
     assert 1 - keep.mean() < EXCLUDED.get(what, 0.01), what
     return keep
-
-
-def _constellation(kind, m):
-    from sionna_b200.phy.mapping import Constellation
-    if kind == "custom":
-        rng = np.random.default_rng(99)
-        pts = (rng.normal(size=2 ** m) + 1j * rng.normal(size=2 ** m)).astype(np.complex64)
-        return Constellation("custom", m, points=pts, normalize=True, center=True)
-    return Constellation(kind, m)
 
 
 # (name, streams, constellation type, bits per symbol, antennas, real representation, k, problems, no, LLR clip)
@@ -101,10 +58,10 @@ DENSE = [("qpsk 4x4 k16", 4, "qam", 2, 4, False, 16, 2048, 0.1, 20.0),
 def test_dense_kbest_against_oracle(cuda_device, case):
     from sionna_b200.phy.mimo import KBestDetector
     name, ns, kind, m, mm, real_rep, k, num, no, clip = case
-    const = _constellation(kind, m)
+    const = constellation(kind, m)
     pts = const().cpu().numpy().astype(np.complex64)
     rng = np.random.default_rng(zlib.crc32(name.encode()))
-    y, h, s = _problem(rng, num, mm, ns, pts, no)
+    y, h, s = mimo_problem(rng, num, mm, ns, pts, no)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
     kw = dict(real_rep=real_rep)
     ref, gap = kbest_detect(y, h, s, pts, k, "bit", llr_clip=clip, **kw)
@@ -114,7 +71,7 @@ def test_dense_kbest_against_oracle(cuda_device, case):
     det.list2llr.llr_clip_val = clip
     got = det(*dev).cpu().numpy()
     assert got.shape == ref.shape == (num, ns, m)
-    bad = _envelope(f"{name} LLRs", got[keep], f32[keep], ref[keep])
+    bad = envelope(f"{name} LLRs", got[keep], f32[keep], ref[keep], BAR)
     for output in ("bit", "symbol"):
         want, _ = kbest_detect(y, h, s, pts, k, output, hard_out=True, **kw)
         hard = KBestDetector(output, ns, k, constellation=const, hard_out=True, use_real_rep=real_rep)(*dev)
@@ -130,7 +87,7 @@ def test_list2llr_clip_is_read_at_every_call(cuda_device):
     from sionna_b200.phy.mimo import KBestDetector
     rng = np.random.default_rng(8)
     pts = MAP.qam(4).astype(np.complex64)
-    y, h, s = _problem(rng, 256, 4, 2, pts, 0.01)
+    y, h, s = mimo_problem(rng, 256, 4, 2, pts, 0.01)
     det = KBestDetector("bit", 2, 4, "qam", 4)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
     a = det(*dev)
@@ -153,7 +110,7 @@ def test_full_k_matches_ml_maxlog(cuda_device, ns, m, real_rep):
     from sionna_b200.phy.mimo import KBestDetector, MaximumLikelihoodDetector
     rng = np.random.default_rng(31 + ns + m + real_rep)
     pts = MAP.qam(m).astype(np.complex64)
-    y, h, s = _problem(rng, 1024, 4, ns, pts, 0.1)
+    y, h, s = mimo_problem(rng, 1024, 4, ns, pts, 0.1)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
     kb = KBestDetector("bit", ns, len(pts) ** ns, "qam", m, use_real_rep=real_rep)
     kb.list2llr.llr_clip_val = np.inf
@@ -161,8 +118,8 @@ def test_full_k_matches_ml_maxlog(cuda_device, ns, m, real_rep):
     ml = MaximumLikelihoodDetector("bit", "maxlog", ns, "qam", m)(*dev).cpu().numpy()
     ref = ml_detect(y, h, s, pts, "maxlog", "bit")
     f32 = ml_detect(y, h, s, pts, "maxlog", "bit", dtype=np.complex64)
-    bad = [_envelope(f"full k {ns}x{2 ** m}-QAM real={real_rep} kbest", got, f32, ref),
-           _envelope(f"full k {ns}x{2 ** m}-QAM real={real_rep} ML kernel", ml, f32, ref)]
+    bad = [envelope(f"full k {ns}x{2 ** m}-QAM real={real_rep} kbest", got, f32, ref, BAR),
+           envelope(f"full k {ns}x{2 ** m}-QAM real={real_rep} ML kernel", ml, f32, ref, BAR)]
     assert not any(bad), "\n".join(b for b in bad if b)
 
 
@@ -177,7 +134,7 @@ def test_noiseless_problems_have_no_errors(cuda_device, kind, bits, real_rep, ns
     from sionna_b200.phy.mimo import KBestDetector
     rng = np.random.default_rng(70 + bits + 5 * real_rep + 11 * (kind == "pam"))
     pts = (MAP.qam(bits) if kind == "qam" else MAP.pam(bits)).astype(np.complex64)
-    h = _c(rng, (100, ant, ns))
+    h = cnormal(rng, (100, ant, ns))
     ind = rng.integers(0, len(pts), (100, ns))
     y = (h @ pts[ind][..., None])[..., 0]
     s = (1e-9 * np.eye(ant)).astype(np.complex64)
@@ -186,27 +143,6 @@ def test_noiseless_problems_have_no_errors(cuda_device, kind, bits, real_rep, ns
     assert np.array_equal(sym, ind)
     b = KBestDetector("bit", ns, k, kind, bits, hard_out=True, use_real_rep=real_rep)(*dev).cpu().numpy()
     assert np.array_equal(b, (ind[..., None] >> np.arange(bits - 1, -1, -1)) & 1)
-
-
-def _ofdm_case(cfg, rng):
-    """(rg, sm, oracle stream dict, y_eff, h, err_var, no, points) on a 3-symbol Kronecker grid (symbol 1 pilots)."""
-    from sionna_b200.phy.ofdm import ResourceGrid
-    from sionna_b200.phy.mimo import StreamManagement
-    name, b, num_tx, spt, rx, ant, m, assoc = cfg[:8]
-    s_ = 3
-    txs = num_tx * spt
-    f_ = txs * max(1, round(12 / txs))
-    rg = ResourceGrid(s_, f_, 15e3, num_tx=num_tx, num_streams_per_tx=spt, pilot_pattern="kronecker",
-                      pilot_ofdm_symbol_indices=[1])
-    sm = StreamManagement(np.array(assoc), spt)
-    pts = MAP.qam(m).astype(np.complex64)
-    h = _c(rng, (b, rx, ant, num_tx, spt, s_, f_))
-    x = pts[rng.integers(0, len(pts), (b, num_tx, spt, s_, f_))]
-    no = rng.uniform(0.02, 0.06, size=(b, rx, ant)).astype(np.float32)
-    y = np.einsum("brmtksf,btksf->brmsf", h.astype(np.complex128), x)
-    y = (y + _c(rng, y.shape) * np.sqrt(no)[..., None, None]).astype(np.complex64)
-    ev = (0.01 * rng.uniform(size=(b, rx, ant, num_tx, spt, s_, f_))).astype(np.float32)
-    return rg, sm, F.stream_management(assoc, spt), y, h, ev, no, pts
 
 
 # (name, batch, num_tx, streams per tx, num_rx, rx antennas, bits per symbol, association, k, real representation)
@@ -220,7 +156,7 @@ OFDM = [("2 rx interfering", 8, 2, 2, 2, 4, 4, [[1, 0], [0, 1]], 8, False),
 def test_ofdm_kbest_against_oracle(cuda_device, cfg):
     from sionna_b200.phy.ofdm import KBestDetector
     rng = np.random.default_rng(zlib.crc32(cfg[0].encode()))
-    rg, sm, smr, y, h, ev, no, pts = _ofdm_case(cfg, rng)
+    rg, sm, smr, y, h, ev, no, pts = ofdm_detection_case(cfg, rng, (0.02, 0.06))
     m, k, real_rep = cfg[6], cfg[8], cfg[9]
     ns = sm.num_streams_per_rx
     mask = rg.pilot_pattern.mask.astype(bool)
@@ -232,7 +168,7 @@ def test_ofdm_kbest_against_oracle(cuda_device, cfg):
     got = KBestDetector("bit", ns, k, rg, sm, "qam", m, use_real_rep=real_rep)(*args).cpu().numpy()
     assert got.shape == ref.shape
     shp = got.shape[:-1] + (-1, m)                              # one stream's LLRs of one RE share a scale
-    bad = _envelope(f"{cfg[0]} LLRs", got.reshape(shp)[keep], f32.reshape(shp)[keep], ref.reshape(shp)[keep])
+    bad = envelope(f"{cfg[0]} LLRs", got.reshape(shp)[keep], f32.reshape(shp)[keep], ref.reshape(shp)[keep], BAR)
     for output in ("bit", "symbol"):
         want, _ = ofdm_kbest_detect(y64, h64, ev64, no, mask, smr, pts, k, output, hard_out=True, real_rep=real_rep)
         hard = KBestDetector(output, ns, k, rg, sm, "qam", m, hard_out=True, use_real_rep=real_rep)(*args)
@@ -381,7 +317,7 @@ def test_constructor_errors(cuda_device):
     # fewer receive antennas than streams (test_too_few_rx_antennas)
     rng = np.random.default_rng(1)
     pts = MAP.qam(4).astype(np.complex64)
-    h = torch.from_numpy(_c(rng, (100, 3, 4))).to(cuda_device)
+    h = torch.from_numpy(cnormal(rng, (100, 3, 4))).to(cuda_device)
     y = h @ torch.from_numpy(pts[rng.integers(0, 16, (100, 4, 1))]).to(cuda_device)
     s = torch.from_numpy((1e-9 * np.eye(3)).astype(np.complex64)).to(cuda_device)
     for real_rep in (False, True):
@@ -395,7 +331,7 @@ def test_double_precision_falls_back_with_a_warning(cuda_device):
     from sionna_b200.phy.block import PrecisionWarning
     rng = np.random.default_rng(5)
     pts = MAP.qam(2).astype(np.complex64)                       # QPSK: the same fp32 points in both precisions
-    y, h, s = _problem(rng, 256, 4, 2, pts, 0.1)
+    y, h, s = mimo_problem(rng, 256, 4, 2, pts, 0.1)
     single = KBestDetector("bit", 2, 8, "qam", 2)(*(torch.from_numpy(v).to(cuda_device) for v in (y, h, s)))
     with pytest.warns(PrecisionWarning):
         double = KBestDetector("bit", 2, 8, "qam", 2, precision="double")(

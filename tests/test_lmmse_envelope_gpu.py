@@ -34,12 +34,14 @@ import torch
 
 from oracle import mapping as MAP
 from oracle import ofdm as F
+from oracle.parity import cnormal, envelope, mimo_problem, noise_covariance
 
 pytestmark = pytest.mark.gpu
 
 KS = (1, 2, 3, 4, 5, 8, 12, 15, 16)
 PAIRS = [(m, k) for k in KS for m in sorted({k, k + 1, 13, 16, 23, 24, 32}) if m >= k]
 NUM = 4097
+NO = 10 ** (-15.0 / 10)                         # 15 dB
 DEFAULT_BAR = (2.0, 3.0)
 BARS = {                                        # (rms, max) bar: worst measured ratio
     "lmmse_equalizer": (2.5, 3.5),              # tall systems 2.01 / 3.00 (whitening by forward substitution)
@@ -49,47 +51,6 @@ BARS = {                                        # (rms, max) bar: worst measured
     "ofdm diag x_hat": (3.2, 4.0),              # register kernel: 2.65 / 3.34
 }                                               # default: lmmse_matrix 1.58 / 2.36, ofdm general 1.64 / 1.96,
                                                 # ofdm diag no_eff 1.44 / 1.68
-
-
-def _c64(rng, shape, scale=1.0):
-    return ((rng.normal(size=shape) + 1j * rng.normal(size=shape)) * scale / np.sqrt(2)).astype(np.complex64)
-
-
-def _herm(a):
-    return np.conj(np.swapaxes(a, -1, -2))
-
-
-def _covariance(rng, num, m, no):
-    """Well-conditioned noise covariances no * (I + 0.5 A A^H / m), one per vector."""
-    a = _c64(rng, (num, m, m))
-    return (no * (np.eye(m) + 0.5 * a @ _herm(a) / m)).astype(np.complex64)
-
-
-def _problem(rng, m, k, snr_db=15.0):
-    """y = H x + n with QPSK ... 16-QAM x and n ~ CN(0, S): NUM vectors."""
-    h = _c64(rng, (NUM, m, k))
-    x = MAP.qam(4)[rng.integers(0, 16, (NUM, k))]
-    s = _covariance(rng, NUM, m, 10 ** (-snr_db / 10))
-    n = (np.linalg.cholesky(s.astype(np.complex128)) @ _c64(rng, (NUM, m, 1)))[..., 0]
-    y = ((h @ x[..., None])[..., 0] + n).astype(np.complex64)
-    return y, h, s
-
-
-def _rel(got, ref, axes=None):
-    """Elementwise |got - ref| over |ref| (axes=None) or over the rms of ref on `axes` (matrices with zero entries)."""
-    den = np.abs(ref) if axes is None else np.sqrt(np.mean(np.abs(ref) ** 2, axis=axes, keepdims=True))
-    return np.abs(got - ref) / np.maximum(den, 1e-30)
-
-
-def _envelope(what, got, f32, ref, bar=DEFAULT_BAR, axes=None):
-    """'' if got's error is within bar = (rms, max) times f32's, both against ref, else the measurement."""
-    a, b = _rel(got, ref, axes), _rel(f32, ref, axes)
-    rms_a, max_a = float(np.sqrt(np.mean(a ** 2))), float(a.max())
-    rms_b, max_b = float(np.sqrt(np.mean(b ** 2))), float(b.max())
-    line = (f"{what}: kernel rms {rms_a:.2e} max {max_a:.2e} | complex64 numpy rms {rms_b:.2e} max {max_b:.2e} "
-            f"| ratio rms {rms_a / rms_b:.2f} max {max_a / max_b:.2f} (bar {bar[0]:g} / {bar[1]:g})")
-    print(line)
-    return "" if rms_a <= bar[0] * rms_b and max_a <= bar[1] * max_b else line
 
 
 def _prefix_identical(fn, args, full):
@@ -105,7 +66,7 @@ def _prefix_identical(fn, args, full):
 def test_lmmse_equalizer_envelope(cuda_device, m, k, whiten):
     from sionna_b200.phy.mimo import lmmse_equalizer
     rng = np.random.default_rng(1000 * m + 10 * k + whiten)
-    y, h, s = _problem(rng, m, k)
+    y, h, s = mimo_problem(rng, NUM, m, k, MAP.qam(4), NO)
     x64, n64 = F.lmmse_equalizer_cholesky(y.astype(np.complex128), h.astype(np.complex128), s.astype(np.complex128),
                                           whiten)
     x32, n32 = F.lmmse_equalizer_cholesky(y, h, s, whiten)
@@ -113,8 +74,8 @@ def test_lmmse_equalizer_envelope(cuda_device, m, k, whiten):
     fn = lambda y_, h_, s_: lmmse_equalizer(y_, h_, s_, whiten_interference=whiten)   # noqa: E731
     xg, ng = fn(*args)
     bar = BARS["lmmse_equalizer square" if m == k else "lmmse_equalizer"]
-    bad = [_envelope(f"x_hat M={m} K={k} whiten={whiten}", xg.cpu().numpy(), x32, x64, bar),
-           _envelope(f"no_eff M={m} K={k} whiten={whiten}", ng.cpu().numpy(), n32, n64, bar)]
+    bad = [envelope(f"x_hat M={m} K={k} whiten={whiten}", xg.cpu().numpy(), x32, x64, bar, scale=np.abs(x64)),
+           envelope(f"no_eff M={m} K={k} whiten={whiten}", ng.cpu().numpy(), n32, n64, bar, scale=np.abs(n64))]
     _prefix_identical(fn, args, (xg, ng))
     assert not any(bad), "\n".join(b for b in bad if b)
 
@@ -123,22 +84,22 @@ def test_lmmse_equalizer_envelope(cuda_device, m, k, whiten):
 def test_whiten_channel_and_lmmse_matrix_envelope(cuda_device, m, k):
     from sionna_b200.phy.mimo import whiten_channel, lmmse_matrix
     rng = np.random.default_rng(2000 * m + k)
-    y, h, s = _problem(rng, m, k)
+    y, h, s = mimo_problem(rng, NUM, m, k, MAP.qam(4), NO)
     mats = (-2, -1)
     c128 = [v.astype(np.complex128) for v in (y, h, s)]
     yd, hd, sd = (torch.from_numpy(v).to(cuda_device) for v in (y, h, s))
     yw, hw, _ = whiten_channel(yd, hd, sd)
     (yw64, hw64), (yw32, hw32) = F.whiten_channel(*c128), F.whiten_channel(y, h, s)
-    bad = [_envelope(f"whiten y M={m} K={k}", yw.cpu().numpy(), yw32, yw64, BARS["whiten_channel"], axes=-1),
-           _envelope(f"whiten H M={m} K={k}", hw.cpu().numpy(), hw32, hw64, BARS["whiten_channel"], axes=mats)]
+    bad = [envelope(f"whiten y M={m} K={k}", yw.cpu().numpy(), yw32, yw64, BARS["whiten_channel"], axis=-1),
+           envelope(f"whiten H M={m} K={k}", hw.cpu().numpy(), hw32, hw64, BARS["whiten_channel"], axis=mats)]
     _prefix_identical(lambda *a: whiten_channel(*a, return_s=False), (yd, hd, sd), (yw, hw))
     g = lmmse_matrix(hd, sd)
-    bad.append(_envelope(f"lmmse_matrix(h, s) M={m} K={k}", g.cpu().numpy(), F.lmmse_matrix(h, s),
-                         F.lmmse_matrix(c128[1], c128[2]), axes=mats))
+    bad.append(envelope(f"lmmse_matrix(h, s) M={m} K={k}", g.cpu().numpy(), F.lmmse_matrix(h, s),
+                        F.lmmse_matrix(c128[1], c128[2]), DEFAULT_BAR, axis=mats))
     _prefix_identical(lmmse_matrix, (hd, sd), g)
     g = lmmse_matrix(hd)
-    bad.append(_envelope(f"lmmse_matrix(h) M={m} K={k}", g.cpu().numpy(), F.lmmse_matrix(h), F.lmmse_matrix(c128[1]),
-                         axes=mats))
+    bad.append(envelope(f"lmmse_matrix(h) M={m} K={k}", g.cpu().numpy(), F.lmmse_matrix(h), F.lmmse_matrix(c128[1]),
+                        DEFAULT_BAR, axis=mats))
     _prefix_identical(lmmse_matrix, (hd,), g)
     assert not any(bad), "\n".join(b for b in bad if b)
 
@@ -147,7 +108,7 @@ def test_whiten_channel_and_lmmse_matrix_envelope(cuda_device, m, k):
 def test_inv_cholesky_envelope(cuda_device, m):
     from sionna_b200.phy.utils import inv_cholesky
     rng = np.random.default_rng(3000 + m)
-    s = _covariance(rng, NUM, m, 1.0)
+    s = noise_covariance(rng, NUM, m, 1.0)
     sd = torch.from_numpy(s).to(cuda_device)
     li = inv_cholesky(sd)
     ref = F.inv_cholesky(s.astype(np.complex128))
@@ -155,7 +116,7 @@ def test_inv_cholesky_envelope(cuda_device, m):
     assert f32.dtype == np.complex64
     got = li.cpu().numpy()
     assert np.all(np.triu(got, 1) == 0)
-    bad = _envelope(f"inv_cholesky M={m}", got, f32, ref, BARS["inv_cholesky"], axes=(-2, -1))
+    bad = envelope(f"inv_cholesky M={m}", got, f32, ref, BARS["inv_cholesky"], axis=(-2, -1))
     _prefix_identical(inv_cholesky, (sd,), li)
     assert not bad, bad
 
@@ -189,11 +150,11 @@ def test_ofdm_lmmse_equalizer_envelope(cuda_device, m, k, interf):
                       pilot_ofdm_symbol_indices=[1])
     sm = StreamManagement(assoc, k)
     rng = np.random.default_rng(4000 + 100 * m + 10 * k + interf)
-    h = _c64(rng, (b, rx, m, num_tx, k, s_, f_))
+    h = cnormal(rng, (b, rx, m, num_tx, k, s_, f_))
     x = MAP.qam(4)[rng.integers(0, 16, (b, num_tx, k, s_, f_))]
     no = rng.uniform(0.02, 0.06, size=(b, rx, m)).astype(np.float32)
     y = np.einsum("brmtksf,btksf->brmsf", h.astype(np.complex128), x)
-    y = (y + _c64(rng, y.shape) * np.sqrt(no)[..., None, None]).astype(np.complex64)
+    y = (y + cnormal(rng, y.shape) * np.sqrt(no)[..., None, None]).astype(np.complex64)
     ev = (0.01 * rng.uniform(size=h.shape)).astype(np.float32)
     mask = rg.pilot_pattern.mask.astype(bool)
     smr = F.stream_management(assoc, k)
@@ -205,9 +166,10 @@ def test_ofdm_lmmse_equalizer_envelope(cuda_device, m, k, interf):
     xg, ng = eq(*args)
     assert xg.shape == x64.shape == (b, num_tx, k, rg.num_data_symbols)
     diag = not interf and k <= 4
-    bad = [_envelope(f"ofdm x_hat M={m} K={k} interf={interf}", xg.cpu().numpy(), x32, x64,
-                     BARS["ofdm diag x_hat"] if diag else DEFAULT_BAR),
-           _envelope(f"ofdm no_eff M={m} K={k} interf={interf}", ng.cpu().numpy(), n32, n64)]
+    bad = [envelope(f"ofdm x_hat M={m} K={k} interf={interf}", xg.cpu().numpy(), x32, x64,
+                    BARS["ofdm diag x_hat"] if diag else DEFAULT_BAR, scale=np.abs(x64)),
+           envelope(f"ofdm no_eff M={m} K={k} interf={interf}", ng.cpu().numpy(), n32, n64, DEFAULT_BAR,
+                    scale=np.abs(n64))]
     x1, n1 = eq(*(a[:1] for a in args))
     assert torch.equal(x1, xg[:1]) and torch.equal(n1, ng[:1])
     assert not any(bad), "\n".join(b for b in bad if b)

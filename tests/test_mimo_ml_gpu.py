@@ -11,8 +11,8 @@ import pytest
 import torch
 
 from oracle import mapping as MAP
-from oracle import ofdm as F
 from oracle.mimo import ml_detect, ofdm_ml_detect
+from oracle.parity import constellation, envelope, mimo_problem, ofdm_detection_case
 
 pytestmark = pytest.mark.gpu
 
@@ -24,43 +24,6 @@ BARS = {                                        # (rms, max) bars of the cases t
     "custom 8-point": (5.0, 8.0),               # 4.41 / 6.50, bit app without prior: this random constellation's app
 }                                               # LLRs are small next to its logits, the difference keeps the kernel's
                                                 # independent rounding of each point's exp sum (symbol logits: 1.16 / 1.24)
-
-
-def _c(rng, shape, scale=1.0):
-    return ((rng.normal(size=shape) + 1j * rng.normal(size=shape)) * scale / np.sqrt(2)).astype(np.complex64)
-
-
-def _covariance(rng, num, m, no):
-    """Non-diagonal noise covariances no * (I + 0.5 A A^H / m)."""
-    a = _c(rng, (num, m, m))
-    return (no * (np.eye(m) + 0.5 * a @ np.conj(np.swapaxes(a, -1, -2)) / m)).astype(np.complex64)
-
-
-def _problem(rng, num, m, k, points, no):
-    h = _c(rng, (num, m, k))
-    x = points[rng.integers(0, len(points), (num, k))]
-    s = _covariance(rng, num, m, no)
-    n = (np.linalg.cholesky(s.astype(np.complex128)) @ _c(rng, (num, m, 1)))[..., 0]
-    return ((h @ x[..., None])[..., 0] + n).astype(np.complex64), h, s
-
-
-def _err(got, ref):
-    fin = np.isfinite(ref)
-    den = np.sqrt(np.mean(np.where(fin, ref, 0) ** 2, axis=-1, keepdims=True))
-    return np.where(fin, np.abs(got - ref), 0) / np.maximum(den, 1e-30)
-
-
-def _envelope(what, got, f32, ref, bar=BAR):
-    """'' if got's error is within bar = (rms, max) times f32's, both against ref, else the measurement."""
-    fin = np.isfinite(ref)
-    assert np.array_equal(np.isfinite(got), fin), f"{what}: kernel finite where the oracle is not (or vice versa)"
-    a, b = _err(got, ref), _err(f32, ref)
-    rms_a, max_a = float(np.sqrt(np.mean(a ** 2))), float(a.max())
-    rms_b, max_b = float(np.sqrt(np.mean(b ** 2))), float(b.max())
-    line = (f"{what}: kernel rms {rms_a:.2e} max {max_a:.2e} | complex64 numpy rms {rms_b:.2e} max {max_b:.2e} "
-            f"| ratio rms {rms_a / max(rms_b, 1e-30):.2f} max {max_a / max(max_b, 1e-30):.2f}")
-    print(line)
-    return "" if rms_a <= bar[0] * rms_b and max_a <= bar[1] * max_b else line
 
 
 def _margin_bound(f32, ref, symbol, bar=BAR):
@@ -87,15 +50,6 @@ def _hard_check(what, got, ref_soft, ref_hard, bound, symbol):
     assert np.array_equal(got[keep], ref_hard[keep]), what
 
 
-def _constellation(kind, m):
-    from sionna_b200.phy.mapping import Constellation
-    if kind == "custom":
-        rng = np.random.default_rng(99)
-        pts = (rng.normal(size=2 ** m) + 1j * rng.normal(size=2 ** m)).astype(np.complex64)
-        return Constellation("custom", m, points=pts, normalize=True, center=True)
-    return Constellation(kind, m)
-
-
 # (name, K, bits per symbol, M, constellation type, problems, no)
 DENSE = [(f"K{k}-{'qpsk' if m == 2 else '16qam'}", k, m, 4, "qam", 128 if m ** k >= 4 ** 4 else 512, 0.1)
          for k in (1, 2, 3, 4) for m in (2, 4)]
@@ -111,10 +65,10 @@ DENSE += [("8 streams qpsk", 8, 2, 8, "qam", 64, 0.1),
 def test_dense_ml_against_oracle(cuda_device, case):
     from sionna_b200.phy.mimo import MaximumLikelihoodDetector
     name, k, m, mm, kind, num, no = case
-    const = _constellation(kind, m)
+    const = constellation(kind, m)
     pts = const().cpu().numpy().astype(np.complex64)
     rng = np.random.default_rng(zlib.crc32(name.encode()))
-    y, h, s = _problem(rng, num, mm, k, pts, no)
+    y, h, s = mimo_problem(rng, num, mm, k, pts, no)
     dev = [torch.from_numpy(v).to(cuda_device) for v in (y, h, s)]
     bad = []
     for output in ("bit", "symbol"):
@@ -130,7 +84,7 @@ def test_dense_ml_against_oracle(cuda_device, case):
                 det = MaximumLikelihoodDetector(output, method, k, constellation=const)
                 got = det(*dev, prior=pd).cpu().numpy()
                 assert got.shape == ref.shape, tag
-                bad.append(_envelope(tag, got, f32, ref, BARS.get(name, BAR)))
+                bad.append(envelope(tag, got, f32, ref, BARS.get(name, BAR)))
                 hard = MaximumLikelihoodDetector(output, method, k, constellation=const, hard_out=True)(*dev, prior=pd)
                 want = ml_detect(y, h, s, pts, method, output, prior, hard_out=True)
                 assert hard.dtype == (torch.float32 if output == "bit" else torch.int32)
@@ -142,7 +96,7 @@ def test_dense_ml_leading_batch_dims(cuda_device):
     from sionna_b200.phy.mimo import MaximumLikelihoodDetector
     rng = np.random.default_rng(3)
     pts = MAP.qam(4).astype(np.complex64)
-    y, h, s = _problem(rng, 24, 4, 2, pts, 0.1)
+    y, h, s = mimo_problem(rng, 24, 4, 2, pts, 0.1)
     det = MaximumLikelihoodDetector("bit", "app", 2, "qam", 4)
     flat = det(*(torch.from_numpy(v).to(cuda_device) for v in (y, h, s)))
     shaped = det(*(torch.from_numpy(v.reshape((2, 3, 4) + v.shape[1:])).to(cuda_device) for v in (y, h, s)))
@@ -157,13 +111,13 @@ def test_high_snr_outputs_stay_finite(cuda_device, output):
     from sionna_b200.phy.mimo import MaximumLikelihoodDetector
     rng = np.random.default_rng(17)
     pts = MAP.qam(4).astype(np.complex64)
-    y, h, s = _problem(rng, 128, 4, 4, pts, 1e-4)
+    y, h, s = mimo_problem(rng, 128, 4, 4, pts, 1e-4)
     ref = ml_detect(y, h, s, pts, "app", output)
     f32 = ml_detect(y, h, s, pts, "app", output, dtype=np.complex64)
     got = MaximumLikelihoodDetector(output, "app", 4, "qam", 4)(*(torch.from_numpy(v).to(cuda_device) for v in (y, h, s)))
     got = got.cpu().numpy()
     assert np.all(np.isfinite(got[np.isfinite(ref)]))
-    bad = _envelope(f"high SNR {output}", got, f32, ref)
+    bad = envelope(f"high SNR {output}", got, f32, ref, BAR)
     assert not bad, bad
 
 
@@ -181,30 +135,6 @@ def test_oversize_configuration_is_rejected_before_launch():
         OFDMML("bit", "app", rg, StreamManagement(np.ones((1, 1), int), 3), "qam", 8)   # 256^3
 
 
-def _ofdm_case(cfg, rng):
-    """(rg, sm, oracle stream dict, y_eff, h, err_var, no, points) on a 3-symbol Kronecker grid (symbol 1 pilots)."""
-    from sionna_b200.phy.ofdm import ResourceGrid
-    from sionna_b200.phy.mimo import StreamManagement
-    name, b, num_tx, spt, rx, ant, m, assoc, ev_shape, no_shape = cfg
-    s_ = 3
-    txs = num_tx * spt
-    f_ = txs * max(1, round(12 / txs))
-    rg = ResourceGrid(s_, f_, 15e3, num_tx=num_tx, num_streams_per_tx=spt, pilot_pattern="kronecker",
-                      pilot_ofdm_symbol_indices=[1])
-    sm = StreamManagement(np.array(assoc), spt)
-    pts = MAP.qam(m).astype(np.complex64)
-    h = _c(rng, (b, rx, ant, num_tx, spt, s_, f_))
-    x = pts[rng.integers(0, len(pts), (b, num_tx, spt, s_, f_))]
-    no_full = rng.uniform(0.05, 0.15, size=(b, rx, ant)).astype(np.float32)
-    no = no_full[(slice(None),) * len(no_shape) + (0,) * (3 - len(no_shape))].reshape(no_shape) if no_shape else \
-        np.float32(0.1)
-    no_b = np.broadcast_to(np.asarray(no).reshape(np.shape(no) + (1,) * (3 - np.ndim(no))), (b, rx, ant))
-    y = np.einsum("brmtksf,btksf->brmsf", h.astype(np.complex128), x)
-    y = (y + _c(rng, y.shape) * np.sqrt(no_b)[..., None, None]).astype(np.complex64)
-    ev = (0.01 * rng.uniform(size=ev_shape)).astype(np.float32) if ev_shape else np.float32(0.005)
-    return rg, sm, F.stream_management(assoc, spt), y, h, ev, no, pts
-
-
 # (name, batch, num_tx, streams per tx, num_rx, rx antennas, bits per symbol, association, err_var shape, no shape)
 OFDM = [("siso", 16, 1, 1, 1, 1, 4, [[1]], (), ()),
         ("4x16 mu-mimo", 2, 4, 1, 1, 16, 4, [[1, 1, 1, 1]], (2, 1, 16, 4, 1, 3, 12), (2, 1, 16)),
@@ -217,7 +147,7 @@ OFDM = [("siso", 16, 1, 1, 1, 1, 4, [[1]], (), ()),
 def test_ofdm_ml_against_oracle(cuda_device, cfg):
     from sionna_b200.phy.ofdm import MaximumLikelihoodDetector
     rng = np.random.default_rng(zlib.crc32(cfg[0].encode()))
-    rg, sm, smr, y, h, ev, no, pts = _ofdm_case(cfg, rng)
+    rg, sm, smr, y, h, ev, no, pts = ofdm_detection_case(cfg, rng, (0.05, 0.15), cfg[8], cfg[9])
     mask = rg.pilot_pattern.mask.astype(bool)
     m = cfg[6]
     args = [torch.as_tensor(v).to(cuda_device) for v in (y, h, ev, no)]
@@ -233,7 +163,7 @@ def test_ofdm_ml_against_oracle(cuda_device, cfg):
             if output == "bit":                                     # one stream's LLRs of one RE share a scale
                 shp = got.shape[:-1] + (-1, m)
                 got, ref, f32 = got.reshape(shp), ref.reshape(shp), f32.reshape(shp)
-            bad.append(_envelope(tag, got, f32, ref, BARS.get(cfg[0], BAR)))
+            bad.append(envelope(tag, got, f32, ref, BARS.get(cfg[0], BAR)))
     for output in ("bit", "symbol"):                                # hard bits and hard symbol indices
         sym = output == "symbol"
         hard = MaximumLikelihoodDetector(output, "maxlog", rg, sm, "qam", m, hard_out=True)(*args).cpu().numpy()
@@ -253,7 +183,7 @@ def test_ofdm_ml_with_prior_single_receiver(cuda_device, output, streams):
     from sionna_b200.phy.ofdm import MaximumLikelihoodDetectorWithPrior
     cfg = ("prior", 2, 1, streams, 1, 4, 4, [[1]], (2, 1, 4, 1, streams, 3, 12), (2, 1, 4))
     rng = np.random.default_rng(23 + (output == "bit") + 10 * streams)
-    rg, sm, smr, y, h, ev, no, pts = _ofdm_case(cfg, rng)
+    rg, sm, smr, y, h, ev, no, pts = ofdm_detection_case(cfg, rng, (0.05, 0.15), cfg[8], cfg[9])
     mask = rg.pilot_pattern.mask.astype(bool)
     nd = rg.num_data_symbols
     shape = (2, 1, streams, nd * 4) if output == "bit" else (2, 1, streams, nd, 16)
@@ -268,7 +198,7 @@ def test_ofdm_ml_with_prior_single_receiver(cuda_device, output, streams):
         got = det(*args).cpu().numpy()
         if output == "bit":
             got, ref, f32 = (v.reshape(v.shape[:-1] + (-1, 4)) for v in (got, ref, f32))
-        bad.append(_envelope(f"with prior {streams} streams {output} {method}", got, f32, ref))
+        bad.append(envelope(f"with prior {streams} streams {output} {method}", got, f32, ref, BAR))
     assert not any(bad), "\n".join(b for b in bad if b)
 
 
@@ -332,7 +262,7 @@ def test_double_precision_falls_back_with_a_warning(cuda_device):
     from sionna_b200.phy.block import PrecisionWarning
     rng = np.random.default_rng(5)
     pts = MAP.qam(2).astype(np.complex64)
-    y, h, s = _problem(rng, 64, 2, 2, pts, 0.1)
+    y, h, s = mimo_problem(rng, 64, 2, 2, pts, 0.1)
     single = MaximumLikelihoodDetector("bit", "app", 2, "qam", 2)(*(torch.from_numpy(v).to(cuda_device) for v in (y, h, s)))
     with pytest.warns(PrecisionWarning):
         double = MaximumLikelihoodDetector("bit", "app", 2, "qam", 2, precision="double")(
