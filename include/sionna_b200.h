@@ -470,6 +470,34 @@ int sb_ofdm_mmse_pic(const float* d_y, const float* d_h_hat, const float* d_err_
                      int32_t streams_per_rx, int32_t interferers_per_rx, int32_t num_data, int32_t num_points,
                      int32_t num_iter, int32_t method, int32_t hard_out, void* stream);
 
+/* Transmit precoding (csrc/precoding.cu), complex64. kind 0: RZF, G = V D with V = H^H (H H^H + alpha I)^-1 computed
+ * as the adjoint of cholesky_solve(chol(H H^H + alpha I), H); kind 1: CBF, V = H^H; kind 2 (OFDM only): identity. D
+ * scales every column of V to unit norm, a zero column stays zero (mimo/precoding.py:12-245). alpha = 0 with K > M
+ * gives a singular Gram matrix; the outputs are then not finite. Limits: K <= 16 streams, M <= 1024 transmit
+ * antennas; beyond them SB_EUNSUPPORTED with a message. Malformed arguments return SB_EINVAL; all checks run before any
+ * device access.
+ * Dense problems: d_h [num, K, M]; d_alpha (RZF only; NULL: 0) one value (alpha_stride 0) or one per problem (1);
+ * d_x [num, K] (needed for d_gx). Outputs, either may be NULL but not both: d_g [num, M, K], d_gx = G x [num, M]. */
+int sb_mimo_precode(const float* d_h, const float* d_alpha, int64_t alpha_stride, const float* d_x, float* d_g,
+                    float* d_gx, int64_t num, int32_t K, int32_t M, int32_t kind, void* stream);
+/* RZFPrecoder / RZFPrecodedChannel / CBFPrecodedChannel / EyePrecodedChannel (ofdm/precoding.py:15-566) per resource
+ * element, K = num_streams_per_tx, M = num_tx_ant. d_h_hat [batch, num_rx, num_rx_ant, num_tx, M, S, fft_size] is the
+ * channel the precoder is computed from: stream k of transmitter j uses row k % num_rx_ant of the channel to receiver
+ * d_precoding_ind[j, k / num_rx_ant] (d_precoding_ind [num_tx, K / num_rx_ant], StreamManagement.precoding_ind).
+ * K must equal num_rx_per_tx * num_rx_ant (SB_EINVAL otherwise). d_alpha (RZF; NULL: 0) with element strides
+ * h_alpha_stride[4] over (batch, tx, symbol, subcarrier), d_tx_power (NULL: 1) with h_tx_power_stride[5] over
+ * (batch, tx, stream, symbol, subcarrier); a stride of 0 broadcasts. sqrt(tx_power) scales column k of G.
+ * Outputs, either may be NULL but not both: d_x_precoded = G x [batch, num_tx, M, S, fft_size] from d_x
+ * [batch, num_tx, K, S, fft_size]; d_h_eff [batch, num_rx, num_rx_ant, num_tx, K, S, num_effective_subcarriers] =
+ * H_ij G_j for every receiver i and transmitter j, computed from d_h (same layout as d_h_hat, may be the same
+ * pointer); d_sc_pos [fft_size] gives each subcarrier's column in h_eff, -1 for a nulled one. */
+int sb_ofdm_precode(const float* d_h_hat, const float* d_h, const int32_t* d_precoding_ind, const float* d_x,
+                    const float* d_alpha, const int64_t* h_alpha_stride, const float* d_tx_power,
+                    const int64_t* h_tx_power_stride, const int32_t* d_sc_pos, float* d_x_precoded, float* d_h_eff,
+                    int64_t batch, int32_t num_rx, int32_t num_rx_ant, int32_t num_tx, int32_t num_tx_ant,
+                    int32_t num_streams_per_tx, int32_t num_symbols, int32_t fft_size,
+                    int32_t num_effective_subcarriers, int32_t kind, void* stream);
+
 /* Fused receive front-end (csrc/frontend.cu): LS estimation at the pilots (+ PUSCH CDM de-spreading) + nearest /
  * linear interpolation + OFDM equaliser glue + LMMSE equalisation + square-QAM demapping in ONE launch, for receivers
  * without interfering streams and 1..4 streams (ofdm/channel_estimation.py:138-285, 364-734, ofdm/equalization.py:126-275,

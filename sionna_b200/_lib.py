@@ -81,6 +81,8 @@ SIGNATURES = {
     "sb_ofdm_ep": (i32, [vp] * 12 + [i64] + [i32] * 10 + [f32, i32, i32, vp]),
     "sb_mimo_mmse_pic": (i32, [vp] * 6 + [i64] + [i32] * 6 + [vp]),
     "sb_ofdm_mmse_pic": (i32, [vp] * 13 + [i64] + [i32] * 12 + [vp]),
+    "sb_mimo_precode": (i32, [vp, vp, i64, vp, vp, vp, i64, i32, i32, i32, vp]),
+    "sb_ofdm_precode": (i32, [vp] * 11 + [i64] + [i32] * 9 + [vp]),
 }
 
 

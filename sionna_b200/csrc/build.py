@@ -19,7 +19,7 @@ LIB = os.path.join(HERE, "..", "libsionna_b200.so")
 OBJ_DIR = os.path.join(HERE, "..", "..", "build", "obj")
 EXACT = ["common.cu", "ldpc_bp.cu", "ldpc_bp_qc.cu", "ldpc_bp_flat.cu", "ldpc_enc.cu", "phy_kernels.cu"]   # -fmad=false
 FAST = ["ofdm_mimo.cu", "channel.cu", "frontend.cu", "mimo_ml.cu", "mimo_kbest.cu",
-        "mimo_iterative.cu"]                                                                     # -fmad=true
+        "mimo_iterative.cu", "precoding.cu"]                                                     # -fmad=true
 SOURCES = EXACT + FAST
 HEADERS = ["sb_common.h", "sb_math.h", "sb_math2.cuh", "sb_logtab.h", "rng.cuh", "ldpc_graph.h", "ldpc_rules.cuh",
            "lmmse_diag.cuh", "dense_mimo.cuh", "demap_qam.cuh", "demap_prior.cuh", os.path.join("..", "..", "include", "sionna_b200.h")]

@@ -1,10 +1,12 @@
 // dense_mimo.cuh -- per-vector dense linear algebra, the OFDM per-resource-element problem assembly and the front half
-// of the MIMO detectors, shared by the LMMSE kernels (ofdm_mimo.cu) and the ML, K-Best, EP and MMSE-PIC detectors
-// (mimo_ml.cu, mimo_kbest.cu, mimo_iterative.cu), so all whiten with the same arithmetic.
+// of the MIMO detectors, shared by the LMMSE kernels (ofdm_mimo.cu), the ML, K-Best, EP and MMSE-PIC detectors
+// (mimo_ml.cu, mimo_kbest.cu, mimo_iterative.cu) and the precoders (precoding.cu), so all whiten and solve with the
+// same arithmetic.
 //   Scratch          per-thread view of a shared-memory matrix, interleaved by thread (element e of thread t at
 //                    [e * T + t]: conflict-free; ScratchOf<float> for real matrices); scratch_threads sizes the CTA,
 //                    detector_threads also under kScratchSmemCap with the error message
 //   chol_lower       L = chol(S), in place                                   (utils/linalg.py:28-32)
+//   chol_solve_col   one column of (L L^H)^-1 B                              (tf.linalg.cholesky_solve)
 //   whiten           y_w = L^-1 y, H_w = L^-1 H                              (mimo/utils.py:343-347)
 //   qr_record        modified Gram-Schmidt of [H_w | y_w] in a given column order: R, Q^H y_w, out-of-span term
 //                    (qr_record_size float2)
@@ -40,6 +42,24 @@ static __device__ void chol_lower(const Scratch& A, int n) {
             for (int k = 0; k < j; ++k) v = csub(v, cmulc(A(i * n + k), A(j * n + k)));
             A(i * n + j) = make_float2(v.x / d, v.y / d);
         }
+    }
+}
+
+// solve (C C^H) x = b for one column, b_i = b(i), x_i in X(i * ldx + col); C lower triangular n x n. b may read the
+// column being solved: b(i) is read before X(i * ldx + col) is written.
+template <typename BF>
+__device__ void chol_solve_col(const Scratch& C, int n, const BF& b, const Scratch& X, int ldx, int col) {
+    for (int i = 0; i < n; ++i) {
+        float2 v = b(i);
+        for (int k = 0; k < i; ++k) v = csub(v, cmul(C(i * n + k), X(k * ldx + col)));
+        float d = C(i * n + i).x;
+        X(i * ldx + col) = make_float2(v.x / d, v.y / d);
+    }
+    for (int i = n - 1; i >= 0; --i) {
+        float2 v = X(i * ldx + col);
+        for (int k = i + 1; k < n; ++k) { float2 c = C(k * n + i); c.y = -c.y; v = csub(v, cmul(c, X(k * ldx + col))); }
+        float d = C(i * n + i).x;
+        X(i * ldx + col) = make_float2(v.x / d, v.y / d);
     }
 }
 

@@ -25,6 +25,7 @@ namespace {
 
 using sb_dense::Scratch;
 using sb_dense::chol_lower;
+using sb_dense::chol_solve_col;
 using sb_dense::whiten;
 using sb_dense::OfdmEqParams;
 
@@ -721,23 +722,6 @@ __global__ void interp_lin_kernel(const T* __restrict__ h, const int* __restrict
 //   tx_lmmse_matrix  G = (H^H H + I)^-1 H^H via chol + cholesky_solve        (mimo/equalization.py:95-97)
 //   lmmse_epilogue   x_hat = G y / diag(G H), no_eff = Re(1 / diag(G H) - 1)  (mimo/equalization.py:217-231)
 // ---------------------------------------------------------------------------------------------------------------
-// solve (C C^H) x = b for one column, b_i = b(i), x_i in X(i * ldx + col); C lower triangular n x n
-template <typename BF>
-__device__ void chol_solve_col(const Scratch& C, int n, const BF& b, const Scratch& X, int ldx, int col) {
-    for (int i = 0; i < n; ++i) {
-        float2 v = b(i);
-        for (int k = 0; k < i; ++k) v = csub(v, cmul(C(i * n + k), X(k * ldx + col)));
-        float d = C(i * n + i).x;
-        X(i * ldx + col) = make_float2(v.x / d, v.y / d);
-    }
-    for (int i = n - 1; i >= 0; --i) {
-        float2 v = X(i * ldx + col);
-        for (int k = i + 1; k < n; ++k) { float2 c = C(k * n + i); c.y = -c.y; v = csub(v, cmul(c, X(k * ldx + col))); }
-        float d = C(i * n + i).x;
-        X(i * ldx + col) = make_float2(v.x / d, v.y / d);
-    }
-}
-
 // G = (H^H H + I)^-1 H^H (K x M) for H (M x K): A = H^H H + I = C C^H (K x K, A is overwritten by C), then
 // C C^H G = H^H column by column
 __device__ void tx_lmmse_matrix(const Scratch& H, const Scratch& A, const Scratch& G, int M, int K) {

@@ -6,6 +6,7 @@ from .demodulator import OFDMDemodulator
 from .channel_estimation import (BaseChannelEstimator, BaseChannelInterpolator, LSChannelEstimator,
                                  NearestNeighborInterpolator, LinearInterpolator)
 from .equalization import OFDMEqualizer, LMMSEEqualizer
+from .precoding import RZFPrecoder, PrecodedChannel, RZFPrecodedChannel, CBFPrecodedChannel, EyePrecodedChannel
 from .detection import (LinearDetector, MaximumLikelihoodDetector, MaximumLikelihoodDetectorWithPrior, KBestDetector,
                         EPDetector, MMSEPICDetector)
 from .frontend import FusedLSLinearDetector, fusable, frontend_tables
