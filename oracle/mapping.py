@@ -113,6 +113,34 @@ def demapper(y, no, points, method="app", prior=None, hard_out=False, math_mode=
     return llr
 
 
+def demapper_f64(y, no, points, method="app", prior=None):
+    """The reference's 2-D demapping formula in float64 (mapping.py:664-691, 915-967), plain NumPy / SciPy: exponents
+    -|y - c|^2 / max(no, float32 tiny) (+ sum_k log_sigmoid(+-prior_k)), then logsumexp ("app") or max ("maxlog") over
+    the points with label bit i = 1 minus the same over bit i = 0, each group relative to its own maximum. Inputs as
+    `demapper`, evaluated at their float32 / complex64 values; -> llr [..., S*m] float64."""
+    from scipy.special import logsumexp
+    y = np.asarray(y, np.complex64).astype(np.complex128)
+    pts = np.asarray(points, np.complex64).astype(np.complex128)
+    m = int(np.log2(len(pts)))
+    no = np.asarray(no, np.float32).astype(np.float64)
+    no = np.broadcast_to(no.reshape(no.shape + (1,) * (y.ndim - no.ndim)), y.shape)
+    tiny = float(np.finfo(np.float32).tiny)
+    e = -np.abs(y[..., None] - pts) ** 2 / np.maximum(no, tiny)[..., None]          # [..., S, 2^m]
+    lab = (np.arange(2 ** m)[:, None] >> np.arange(m - 1, -1, -1)) & 1               # [2^m, m] label bits, MSB first
+    if prior is not None:
+        p = np.broadcast_to(np.asarray(prior, np.float32).astype(np.float64), y.shape + (m,))
+        s = 2.0 * lab - 1.0                                                          # bit 1 -> +prior, 0 -> -prior
+        for k in range(m):
+            e = e - np.logaddexp(0.0, -s[:, k] * p[..., k, None])                    # log_sigmoid(s * prior_k)
+    e = e.reshape(-1, 2 ** m)
+    out = np.empty((e.shape[0], m))
+    for i in range(m):
+        g = e.reshape(-1, 2 ** i, 2, 2 ** (m - 1 - i))                               # [.., higher bits, bit i, lower]
+        red = (lambda a: logsumexp(a, axis=(1, 2))) if method == "app" else (lambda a: np.max(a, axis=(1, 2)))
+        out[:, i] = red(g[:, :, 1, :]) - red(g[:, :, 0, :])
+    return out.reshape(y.shape[:-1] + (y.shape[-1] * m,))
+
+
 def ebnodb2no(ebno_db, num_bits_per_symbol, coderate):             # utils/misc.py:233-251 (no resource grid)
     ebno = np.power(np.float32(10), np.float32(ebno_db) / np.float32(10))
     return np.float32(1) / (ebno * np.float32(coderate) * np.float32(num_bits_per_symbol) / np.float32(1.0))

@@ -113,9 +113,9 @@ void sbo_demap_qam(const float* y, const float* no, int64_t no_inner, const floa
                 } else {
                     float s0 = 0.f, s1 = 0.f;
                     for (int t = 0; t < L; ++t) { if (t & mask) s1 += wgt[t]; else s0 += wgt[t]; }   /* ascending t */
-                    if (s0 > 0.f && s1 > 0.f) {
+                    if (fminf(s0, s1) >= 0x1p-92f) {              /* demap_qam.cuh DEMAP_QAM_GROUP_MIN */
                         l = sb_logf(s1) - sb_logf(s0);
-                    } else {                                       /* a whole group underflowed: per-group maxima */
+                    } else {                                       /* a group's shared sum is tiny: per-group maxima */
                         mx0 = isfinite(mx0) ? mx0 : 0.f;
                         mx1 = isfinite(mx1) ? mx1 : 0.f;
                         s0 = 0.f; s1 = 0.f;

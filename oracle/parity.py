@@ -98,6 +98,32 @@ def ofdm_detection_case(cfg, rng, no_range, ev_shape=None, no_shape=None):
     return rg, sm, F.stream_management(assoc, spt), y, h, ev, no, pts
 
 
+# ---- demapper inputs --------------------------------------------------------------------------------------------------
+def demap_noisy(rng, points, num_sym, num_no=40, no_range=(1e-4, 3.0)):
+    """Noisy constellation points, one row per noise variance: (y [num_no, num_sym] complex64, no [num_no] float32)
+    with no on a geometric grid over no_range and the points drawn uniformly."""
+    no = np.geomspace(*no_range, num_no).astype(np.float32)
+    x = points[rng.integers(0, len(points), (num_no, num_sym))]
+    return (x + cnormal(rng, x.shape) * np.sqrt(no)[:, None]).astype(np.complex64), no
+
+
+def demap_window(rng, points, num_sym, num_no=48):
+    """Inputs whose float64 LLRs sweep through |LLR| = 60 ... 100, where the app demapper's exponents relative to a
+    dimension's largest one cross exp's underflow at -87.3: y uniform over the constellation's bounding box (one row
+    per noise variance), no on a fine geometric grid around the squared smallest spacing of the levels (of either
+    dimension) over 80. -> (y [num_no, num_sym] complex64, no [num_no] float32)."""
+    gaps = [np.diff(np.unique(part.astype(np.float64))) for part in (points.real, points.imag)]
+    gaps = np.concatenate([g[g > 1e-6] for g in gaps])
+    d = gaps.min() if len(gaps) else 1.0
+    no = (d * d * np.geomspace(1 / 200, 1 / 20, num_no)).astype(np.float32)
+    lo, hi = np.min(points.real), np.max(points.real)
+    lo_i, hi_i = np.min(points.imag), np.max(points.imag)
+    if hi_i - lo_i < 1e-6:                                                  # PAM: imaginary part around 0
+        lo_i, hi_i = -d, d
+    y = rng.uniform(lo, hi, (num_no, num_sym)) + 1j * rng.uniform(lo_i, hi_i, (num_no, num_sym))
+    return y.astype(np.complex64), no
+
+
 # ---- LDPC inputs and checks -------------------------------------------------------------------------------------------
 def bpsk_llr(c, ebno_db, rate, rng):
     """Channel LLRs (float32) of codewords c [B, n] sent as BPSK (bit 1 -> +1) over AWGN at Eb/N0 ebno_db [B] (dB) and

@@ -10,12 +10,18 @@
 #include "sb_math.h"
 #include "sb_math2.cuh"
 
-// Slow path of "app": the bit group that does NOT contain the dimension's largest exponent underflowed as a whole
-// relative to it (e_t - max < -87.3, |LLR| > ~85: high SNR), so the shared-maximum form would return log(0). That group is
-// summed relative to its OWN maximum, as the reference's per-group logsumexp does (mapping.py:915-918); the other group
-// keeps its shared sum `s_ok` (its maximum IS the dimension's maximum `mx`). Out of line and loop-rolled on purpose: it
-// must not bloat the callers' instruction stream. `lev` points at the 2^H levels of the dimension (global or kernel-
-// parameter memory); g = the underflowed group (value of bit u). Returns LLR = logsumexp(group 1) - logsumexp(group 0).
+// Least shared sum (relative to the dimension's maximum) of a bit group that the shared-maximum form keeps; below it the
+// group is summed relative to its own maximum (derivation in demap_qam_dim). oracle/mapping_ref.c uses the same value.
+constexpr float DEMAP_QAM_GROUP_MIN = 0x1p-92f;
+
+// Slow path of "app": the shared sum of the bit group that does NOT contain the dimension's largest exponent is below
+// DEMAP_QAM_GROUP_MIN (|LLR| > ~64: high SNR), so members of that group may have been flushed to 0 (e_t - max < -87.3)
+// while they are still comparable to the group's own maximum, or the whole group underflowed and the shared-maximum form
+// would return log(0). That group is summed relative to its OWN maximum, as the reference's per-group logsumexp does
+// (mapping.py:915-918); the other group keeps its shared sum `s_ok` (its maximum IS the dimension's maximum `mx`). Out of
+// line and loop-rolled on purpose: it must not bloat the callers' instruction stream. `lev` points at the 2^H levels of
+// the dimension (global or kernel-parameter memory); g = the small group (value of bit u). Returns LLR =
+// logsumexp(group 1) - logsumexp(group 0).
 static __device__ __noinline__ float demap_qam_group_fallback(float yd, float inv_n0, const float* lev, int H, int u, int g,
                                                              float s_ok, float mx) {
     const int L = 1 << H, sh = H - 1 - u;
@@ -27,11 +33,13 @@ static __device__ __noinline__ float demap_qam_group_fallback(float yd, float in
         m2 = fmaxf(m2, fminf(mg, e));
         mg = fmaxf(mg, e);
     }
-    mg = (mg > -INFINITY && mg < INFINITY) ? mg : 0.f;
+    const bool finite = mg > -INFINITY && mg < INFINITY;
+    mg = finite ? mg : 0.f;
     float sg = 1.f;
     // High SNR: every other member is below exp(-21) of the group's maximum. At most 15 such terms sum to < 2^-25, so the
-    // reference's fp32 sum (ascending t, the maximum contributes exp(0) == 1) rounds to exactly 1 and its log to 0.
-    if (!(__fsub_rn(m2, mg) < -21.f)) {
+    // reference's fp32 sum (ascending t, the maximum contributes exp(0) == 1) rounds to exactly 1 and its log to 0. Only
+    // for a finite maximum: a group whose exponents are all -inf (no = 0 far from every level) sums to 0, log -inf.
+    if (!(finite && __fsub_rn(m2, mg) < -21.f)) {
         sg = 0.f;
         for (int t = 0; t < L; ++t) {                               // ascending t inside the group
             if (((t >> sh) & 1) != g) continue;
@@ -41,7 +49,8 @@ static __device__ __noinline__ float demap_qam_group_fallback(float yd, float in
         }
     }
     const float lg = __fadd_rn(sg > 0.f ? sb_logf(sg) : -INFINITY, mg);
-    const float lo = __fadd_rn(sb_logf(s_ok), mx);
+    // s_ok == 0 only when every exponent of the dimension is -inf: then both groups are log(0) and the LLR is NaN
+    const float lo = __fadd_rn(s_ok > 0.f ? sb_logf(s_ok) : -INFINITY, mx);
     return g ? __fsub_rn(lg, lo) : __fsub_rn(lo, lg);
 }
 
@@ -60,7 +69,7 @@ __device__ __forceinline__ void demap_qam_dim(float yd, float inv_n0, const Lev&
     }
     // "app": exponentials relative to the LARGEST exponent of the dimension, evaluated once (L exps) and shared by the
     // H bits of the dimension: LLR = log(sum_{bit=1} w_t) - log(sum_{bit=0} w_t), the maximum cancels. The reference's
-    // per-group logsumexp is the same number up to rounding (fallback above for the underflow case).
+    // per-group logsumexp is the same number up to rounding as long as neither group's sum is tiny (fallback above).
     float wgt[L];
     float mx = -INFINITY;
     if (METHOD == 0 && H > 1) {
@@ -95,11 +104,18 @@ __device__ __forceinline__ void demap_qam_dim(float yd, float inv_n0, const Lev&
                 if ((t >> (H - 1 - u)) & 1) s1 = __fadd_rn(s1, wgt[t]);
                 else s0 = __fadd_rn(s0, wgt[t]);
             }
-            if (s0 > 0.f && s1 > 0.f) {
+            // The group holding mx sums to >= 1. The other one may have lost members flushed at e_t - mx < -87.3; they
+            // matter only if they are not negligible next to that group's own maximum e_g. With a shared sum
+            // s >= DEMAP_QAM_GROUP_MIN = 2^-92 and at most 2^(H-1) <= 16 members in it, exp(e_g - mx) >= 2^-96, i.e.
+            // e_g - mx >= -66.5, so every flushed member lies more than 20.7 below e_g, and the at most 15 of them add
+            // < 15 e^-20.7 < 2^-26 to the group's sum relative to its maximum: below fp32 rounding of the log.
+            // Smaller sums take the per-group path.
+            if (fminf(s0, s1) >= DEMAP_QAM_GROUP_MIN) {
                 const float2 lg = sb_logf2(make_float2(s0, s1));
                 l = __fsub_rn(lg.y, lg.x);
             } else {
-                l = demap_qam_group_fallback(yd, inv_n0, lev_mem, H, u, s1 > 0.f ? 0 : 1, s1 > 0.f ? s1 : s0, mx);
+                const bool ok1 = s1 >= DEMAP_QAM_GROUP_MIN;
+                l = demap_qam_group_fallback(yd, inv_n0, lev_mem, H, u, ok1 ? 0 : 1, ok1 ? s1 : s0, mx);
             }
         }
         out[u] = hard_out ? (l > 0.f ? 1.f : 0.f) : l;

@@ -21,6 +21,8 @@ Cases and the branches they pin:
                                   the float64 |LLR| exceeds the soft-output bound
   test_high_snr_app               the app demapper's underflow fallback (|LLR| > ~85), levels in kernel-parameter space;
                                   constellations whose real and imaginary levels differ tell the two dimensions apart
+  test_app_llr_window             |LLR| 60 ... 100 with equalised symbols spread over the constellation: bit groups
+                                  that keep some members above exp's underflow and lose others take the per-group path
   test_pusch_tables               CDM de-spreading folded into the tables; NT = 16 terms (double-symbol DMRS, one
                                   additional position, linear interpolation), with 4 layers the opt-in shared memory
   test_batch_slices               the batch-slice loop: more frames than ceil(8 SMs / (tiles * RX)), so a CTA walks
@@ -252,6 +254,30 @@ def test_high_snr_app(cuda_device, h, kind):
     print(f"{tag}: {big.mean():.1%} of the float64 |LLR| > 85")
     assert big.mean() > 0.05                                       # the fallback runs on these bits
     assert np.all(np.isfinite(soft))
+    assert not any(bad), "\n".join(x for x in bad if x)
+
+
+def test_app_llr_window(cuda_device):
+    """16-QAM app with the receiver told a noise variance 50 ... 500 times smaller than the actual one: the equalised
+    symbols spread over the whole constellation while |LLR| sweeps through 60 ... 100, where one member of a bit group
+    falls below exp's underflow relative to the dimension's largest exponent while the group's other member does not.
+    The shared-maximum form dropped that member (up to log 2 of LLR); demap_qam_dim sends such groups to the per-group
+    path. The oracle gets the same noise variance."""
+    from sionna_b200.phy.ofdm import LSChannelEstimator
+    k, h, ant, b = 2, 2, 4, 24
+    rng = np.random.default_rng(zlib.crc32(f"llr window {h}".encode()))
+    rg = _grid(k, 5, 60, [1])
+    const = _demapper_constellation(h)
+    det = _detector(LSChannelEstimator(rg, "lin"), rg, k, const, "app")
+    scale = _no_scale(h, ant, k)
+    y = _received(rng, rg, b, ant, const.points.numpy(), np.float32(10 * scale))
+    no = (scale * np.geomspace(0.02, 0.2, b)[:, None, None] * np.ones((1, 1, ant))).astype(np.float32)
+    soft, eq = _run(det, y, no, cuda_device)
+    tag = f"LLR window K={k} H={h} app"
+    bad, l64, _ = _compare(tag, rg, "lin", y, no, const, "app", soft, eq)
+    window = (np.abs(l64) > 60) & (np.abs(l64) < 100)
+    print(f"{tag}: {window.mean():.1%} of the float64 |LLR| in 60 ... 100")
+    assert window.mean() > 0.05
     assert not any(bad), "\n".join(x for x in bad if x)
 
 

@@ -1,12 +1,14 @@
 """Pin the mapping / demapping oracle against the reference's closed forms and test recipes:
 38.211 5.1 QAM formulas (test/unit/mapping/test_constellation.py:11-62), mapper index identity
 (test_mapping.py:37-45), demapper app / maxlog vs scipy.special.logsumexp / np.max with atol 1e-5
-(test_mapping.py:175-225), with priors (:398-478)."""
+(test_mapping.py:175-225), with priors (:398-478). The float64 reference `demapper_f64` against the same recipe, and the
+kernel-math mode held to the single-precision envelope against it."""
 import numpy as np
 import pytest
 from scipy.special import logsumexp
 
 from oracle import mapping as M
+from oracle import parity as P
 
 
 def _bpsk(b):
@@ -89,6 +91,43 @@ def test_demapper_vs_scipy(m, method, mode):
     prior = rng.normal(size=y.shape + (m,)).astype(np.float32)
     llr = M.demapper(y, no_scalar, pts, method, prior=prior, math_mode=mode)
     assert np.allclose(llr, _ref_llr(y, np.full(y.shape, no_scalar), pts, method, prior), atol=1e-4, rtol=1e-5)
+
+
+@pytest.mark.parametrize("prior_shape", [None, "bits", "full"])
+@pytest.mark.parametrize("method", ["app", "maxlog"])
+def test_demapper_f64_vs_scipy(method, prior_shape):
+    """The float64 reference equals the reference's test recipe (scipy logsumexp / max over the two index sets) on the
+    2-D formula, with per-symbol no, for 64-QAM and a 5-bit custom constellation."""
+    rng = np.random.default_rng(5)
+    for pts in (M.qam(6), (rng.normal(size=32) + 1j * rng.normal(size=32)).astype(np.complex64)):
+        m = int(np.log2(len(pts)))
+        y = (rng.normal(size=(3, 40)) + 1j * rng.normal(size=(3, 40))).astype(np.complex64)
+        no = rng.uniform(0.05, 1.0, y.shape).astype(np.float32)
+        prior = {None: None, "bits": rng.normal(size=m), "full": rng.normal(size=y.shape + (m,))}[prior_shape]
+        prior = None if prior is None else prior.astype(np.float32)
+        ref = _ref_llr(y, no, pts, method, None if prior is None else np.broadcast_to(prior, y.shape + (m,)))
+        np.testing.assert_allclose(M.demapper_f64(y, no, pts, method, prior), ref, rtol=1e-12, atol=1e-12)
+
+
+@pytest.mark.parametrize("inputs", ["noisy", "window"])
+@pytest.mark.parametrize("method", ["app", "maxlog"])
+@pytest.mark.parametrize("m", [2, 4, 6, 8, 10])
+def test_kernel_math_demapper_envelope(m, method, inputs):
+    """What the separable square-QAM kernel computes (the oracle's kernel-math mode, which the GPU kernel equals bit for
+    bit) stays within 2x (rms) / 3x (max) of the libm 2-D formula's error against the float64 reference, errors relative
+    to the rms of each row's reference LLRs. "noisy": constellation points plus noise at 40 noise variances from 1e-4 to 3;
+    "window": y uniform over the constellation, no swept so that |LLR| crosses 60 ... 100, where a bit group's members
+    fall below exp's underflow relative to the dimension's largest exponent while still comparable to the group's own."""
+    rng = np.random.default_rng(100 + m)
+    pts = M.qam(m)
+    y, no = (P.demap_noisy if inputs == "noisy" else P.demap_window)(rng, pts, 256)
+    no = no[:, None]
+    ref = M.demapper_f64(y, no, pts, method)
+    if inputs == "window":
+        assert np.mean((np.abs(ref) > 60) & (np.abs(ref) < 100)) > 0.05
+    bad = P.envelope(f"m={m} {method} {inputs}", M.demapper(y, no, pts, method, math_mode=1),
+                     M.demapper(y, no, pts, method, math_mode=0), ref, (2.0, 3.0))
+    assert not bad, bad
 
 
 def test_ebnodb2no_and_hard_decisions():
