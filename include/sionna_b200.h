@@ -200,6 +200,14 @@ int sb_demap(const float* d_y, const float* d_no, int64_t no_inner, const float*
 int sb_demap_qam(const float* d_y, const float* d_no, int64_t no_inner, const float* d_levels_re,
                  const float* d_levels_im, int32_t m, int32_t method, float* d_llr, int64_t n_sym, int32_t hard_out,
                  void* stream);
+/* SymbolDemapper.call (mapping.py:776-792): e_c = -|y - c|^2 / no + prior_c over the num_points points d_points
+ * (complex, any constellation, 2 <= num_points <= 1024). Symbol s uses d_no[s / no_inner] and, if d_prior is given,
+ * the prior logits d_prior[(s / prior_inner) * num_points ...]. d_out: log_softmax(e) [n_sym, num_points] (float), or
+ * with hard_out = 1 the index of the first maximum [n_sym] (int32). Malformed arguments return SB_EINVAL before any
+ * device access. */
+int sb_symbol_demap(const float* d_y, const float* d_no, int64_t no_inner, const float* d_points, int32_t num_points,
+                    const float* d_prior, int64_t prior_inner, void* d_out, int64_t n_sym, int32_t hard_out,
+                    void* stream);
 /* AWGN.call (channel/awgn.py:63-78, utils/misc.py:19-54): y = x + sqrt(no) * CN(0,1), complex64 [n];
  * element i uses d_no[i / no_inner]. */
 int sb_awgn(const float* d_x, const float* d_no, int64_t no_inner, float* d_y, int64_t n, uint64_t seed,
@@ -343,7 +351,11 @@ int sb_lmmse_equalize(const float* d_y, const float* d_h, const float* d_s, floa
  *   mode 1  whiten_channel(y, h, s)  mimo/utils.py:292-357        -> d_out0 = L^-1 y [num, M], d_out1 = L^-1 H [num, M, K]
  *   mode 2  lmmse_matrix(h, s)       mimo/equalization.py:11-99   -> d_out0 = G [num, K, M]; d_s == NULL: (H^H H + I)^-1 H^H
  *   mode 3  lmmse_equalizer(y, h, s, whiten_interference=False) :183-233 -> d_out0 = x_hat [num, K], d_out1 = no_eff (fp32)
- * 1 <= K <= M (mode 0: K = M). The per-matrix scratch 8 (M^2 + 2 M K) bytes must fit the device's opt-in shared memory per
+ *   mode 4  zf_equalizer(y, h, s)    mimo/equalization.py:235-343 -> d_out0 = x_hat [num, K], d_out1 = no_eff [num, K] (fp32)
+ *   mode 5  mf_equalizer(y, h, s)    mimo/equalization.py:345-466 -> d_out0 = x_hat [num, K], d_out1 = no_eff [num, K] (fp32)
+ *   mode 6  matrix_pinv(h)           utils/linalg.py              -> d_out0 = (H^H H)^-1 H^H [num, K, M]
+ * Modes 2 ... 6 read the lower triangle of S only. Modes 1, 3, 4, 5 need d_y, d_s and d_out1; malformed arguments return
+ * SB_EINVAL. 1 <= K <= M (mode 0: K = M). The per-matrix scratch 8 (M^2 + 2 M K) bytes must fit the device's opt-in shared memory per
  * block (227 KB on H100: inv_cholesky up to M = 98, M <= 155 for K = 16); below 32 matrices per CTA the kernel runs
  * with 16 ... 1 threads per CTA (correct, not tuned for speed); larger shapes return SB_EUNSUPPORTED. */
 int sb_mimo_linalg(int32_t mode, const float* d_y, const float* d_h, const float* d_s, float* d_out0, void* d_out1,
@@ -365,6 +377,20 @@ int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float* d_err_var
                   int32_t num_rx, int32_t num_rx_ant, int32_t num_tx_streams, int32_t num_symbols,
                   int32_t num_subcarriers, int32_t streams_per_rx, int32_t interferers_per_rx, int32_t num_data,
                   void* stream);
+/* LMMSEEqualizer (whitened or not), ZFEqualizer and MFEqualizer (ofdm/equalization.py:277-462, mimo/equalization.py:
+ * 101-466): sb_ofdm_lmmse's arguments, layouts and shared-memory limit with the equaliser chosen by `equalizer`:
+ * 0 LMMSE (sb_ofdm_lmmse), 1 LMMSE with whiten_interference=False, 2 ZF, 3 MF. Receivers without interfering streams
+ * and streams_per_rx <= 4 (equalizer 1: and num_rx_ant >= streams_per_rx + 2) run a register kernel (no limit on
+ * num_rx_ant); all other cases run the shared-memory kernel and its scratch limit.
+ * A bad equalizer, negative or zero sizes (batch may be 0) or, with batch > 0, a missing pointer return SB_EINVAL;
+ * streams_per_rx outside 1 ... min(16, num_rx_ant) and scratch beyond 200 KB return SB_EUNSUPPORTED with a message.
+ * All checks run before any device access. */
+int sb_ofdm_equalize(int32_t equalizer, const float* d_y, const float* d_h_hat, const float* d_err_var,
+                     const int64_t* h_ev_stride, const float* d_no, const int64_t* h_no_stride, const int32_t* d_desired,
+                     const int32_t* d_undesired, const int32_t* d_out_stream, const int32_t* d_data_pos, float* d_x_hat,
+                     float* d_no_eff, int64_t batch, int32_t num_rx, int32_t num_rx_ant, int32_t num_tx_streams,
+                     int32_t num_symbols, int32_t num_subcarriers, int32_t streams_per_rx, int32_t interferers_per_rx,
+                     int32_t num_data, void* stream);
 
 /* MaximumLikelihoodDetector.call (mimo/detection.py:473-537, whiten_channel mimo/utils.py:292-357, SymbolLogits2LLRs.call
  * mapping.py:927-967), complex64: d_y [num, M], d_h [num, M, K], d_s [num, M, M], optional d_prior [num, K, num_points]

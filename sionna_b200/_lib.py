@@ -44,6 +44,7 @@ SIGNATURES = {
     "sb_qam_map": (i32, [vp, vp, i32, vp, vp, i64, vp]),
     "sb_demap": (i32, [vp, vp, i64, vp, i32, i32, vp, i64, vp, i64, i32, vp]),
     "sb_demap_qam": (i32, [vp, vp, i64, vp, vp, i32, i32, vp, i64, i32, vp]),
+    "sb_symbol_demap": (i32, [vp, vp, i64, vp, i32, vp, i64, vp, i64, i32, vp]),
     "sb_awgn": (i32, [vp, vp, i64, vp, i64, u64, u64, vp]),
     "sb_count_errors": (i32, [vp, vp, i64, i32, vp, vp]),
     "sb_crc_encode": (i32, [vp, vp, i32, i32, vp, i64, vp]),
@@ -71,6 +72,7 @@ SIGNATURES = {
     "sb_mimo_linalg": (i32, [i32, vp, vp, vp, vp, vp, i64, i32, i32, vp]),
     "sb_ofdm_frontend": (i32, [vp] * 15 + [i64] + [i32] * 11 + [vp]),
     "sb_ofdm_lmmse": (i32, [vp] * 12 + [i64] + [i32] * 8 + [vp]),
+    "sb_ofdm_equalize": (i32, [i32] + [vp] * 12 + [i64] + [i32] * 8 + [vp]),
     "sb_mimo_ml": (i32, [vp] * 7 + [sz, i64] + [i32] * 6 + [vp]),
     "sb_ml_workspace_bytes": (sz, [i64, i32]),
     "sb_ofdm_ml": (i32, [vp] * 14 + [sz, i64] + [i32] * 12 + [vp]),
@@ -86,8 +88,17 @@ SIGNATURES = {
 }
 
 
+# status codes of include/sionna_b200.h that the host layer tells apart
+SB_EUNSUPPORTED = -4
+
+
 class SbError(RuntimeError):
     """Raised when a C-ABI call returns a non-zero status."""
+
+
+class SbUnsupportedError(SbError, ValueError):
+    """SB_EUNSUPPORTED: a shape or configuration beyond a kernel's documented limits (also a ValueError, the type the
+    reference raises for arguments it does not accept)."""
 
 
 def lib():
@@ -110,7 +121,8 @@ def lib():
 def check(status, what=""):
     if status != 0:
         msg = lib().sb_last_error().decode("utf-8", "replace")
-        raise SbError(f"{what} failed with status {status}: {msg}")
+        err = SbUnsupportedError if status == SB_EUNSUPPORTED else SbError
+        raise err(f"{what} failed with status {status}: {msg}")
 
 
 def ptr(t):

@@ -11,10 +11,14 @@
 //   sb_pusch_ls_combine   PUSCHLSChannelEstimator.estimate_at_pilot_locations   nr/pusch_channel_estimation.py:117-169
 //   sb_lmmse_equalize     lmmse_equalizer mimo/equalization.py:101-233 (+ whiten_channel mimo/utils.py:292-357,
 //                         lmmse_matrix :11-99)
+//   sb_mimo_linalg        inv_cholesky, whiten_channel, lmmse_matrix, lmmse_equalizer(whiten_interference=False),
+//                         zf_equalizer, mf_equalizer, matrix_pinv (mimo/equalization.py:11-466, utils/linalg.py)
 //   sb_ofdm_lmmse         OFDMEqualizer.call ofdm/equalization.py:109-275 with the LMMSE equaliser fused in: the
 //                         interference-plus-noise covariance S = H_u H_u^H + diag(no) + diag(sum err_var) is
 //                         assembled on chip per resource element and never written to HBM (the reference materialises a
 //                         [.., M, M] tensor, 2 KB per RE for M = 16).
+//   sb_ofdm_equalize      the same with the LMMSE (whitened or not), ZF or MF equaliser fused in (LMMSEEqualizer,
+//                         ZFEqualizer, MFEqualizer, ofdm/equalization.py:277-462)
 // All kernels are one pass over HBM; FFT twiddles come from sincospif (<= 1 ulp), parity bar 1e-5 (the reference's own
 // round-trip test tolerance, test/unit/ofdm/test_ofdm.py:85-96).
 #include "sb_common.h"
@@ -719,15 +723,18 @@ __global__ void interp_lin_kernel(const T* __restrict__ h, const int* __restrict
 // Dense per-vector linear algebra, complex64, one thread per received vector; matrices live in shared memory interleaved
 // by thread (Scratch, dense_mimo.cuh). The LMMSE kernels and the mimo_linalg modes are compositions of these steps:
 //   chol_lower, whiten                                                        (dense_mimo.cuh)
-//   tx_lmmse_matrix  G = (H^H H + I)^-1 H^H via chol + cholesky_solve        (mimo/equalization.py:95-97)
+//   tx_lmmse_matrix  G = (H^H H + r I)^-1 H^H via chol + cholesky_solve      (mimo/equalization.py:95-97; r = 0:
+//                    matrix_pinv, utils/linalg.py)
 //   lmmse_epilogue   x_hat = G y / diag(G H), no_eff = Re(1 / diag(G H) - 1)  (mimo/equalization.py:217-231)
+//   herm_quad        Re g S g^H of a row vector g from S's lower triangle      (diag(G S G^H), :335-342, :459-464)
 // ---------------------------------------------------------------------------------------------------------------
-// G = (H^H H + I)^-1 H^H (K x M) for H (M x K): A = H^H H + I = C C^H (K x K, A is overwritten by C), then
-// C C^H G = H^H column by column
-__device__ void tx_lmmse_matrix(const Scratch& H, const Scratch& A, const Scratch& G, int M, int K) {
+// G = (H^H H + ridge I)^-1 H^H (K x M) for H (M x K): A = H^H H + ridge I = C C^H (K x K, A is overwritten by C), then
+// C C^H G = H^H column by column. ridge 1: LMMSE (the diagonal starts at 1, as before the argument existed); 0: the
+// pseudo-inverse.
+__device__ void tx_lmmse_matrix(const Scratch& H, const Scratch& A, const Scratch& G, int M, int K, float ridge) {
     for (int a = 0; a < K; ++a)
         for (int b = 0; b <= a; ++b) {
-            float2 acc = make_float2(a == b ? 1.f : 0.f, 0.f);
+            float2 acc = make_float2(a == b ? ridge : 0.f, 0.f);
             for (int m = 0; m < M; ++m) acc = cadd(acc, cmulc(H(m * K + b), H(m * K + a)));   // conj(H[m,a]) * H[m,b]
             A(a * K + b) = acc;
         }
@@ -752,6 +759,60 @@ __device__ __forceinline__ void lmmse_epilogue(const GF& g, const YF& y, const S
     }
 }
 
+// Re(g S g^H) = sum_a S_aa |g_a|^2 + 2 Re sum_{a > b} g_a S_ab conj(g_b) for Hermitian S, of which only the lower
+// triangle s(a, b), a >= b, is read; g(a) = g_a, a < n
+template <typename SF, typename GF>
+__device__ __forceinline__ float herm_quad(const SF& s, const GF& g, int n) {
+    float diag = 0.f, off = 0.f;
+    for (int a = 0; a < n; ++a) {
+        const float2 ga = g(a);
+        diag += s(a, a).x * (ga.x * ga.x + ga.y * ga.y);
+        float2 t = make_float2(0.f, 0.f);
+        for (int b = 0; b < a; ++b) t = cadd(t, cmulc(s(a, b), g(b)));                // sum_b S_ab conj(g_b)
+        off += ga.x * t.x - ga.y * t.y;                                                   // Re(g_a t)
+    }
+    return diag + 2.f * off;
+}
+
+// ZF / MF per vector from H (M x K) in scratch, y(m) and the noise covariance's lower triangle s(a, b):
+//   ZF (mimo/equalization.py:316-342): G = matrix_pinv(H) = (H^H H)^-1 H^H in G (K x M, A = chol(H^H H) scratch),
+//      x_hat = G y, no_eff = Re diag(G S G^H)
+//   MF (:437-464): B = H^H H, x_hat_k = (H^H y)_k / B_kk and, with G = diag(B)^-1 H^H, whose (I - G H) row k is
+//      -B_kj / B_kk off the diagonal and 0 on it,  no_eff_k = (sum_{j != k} |B_kj|^2 + h_k^H S h_k) / B_kk^2
+template <typename YF, typename SF>
+__device__ void zf_core(const Scratch& H, const YF& y, const Scratch& A, const Scratch& G, const SF& s, int M, int K,
+                        float2* xh, float* ne) {
+    tx_lmmse_matrix(H, A, G, M, K, 0.f);
+    for (int k = 0; k < K; ++k) {
+        float2 gy = make_float2(0.f, 0.f);
+        for (int m = 0; m < M; ++m) gy = cadd(gy, cmul(G(k * M + m), y(m)));
+        xh[k] = gy;
+        ne[k] = herm_quad(s, [&](int m) { return G(k * M + m); }, M);
+    }
+}
+template <typename YF, typename SF>
+__device__ void mf_core(const Scratch& H, const YF& y, const SF& s, int M, int K, float2* xh, float* ne) {
+    for (int k = 0; k < K; ++k) {
+        float bkk = 0.f, off = 0.f;
+        float2 z = make_float2(0.f, 0.f);
+        for (int m = 0; m < M; ++m) {
+            const float2 h = H(m * K + k);
+            bkk += h.x * h.x + h.y * h.y;
+            z = cadd(z, cmulc(y(m), h));                                                  // conj(H_mk) y_m
+        }
+        for (int j = 0; j < K; ++j) {
+            if (j == k) continue;
+            float2 b = make_float2(0.f, 0.f);
+            for (int m = 0; m < M; ++m) b = cadd(b, cmulc(H(m * K + j), H(m * K + k)));   // B_kj
+            off += b.x * b.x + b.y * b.y;
+        }
+        const float q = herm_quad(s, [&](int m) { float2 h = H(m * K + k); h.y = -h.y; return h; }, M);
+        const float inv = 1.f / bkk;
+        xh[k] = cscale(z, inv);
+        ne[k] = fabsf((off + q) * inv * inv);
+    }
+}
+
 // LMMSE equalisation of one received vector with noise covariance S (mimo/equalization.py:101-233, whitening
 // mimo/utils.py:292-357). Per-thread scratch: S [M, M], H [M, K], y [M], A [K, K], G [K, M].
 struct LmmseScratch {
@@ -769,7 +830,7 @@ struct LmmseScratch {
 __device__ void lmmse_core(const LmmseScratch& w, int M, int K, float2* xh, float* ne) {
     chol_lower(w.S, M);
     whiten(w.S, w.Y, w.H, M, K);
-    tx_lmmse_matrix(w.H, w.A, w.G, M, K);
+    tx_lmmse_matrix(w.H, w.A, w.G, M, K, 1.f);
     lmmse_epilogue([&](int k, int m) { return w.G(k * M + m); }, w.Y, w.H, M, K, xh, ne);
 }
 
@@ -796,6 +857,9 @@ __global__ void lmmse_kernel(const float2* __restrict__ y, const float2* __restr
 //   mode 2  lmmse_matrix(h, s)         mimo/equalization.py:11-99    out0 = G = H^H (H H^H + S)^-1 [R, K, M]; s == nullptr:
 //                                                                    G = (H^H H + I)^-1 H^H
 //   mode 3  lmmse_equalizer(whiten_interference=False)  :183-233     out0 = x_hat [R, K], out1 = no_eff [R, K] (float)
+//   mode 4  zf_equalizer(y, h, s)      mimo/equalization.py:235-343  out0 = x_hat [R, K], out1 = no_eff [R, K] (float)
+//   mode 5  mf_equalizer(y, h, s)      mimo/equalization.py:345-466  out0 = x_hat [R, K], out1 = no_eff [R, K] (float)
+//   mode 6  matrix_pinv(h)             utils/linalg.py               out0 = (H^H H)^-1 H^H [R, K, M]
 __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const float2* __restrict__ h,
                                    const float2* __restrict__ s, float2* __restrict__ out0, void* __restrict__ out1v,
                                    long long R, int M, int K) {
@@ -826,6 +890,20 @@ __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const
             }
             continue;
         }
+        if (mode >= 4) {                                            // ZF, MF, pinv: K x K Gram matrix in A, G in X
+            const long long rs = r * M * M;
+            const auto sf = [&](int a, int b) { return s[rs + a * M + b]; };
+            const auto yf = [&](int m) { return y[r * M + m]; };
+            if (mode == 4) {
+                zf_core(H, yf, A, X, sf, M, K, out0 + r * K, reinterpret_cast<float*>(out1v) + r * K);
+            } else if (mode == 5) {
+                mf_core(H, yf, sf, M, K, out0 + r * K, reinterpret_cast<float*>(out1v) + r * K);
+            } else {
+                tx_lmmse_matrix(H, A, X, M, K, 0.f);
+                for (int e = 0; e < K * M; ++e) out0[r * K * M + e] = X(e);
+            }
+            continue;
+        }
         // modes 2, 3: G
         if (rx_side) {                                              // G^H = (H H^H + S)^-1 H, column by column
             for (int a = 0; a < M; ++a)
@@ -837,7 +915,7 @@ __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const
             chol_lower(A, M);
             for (int c = 0; c < K; ++c) chol_solve_col(A, M, [&](int i) { return H(i * K + c); }, X, K, c);   // X = G^H [M, K]
         } else {
-            tx_lmmse_matrix(H, A, X, M, K);                                // X = G [K, M]
+            tx_lmmse_matrix(H, A, X, M, K, 1.f);                           // X = G [K, M]
         }
         if (mode == 2) {
             for (int k = 0; k < K; ++k)
@@ -854,8 +932,37 @@ __global__ void mimo_linalg_kernel(int mode, const float2* __restrict__ y, const
     }
 }
 
-// OFDMEqualizer + LMMSE fused (inputs and tables: OfdmEqParams, dense_mimo.cuh) -> x_hat / no_eff [B, TXS, num_data]
-__global__ void ofdm_lmmse_kernel(const OfdmEqParams p) {
+// Equalisers of sb_ofdm_equalize
+enum { EQ_LMMSE = 0, EQ_LMMSE_NO_WHITEN = 1, EQ_ZF = 2, EQ_MF = 3 };
+
+// One resource element of ofdm_linear_kernel: S (lower triangle, ofdm_load_re), H, y in w -> xh[K], ne[K]
+template <int EQ>
+__device__ __forceinline__ void linear_core(const LmmseScratch& w, int M, int K, float2* xh, float* ne) {
+    const auto sf = [&](int a, int b) { return w.S(a * M + b); };
+    const auto yf = [&](int m) { return w.Y(m); };
+    if constexpr (EQ == EQ_LMMSE) {
+        lmmse_core(w, M, K, xh, ne);
+    } else if constexpr (EQ == EQ_LMMSE_NO_WHITEN) {              // as sb_mimo_linalg mode 3: (H H^H + S) G^H = H
+        for (int a = 0; a < M; ++a)
+            for (int b = 0; b <= a; ++b) {
+                float2 acc = w.S(a * M + b);
+                for (int k = 0; k < K; ++k) acc = cadd(acc, cmulc(w.H(a * K + k), w.H(b * K + k)));
+                w.S(a * M + b) = acc;
+            }
+        chol_lower(w.S, M);
+        for (int c = 0; c < K; ++c) chol_solve_col(w.S, M, [&](int i) { return w.H(i * K + c); }, w.G, K, c);
+        lmmse_epilogue([&](int k, int m) { float2 g = w.G(m * K + k); g.y = -g.y; return g; }, yf, w.H, M, K, xh, ne);
+    } else if constexpr (EQ == EQ_ZF) {
+        zf_core(w.H, yf, w.A, w.G, sf, M, K, xh, ne);
+    } else {
+        mf_core(w.H, yf, sf, M, K, xh, ne);
+    }
+}
+
+// OFDMEqualizer + a linear equaliser fused (inputs and tables: OfdmEqParams, dense_mimo.cuh) -> x_hat / no_eff
+// [B, TXS, num_data]
+template <int EQ>
+__global__ void ofdm_linear_kernel(const OfdmEqParams p) {
     extern __shared__ float2 smem[];
     const int T = blockDim.x, t = threadIdx.x, M = p.ANT, K = p.K;
     const LmmseScratch w(smem, T, t, M, K);
@@ -867,7 +974,7 @@ __global__ void ofdm_lmmse_kernel(const OfdmEqParams p) {
         // skip resource elements that carry data for none of this receiver's streams
         if (!sb_dense::ofdm_re_has_data(p, e)) continue;
         sb_dense::ofdm_load_re(p, e, w.Y, w.H, w.S);
-        lmmse_core(w, M, K, xo, no_e);
+        linear_core<EQ>(w, M, K, xo, no_e);
         for (int k = 0; k < K; ++k) {
             const long long o = sb_dense::ofdm_out_index(p, e, k);
             if (o >= 0) {
@@ -878,14 +985,22 @@ __global__ void ofdm_lmmse_kernel(const OfdmEqParams p) {
     }
 }
 
-// Fast path of ofdm_lmmse_kernel for receivers without interfering streams (KU == 0): S = diag(no + sum err_var) is
-// diagonal, whitening is a per-antenna scaling, and everything fits in registers. One thread per resource element
-// streams once over the antennas (reads coalesced over the subcarrier index) and accumulates
-//   B = H_w^H H_w (K x K Hermitian, lower triangle) and z = H_w^H y_w,          H_w = H / sqrt(d), y_w = y / sqrt(d)
-// then A = B + I = C C^H, A^-1 = C^-H C^-1 and, without forming G = A^-1 H_w^H (K x M),
-//   G y_w = A^-1 z,   diag(G H_w)_k = sum_j (A^-1)_kj B_jk          (same quantities as lmmse_core)
-template <int K>
-__global__ void __launch_bounds__(128, 4) ofdm_lmmse_diag_kernel(const OfdmEqParams p) {
+// Fast path of ofdm_linear_kernel for receivers without interfering streams (KU == 0): S = D = diag(no + sum err_var)
+// is diagonal and everything fits in registers. One thread per resource element streams once over the antennas (reads
+// coalesced over the subcarrier index) and accumulates
+//   LMMSE:   B = H_w^H H_w (K x K Hermitian, lower triangle) and z = H_w^H y_w,  H_w = H / sqrt(d), y_w = y / sqrt(d)
+//            then A = B + I = C C^H, A^-1 = C^-H C^-1 and, without forming G = A^-1 H_w^H (K x M),
+//            G y_w = A^-1 z,   diag(G H_w)_k = sum_j (A^-1)_kj B_jk          (same quantities as lmmse_core)
+//   ZF, MF:  B = H^H H, z = H^H y and C = H^H D H (ZF: lower triangle, MF: diagonal) of the unwhitened channel
+//            (lmmse_diag.cuh: zf_diag_solve, mf_diag_solve)
+// LMMSE without whitening runs the LMMSE instantiation when M >= K + 2: with a diagonal S both forms are the same
+// estimate. On (nearly) square systems the whitened register solve's single-precision error exceeds the unwhitened
+// evaluation's (10x at M = K = 3), so M <= K + 1 runs the shared-memory kernel, which keeps the unwhitened steps.
+// ZF holds the full C
+// besides B and the chunk's loads; it runs 3 CTAs per SM (2 at K = 4), which leaves it the registers to do so without
+// spilling.
+template <int EQ, int K>
+__global__ void __launch_bounds__(128, EQ == EQ_ZF ? (K == 4 ? 2 : 3) : 4) ofdm_linear_diag_kernel(const OfdmEqParams p) {
     const long long SF = (long long)p.S * p.F;
     const long long total = p.B * p.RX * SF;
     const int M = p.ANT;
@@ -908,6 +1023,10 @@ __global__ void __launch_bounds__(128, 4) ofdm_lmmse_diag_kernel(const OfdmEqPar
         for (int k = 0; k < K; ++k) des[k] = p.des[rx * K + k];
         float2 Bm[K * (K + 1) / 2], z[K];
         sb_lmmse::lmmse_diag_clear<K>(Bm, z);
+        constexpr int NC = EQ == EQ_ZF ? K * (K + 1) / 2 : K;
+        float2 Cm[NC];                                                              // C = H^H D H (ZF, MF)
+#pragma unroll
+        for (int e = 0; e < NC; ++e) Cm[e] = make_float2(0.f, 0.f);
         // antennas in chunks of 4: all loads of a chunk (y, K channel columns, the error variances, no) are issued before
         // any of them is used, so 4 * (K + 1) 8-byte loads per thread are in flight instead of one dependent load at a
         // time (the one-antenna-per-trip version was latency bound: long_scoreboard 3.4 warps per issue, 27 % of HBM peak).
@@ -923,17 +1042,31 @@ __global__ void __launch_bounds__(128, 4) ofdm_lmmse_diag_kernel(const OfdmEqPar
         const float* nop = p.no + b * p.no_stride[0] + rx * p.no_stride[1];
         const long long ev_m = p.ev_stride[2], ev_q = p.ev_stride[3], no_m = p.no_stride[2];
         auto accumulate = [&](float2 yv, const float2* hv, float d) {
-            // whitening by 1 / sqrt(d): one division per antenna, multiplications for the K + 1 scalings
-            const float w = rsqrtf(d);                                    // MUFU.RSQ, <= 2 ulp
-            const float2 yw = make_float2(yv.x * w, yv.y * w);
-            float2 hw[K];
+            if constexpr (EQ == EQ_LMMSE) {
+                // whitening by 1 / sqrt(d): one division per antenna, multiplications for the K + 1 scalings
+                const float w = rsqrtf(d);                                    // MUFU.RSQ, <= 2 ulp
+                const float2 yw = make_float2(yv.x * w, yv.y * w);
+                float2 hw[K];
 #pragma unroll
-            for (int k = 0; k < K; ++k) hw[k] = make_float2(hv[k].x * w, hv[k].y * w);
+                for (int k = 0; k < K; ++k) hw[k] = make_float2(hv[k].x * w, hv[k].y * w);
 #pragma unroll
-            for (int a = 0; a < K; ++a) {
-                z[a] = cadd(z[a], cmulc(yw, hw[a]));                       // conj(H_w[m, a]) * y_w[m]
+                for (int a = 0; a < K; ++a) {
+                    z[a] = cadd(z[a], cmulc(yw, hw[a]));                       // conj(H_w[m, a]) * y_w[m]
 #pragma unroll
-                for (int q = 0; q <= a; ++q) Bm[a * (a + 1) / 2 + q] = cadd(Bm[a * (a + 1) / 2 + q], cmulc(hw[q], hw[a]));
+                    for (int q = 0; q <= a; ++q) Bm[a * (a + 1) / 2 + q] = cadd(Bm[a * (a + 1) / 2 + q], cmulc(hw[q], hw[a]));
+                }
+            } else {
+#pragma unroll
+                for (int a = 0; a < K; ++a) {
+                    z[a] = cadd(z[a], cmulc(yv, hv[a]));                       // conj(H[m, a]) * y[m]
+#pragma unroll
+                    for (int q = 0; q <= a; ++q) {
+                        const float2 b = cmulc(hv[q], hv[a]);                  // conj(H[m, a]) * H[m, q]
+                        Bm[a * (a + 1) / 2 + q] = cadd(Bm[a * (a + 1) / 2 + q], b);
+                        if constexpr (EQ == EQ_ZF) Cm[a * (a + 1) / 2 + q] = cadd(Cm[a * (a + 1) / 2 + q], cscale(b, d));
+                        else if (q == a) Cm[a].x += d * b.x;
+                    }
+                }
             }
         };
         int m0 = 0;
@@ -968,7 +1101,9 @@ __global__ void __launch_bounds__(128, 4) ofdm_lmmse_diag_kernel(const OfdmEqPar
         }
         float2 xo[K];
         float no_e[K];
-        sb_lmmse::lmmse_diag_solve<K>(Bm, z, xo, no_e);
+        if constexpr (EQ == EQ_LMMSE) sb_lmmse::lmmse_diag_solve<K>(Bm, z, xo, no_e);
+        else if constexpr (EQ == EQ_ZF) sb_lmmse::zf_diag_solve<K>(Bm, Cm, z, xo, no_e);
+        else sb_lmmse::mf_diag_solve<K>(Bm, Cm, z, xo, no_e);
 #pragma unroll
         for (int k = 0; k < K; ++k) {
             if (dp[k] >= 0) {
@@ -1302,10 +1437,11 @@ extern "C" int sb_lmmse_equalize(const float* d_y, const float* d_h, const float
 extern "C" int sb_mimo_linalg(int32_t mode, const float* d_y, const float* d_h, const float* d_s, float* d_out0, void* d_out1,
                               int64_t num, int32_t M, int32_t K, void* stream) {
     if (num == 0) return SB_OK;
-    SB_CHECK_ARG(mode >= 0 && mode <= 3 && num > 0 && M >= 1 && d_out0, "sb_mimo_linalg: bad arguments");
+    SB_CHECK_ARG(mode >= 0 && mode <= 6 && num > 0 && M >= 1 && d_out0, "sb_mimo_linalg: bad arguments");
     SB_CHECK_ARG(mode == 0 ? (d_s != nullptr) : (d_h && K >= 1 && K <= M), "sb_mimo_linalg: missing input / need 1 <= K <= M");
     SB_CHECK_ARG(mode != 1 || (d_y && d_s && d_out1), "sb_mimo_linalg: whiten_channel needs y, h, s and two outputs");
-    SB_CHECK_ARG(mode != 3 || (d_y && d_s && d_out1), "sb_mimo_linalg: the equaliser needs y, h, s and two outputs");
+    SB_CHECK_ARG((mode != 3 && mode != 4 && mode != 5) || (d_y && d_s && d_out1),
+                 "sb_mimo_linalg: the equaliser needs y, h, s and two outputs");
     if (mode == 0) K = M;
     int dev = 0, optin = 0;
     SB_CUDA(cudaGetDevice(&dev));
@@ -1321,6 +1457,40 @@ extern "C" int sb_mimo_linalg(int32_t mode, const float* d_y, const float* d_h, 
     SB_CUDA(cudaFuncSetAttribute(mimo_linalg_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     mimo_linalg_kernel<<<sb_grid(num, threads, 16), threads, smem, (cudaStream_t)stream>>>(
         mode, (const float2*)d_y, (const float2*)d_h, (const float2*)d_s, (float2*)d_out0, d_out1, num, M, K);
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+// Launches the equaliser eq (EQ_*) over the OFDM problem p after the caller's argument checks (who names the caller in
+// the scratch-limit message)
+static int ofdm_linear(const char* who, int eq, const OfdmEqParams& p, long long total_re, cudaStream_t stream) {
+    const int M = p.ANT, K = p.K;
+    if (p.KU == 0 && K <= 4 && (eq != EQ_LMMSE_NO_WHITEN || M >= K + 2)) {   // diagonal S: register kernel
+        const int rc = sb_dispatch<1, 4>(K, [&](auto KC) {
+            const int grid = sb_grid(total_re, 128, 16);
+            if (eq == EQ_ZF) ofdm_linear_diag_kernel<EQ_ZF, KC><<<grid, 128, 0, stream>>>(p);
+            else if (eq == EQ_MF) ofdm_linear_diag_kernel<EQ_MF, KC><<<grid, 128, 0, stream>>>(p);
+            else ofdm_linear_diag_kernel<EQ_LMMSE, KC><<<grid, 128, 0, stream>>>(p);
+            return SB_OK;
+        });
+        if (rc) return rc;
+        SB_LAUNCH_CHECK();
+        return SB_OK;
+    }
+    size_t smem = 0;
+    const size_t per_thread = sizeof(float2) * LmmseScratch::elems(M, K);
+    int threads = scratch_threads(per_thread, kScratchSmemCap, &smem);
+    if (!threads) {
+        sb_set_error("%s: %d receive antennas, %d streams need %zu bytes of shared-memory scratch per resource "
+                     "element, the limit is %zu", who, M, K, per_thread, kScratchSmemCap);
+        return SB_EUNSUPPORTED;
+    }
+    const int rc = sb_dispatch<0, 3>(eq, [&](auto E) {
+        SB_CUDA(cudaFuncSetAttribute(ofdm_linear_kernel<E>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        ofdm_linear_kernel<E><<<sb_grid(total_re, threads, 16), threads, smem, stream>>>(p);
+        return SB_OK;
+    });
+    if (rc) return rc;
     SB_LAUNCH_CHECK();
     return SB_OK;
 }
@@ -1343,25 +1513,36 @@ extern "C" int sb_ofdm_lmmse(const float* d_y, const float* d_h_hat, const float
                                                             num_data);
     OfdmEqParams p = pb.ofdm;
     p.xh = (float2*)d_x_hat; p.ne = d_no_eff;
-    const long long total_re = pb.P;
-    if (interferers_per_rx == 0 && streams_per_rx <= 4) {     // diagonal noise covariance: register kernel
-        sb_dispatch<1, 4>(streams_per_rx, [&](auto K) {
-            ofdm_lmmse_diag_kernel<K><<<sb_grid(total_re, 128, 16), 128, 0, (cudaStream_t)stream>>>(p);
-            return SB_OK;
-        });
-        SB_LAUNCH_CHECK();
-        return SB_OK;
-    }
-    size_t smem = 0;
-    const size_t per_thread = sizeof(float2) * LmmseScratch::elems(num_rx_ant, streams_per_rx);
-    int threads = scratch_threads(per_thread, kScratchSmemCap, &smem);
-    if (!threads) {
-        sb_set_error("sb_ofdm_lmmse: %d receive antennas, %d streams need %zu bytes of shared-memory scratch per resource "
-                     "element, the limit is %zu", num_rx_ant, streams_per_rx, per_thread, kScratchSmemCap);
+    return ofdm_linear("sb_ofdm_lmmse", EQ_LMMSE, p, pb.P, (cudaStream_t)stream);
+}
+
+extern "C" int sb_ofdm_equalize(int32_t equalizer, const float* d_y, const float* d_h_hat, const float* d_err_var,
+                                const int64_t* h_ev_stride, const float* d_no, const int64_t* h_no_stride,
+                                const int32_t* d_desired, const int32_t* d_undesired, const int32_t* d_out_stream,
+                                const int32_t* d_data_pos, float* d_x_hat, float* d_no_eff, int64_t batch,
+                                int32_t num_rx, int32_t num_rx_ant, int32_t num_tx_streams, int32_t num_symbols,
+                                int32_t num_subcarriers, int32_t streams_per_rx, int32_t interferers_per_rx,
+                                int32_t num_data, void* stream) {
+    SB_CHECK_ARG(equalizer >= EQ_LMMSE && equalizer <= EQ_MF, "sb_ofdm_equalize: equalizer must be 0 (lmmse), "
+                 "1 (lmmse without whitening), 2 (zf) or 3 (mf)");
+    SB_CHECK_ARG(batch >= 0 && num_rx >= 1 && num_rx_ant >= 1 && num_tx_streams >= 1 && num_symbols >= 1 &&
+                     num_subcarriers >= 1 && interferers_per_rx >= 0 && num_data >= 0,
+                 "sb_ofdm_equalize: bad sizes");
+    if (streams_per_rx < 1 || streams_per_rx > 16 || streams_per_rx > num_rx_ant) {
+        sb_set_error("sb_ofdm_equalize: %d streams per receiver with %d receive antennas; supported are "
+                     "1 <= streams_per_rx <= min(16, num_rx_ant)", streams_per_rx, num_rx_ant);
         return SB_EUNSUPPORTED;
     }
-    SB_CUDA(cudaFuncSetAttribute(ofdm_lmmse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    ofdm_lmmse_kernel<<<sb_grid(total_re, threads, 16), threads, smem, (cudaStream_t)stream>>>(p);
-    SB_LAUNCH_CHECK();
-    return SB_OK;
+    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    SB_CHECK_ARG(d_y && d_h_hat && d_err_var && h_ev_stride && d_no && h_no_stride && d_desired && d_out_stream &&
+                     d_data_pos && d_x_hat && d_no_eff && (interferers_per_rx == 0 || d_undesired),
+                 "sb_ofdm_equalize: bad pointers");
+    const sb_dense::MimoProblem pb = sb_dense::ofdm_problem(d_y, d_h_hat, d_err_var, h_ev_stride, d_no, h_no_stride,
+                                                            d_desired, d_undesired, d_out_stream, d_data_pos, batch,
+                                                            num_rx, num_rx_ant, num_tx_streams, num_symbols,
+                                                            num_subcarriers, streams_per_rx, interferers_per_rx,
+                                                            num_data);
+    OfdmEqParams p = pb.ofdm;
+    p.xh = (float2*)d_x_hat; p.ne = d_no_eff;
+    return ofdm_linear("sb_ofdm_equalize", equalizer, p, pb.P, (cudaStream_t)stream);
 }

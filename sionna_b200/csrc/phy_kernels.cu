@@ -2,6 +2,7 @@
 //   sb_binary_source   BinarySource.call                 mapping.py:1350-1352
 //   sb_qam_map         Mapper.call                       mapping.py:497-519
 //   sb_demap           Demapper.call + SymbolLogits2LLRs mapping.py:664-691, 927-967
+//   sb_symbol_demap    SymbolDemapper.call               mapping.py:776-792
 //   sb_awgn            AWGN.call + complex_normal        channel/awgn.py:63-78, utils/misc.py:19-54
 //   sb_count_errors    count_errors / count_block_errors utils/metrics.py:94-144
 // (paths relative to /root/reference/src/sionna/phy). All are one pass over HBM with coalesced accesses and
@@ -135,6 +136,71 @@ __global__ void __launch_bounds__(128) demap_qam_kernel(const float2* __restrict
             demap_qam_symbol<METHOD, H>(yy, inv_n0, lr, li, lev_re, lev_im, hard_out, out);
         }
         store_llrs_warp<M>(s_out_q, out, base, n_sym, llr);
+    }
+}
+
+// ---------------------------------------------------------------------------------------------------------
+// SymbolDemapper: e_c = -|y - c|^2 / no + prior_c over the P points, out = log_softmax(e) [n_sym, P] (float) or the
+// first argmax [n_sym] (int32). G lanes (a power of two >= min(P, 32), at most a warp) serve one symbol, lane l the
+// points l, l + G, ...; a warp's 32 / G symbols are consecutive, so each store instruction of the warp writes 32
+// consecutive logits (4 P bytes out per 8 bytes in: the kernel is bound by its stores). The exponents are recomputed
+// in each of the three passes (max, sum of exp, store) from the points in shared memory. exp and log are sb_math.h's.
+// a / b for a >= 0, b >= 1 with a 32-bit division when both fit (a 64-bit one costs several times more instructions)
+__device__ __forceinline__ long long idx_div(long long a, long long b) {
+    return ((a | b) >> 32) == 0 ? (long long)((unsigned)a / (unsigned)b) : a / b;
+}
+
+template <int G>
+__global__ void __launch_bounds__(256) symbol_demap_kernel(const float2* __restrict__ y, const float* __restrict__ no,
+                                                           long long no_inner, const float2* __restrict__ points,
+                                                           int P, const float* __restrict__ prior,
+                                                           long long prior_inner, void* __restrict__ out,
+                                                           long long n_sym, int hard_out) {
+    extern __shared__ float2 s_pts[];
+    for (int i = threadIdx.x; i < P; i += blockDim.x) s_pts[i] = points[i];
+    __syncthreads();
+    constexpr int SPW = 32 / G;                                     // symbols per warp
+    const int lane = threadIdx.x & 31, g = lane % G;
+    const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+    const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+    for (long long w = warp; w * SPW < n_sym; w += nwarps) {       // warp-uniform trip count: shuffles see every lane
+        const long long s = w * SPW + lane / G;
+        const bool valid = s < n_sym;
+        const long long sv = valid ? s : n_sym - 1;
+        const float2 yy = y[sv];
+        const float inv_n0 = __frcp_rn(no[idx_div(sv, no_inner)]);   // one reciprocal per symbol, as demap_qam_kernel
+        const float* pr = prior ? prior + idx_div(sv, prior_inner) * P : nullptr;
+        auto expo = [&](int c) {
+            const float2 pt = s_pts[c];
+            const float dr = yy.x - pt.x, di = yy.y - pt.y;
+            float e = -((dr * dr + di * di) * inv_n0);
+            if (pr) e += pr[c];
+            return e;
+        };
+        float mx = -INFINITY;
+        int arg = P;                                                // P: this lane has no point
+        for (int c = g; c < P; c += G) {
+            const float e = expo(c);
+            if (e > mx || c == g) { mx = e; arg = c; }               // first maximum
+        }
+#pragma unroll
+        for (int o = G / 2; o > 0; o >>= 1) {                       // maximum over the group, ties to the lowest index
+            const float om = __shfl_xor_sync(0xffffffffu, mx, o);
+            const int oa = __shfl_xor_sync(0xffffffffu, arg, o);
+            if (om > mx || (om == mx && oa < arg)) { mx = om; arg = oa; }
+        }
+        if (hard_out) {
+            if (valid && g == 0) reinterpret_cast<int*>(out)[s] = arg;
+            continue;
+        }
+        float sum = 0.f;
+        for (int c = g; c < P; c += G) sum += sb_expf(expo(c) - mx);          // sum >= 1: the maximum's term
+#pragma unroll
+        for (int o = G / 2; o > 0; o >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, o);
+        const float lse = sb_logf(sum);
+        float* o_row = reinterpret_cast<float*>(out) + s * P;
+        if (valid)
+            for (int c = g; c < P; c += G) o_row[c] = (expo(c) - mx) - lse;   // tf.nn.log_softmax: shifted - log sum
     }
 }
 
@@ -298,6 +364,31 @@ extern "C" int sb_demap(const float* d_y, const float* d_no, int64_t no_inner, c
             return SB_OK;
         });
     });
+    SB_LAUNCH_CHECK();
+    return SB_OK;
+}
+
+extern "C" int sb_symbol_demap(const float* d_y, const float* d_no, int64_t no_inner, const float* d_points,
+                               int32_t num_points, const float* d_prior, int64_t prior_inner, void* d_out, int64_t n_sym,
+                               int32_t hard_out, void* stream) {
+    SB_CHECK_ARG(num_points >= 2 && num_points <= 1024, "sb_symbol_demap: num_points = %d, supported are 2 ... 1024",
+                 num_points);
+    SB_CHECK_ARG(n_sym >= 0 && no_inner >= 1 && (!d_prior || prior_inner >= 1) && (hard_out == 0 || hard_out == 1),
+                 "sb_symbol_demap: bad arguments");
+    if (n_sym == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    SB_CHECK_ARG(d_y && d_no && d_points && d_out, "sb_symbol_demap: missing input or output");
+    int lanes = 1;
+    while (lanes < num_points && lanes < 32) lanes *= 2;
+    const long long warps = (n_sym + 32 / lanes - 1) / (32 / lanes);
+    const int grid = sb_grid(warps, 8, 8);
+    const size_t smem = sizeof(float2) * num_points;
+    const int rc = sb_dispatch<1, 5>(__builtin_ctz(lanes), [&](auto L) {
+        symbol_demap_kernel<(1 << L)><<<grid, 256, smem, (cudaStream_t)stream>>>(
+            (const float2*)d_y, d_no, no_inner, (const float2*)d_points, num_points, d_prior, prior_inner, d_out, n_sym,
+            hard_out);
+        return SB_OK;
+    });
+    if (rc) return rc;
     SB_LAUNCH_CHECK();
     return SB_OK;
 }

@@ -2,8 +2,8 @@
 
 Host side: ``pam_gray`` / ``qam`` / ``pam`` (mapping.py:15-193) and ``Constellation`` (:195-469) build the point
 tables with NumPy exactly as the reference does (38.211 5.1 Gray labelling, closed-form unit-energy
-normalisation). Device side: ``Mapper`` -> ``sb_qam_map``, ``Demapper`` -> ``sb_demap``, ``BinarySource`` ->
-``sb_binary_source`` (``csrc/phy_kernels.cu``).
+normalisation). Device side: ``Mapper`` -> ``sb_qam_map``, ``Demapper`` -> ``sb_demap``, ``SymbolDemapper`` ->
+``sb_symbol_demap``, ``BinarySource`` -> ``sb_binary_source`` (``csrc/phy_kernels.cu``).
 """
 import numpy as np
 import torch
@@ -309,6 +309,51 @@ class Demapper(Block):
         val = None if lev is None else (torch.from_numpy(lev[0]).to(pts.device), torch.from_numpy(lev[1]).to(pts.device))
         self._sep_key, self._sep_val = key, val
         return val
+
+
+class SymbolDemapper(Block):
+    """SymbolDemapper(constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None)
+
+    Normalised log-probabilities (logits) or hard decisions on the constellation points for received symbols
+    (mapping.py:693-792): ``e_c = -|y - c|^2 / no + prior_c`` and ``log_softmax(e)`` over the points, or the index of
+    the first maximum of ``e`` (``hard_out``). ``call(y [..., n], no, prior=None)``: ``no`` a scalar or broadcastable
+    to ``y``, ``prior`` logits ``[num_points]`` or broadcastable to ``[..., n, num_points]`` -> ``[..., n, num_points]``
+    float or ``[..., n]`` int32. Kernel: ``sb_symbol_demap``."""
+
+    def __init__(self, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False,
+                 precision=None, **kwargs):
+        super().__init__(precision=precision, **kwargs)
+        self._hard_out = hard_out
+        self._constellation = Constellation.check_or_create(constellation_type=constellation_type,
+                                                            num_bits_per_symbol=num_bits_per_symbol,
+                                                            constellation=constellation, precision=precision)
+
+    @property
+    def constellation(self):
+        return self._constellation
+
+    def call(self, y, no, prior=None):
+        _need_single(self, "sb_symbol_demap")
+        dev = self.device
+        npts = self._constellation.num_points
+        y = y.to(device=dev, dtype=torch.complex64).contiguous()
+        n_sym = y.numel()
+        no_t, no_inner = _broadcast_inner(no, y.shape, dev, torch.float32)
+        pr_t, pr_inner = None, 1
+        if prior is not None:
+            p = torch.as_tensor(prior).to(device=dev, dtype=torch.float32)
+            if p.dim() == 1:
+                pr_t, pr_inner = p.expand(npts).contiguous(), max(n_sym, 1)
+            else:
+                pr_t = p.expand(list(y.shape) + [npts]).contiguous().reshape(-1)
+        if self._hard_out:
+            out = torch.empty(list(y.shape), dtype=torch.int32, device=dev)
+        else:
+            out = torch.empty(list(y.shape) + [npts], dtype=torch.float32, device=dev)
+        pts = self._constellation().to(torch.complex64)
+        check(lib().sb_symbol_demap(ptr(y), ptr(no_t), no_inner, ptr(pts), npts, ptr(pr_t), pr_inner, ptr(out), n_sym,
+                                    int(bool(self._hard_out)), current_stream()), "sb_symbol_demap")
+        return out
 
 
 class BinarySource(Block):

@@ -7,15 +7,17 @@ import torch
 
 from ..._lib import lib, check, ptr, current_stream
 from ..block import Block
-from ..mapping import Constellation, Demapper, pam
-from .equalization import lmmse_equalizer
+from ..mapping import Constellation, Demapper, SymbolDemapper, pam
+from .equalization import lmmse_equalizer, zf_equalizer, mf_equalizer
 
 
 class LinearDetector(Block):
     """LinearDetector(equalizer, output, demapping_method, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None)
 
-    Equaliser followed by a demapper (detection.py:87-143): ``call(y, h, s)`` -> LLRs ``[..., K, num_bits_per_symbol]``
-    (``output="bit"``). ``equalizer`` is ``"lmmse"`` or a callable ``(y, h, s) -> (x_hat, no_eff)``."""
+    Equaliser followed by a demapper (detection.py:87-143): ``call(y, h, s)`` -> LLRs / hard bits
+    ``[..., K, num_bits_per_symbol]`` (``output="bit"``, ``Demapper``) or logits ``[..., K, num_points]`` / int32
+    indices ``[..., K]`` (``output="symbol"``, ``SymbolDemapper``). ``equalizer`` is ``"lmmse"``, ``"zf"``, ``"mf"``
+    or a callable ``(y, h, s) -> (x_hat, no_eff)``."""
 
     def __init__(self, equalizer, output, demapping_method, constellation_type=None, num_bits_per_symbol=None,
                  constellation=None, hard_out=False, precision=None, **kwargs):
@@ -25,24 +27,24 @@ class LinearDetector(Block):
         # same argument checks and error types as the reference (detection.py:103-115)
         if isinstance(equalizer, str):
             assert equalizer in ["lmmse", "zf", "mf"], "Unknown equalizer."
-            if equalizer != "lmmse":
-                raise NotImplementedError(f"equalizer='{equalizer}': only the LMMSE equaliser has a kernel here "
-                                          "(pass a callable (y, h, s) -> (x_hat, no_eff) for anything else).")
-            equalizer = lmmse_equalizer
+            equalizer = {"lmmse": lmmse_equalizer, "zf": zf_equalizer, "mf": mf_equalizer}[equalizer]
         self._equalizer = equalizer
         assert output in ("bit", "symbol"), "Unknown output"
         assert demapping_method in ("app", "maxlog"), "Unknown demapping method"
-        if output != "bit":
-            raise NotImplementedError("output='symbol' (SymbolDemapper) is not provided; use output='bit'.")
         self._constellation = Constellation.check_or_create(constellation_type=constellation_type,
                                                             num_bits_per_symbol=num_bits_per_symbol,
                                                             constellation=constellation, precision=precision)
-        self._demapper = Demapper(demapping_method, constellation=self._constellation, hard_out=hard_out,
-                                  precision=precision)
+        if output == "bit":
+            self._demapper = Demapper(demapping_method, constellation=self._constellation, hard_out=hard_out,
+                                      precision=precision)
+        else:
+            self._demapper = SymbolDemapper(constellation=self._constellation, hard_out=hard_out, precision=precision)
 
     def call(self, y, h, s):
         x_hat, no_eff = self._equalizer(y, h, s)
         z = self._demapper(x_hat, no_eff)
+        if self._output == "symbol":
+            return z
         m = self._constellation.num_bits_per_symbol
         return z.reshape(list(x_hat.shape) + [m])
 

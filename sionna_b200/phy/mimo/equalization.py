@@ -1,4 +1,4 @@
-"""MIMO equalisation (mirror of /root/reference/src/sionna/phy/mimo/equalization.py:101-233)."""
+"""MIMO equalisation (mirror of /root/reference/src/sionna/phy/mimo/equalization.py:11-466): LMMSE, ZF and MF."""
 import torch
 
 from ..config import config
@@ -60,3 +60,40 @@ def lmmse_matrix(h, s=None, precision=None):
           "sb_mimo_linalg")
     return g
 
+
+
+def _dense_equalizer(name, mode, y, h, s, precision):
+    """x_hat [..., K], no_eff [..., K] of sb_mimo_linalg mode 4 (ZF) or 5 (MF) with the broadcasting of
+    ``lmmse_equalizer``."""
+    from ..block import fallback_to_single
+    if fallback_to_single(name, precision):
+        x_hat, no_eff = _dense_equalizer(name, mode, y, h, s, "single")
+        return x_hat.to(torch.complex128), no_eff.to(torch.float64)
+    dev = config.device
+    y, h, s = _c64(y, dev), _c64(h, dev), _c64(s, dev)
+    m, k = h.shape[-2], h.shape[-1]
+    lead = torch.broadcast_shapes(y.shape[:-1], h.shape[:-2], s.shape[:-2])
+    y = y.expand(*lead, m).contiguous()
+    h = h.expand(*lead, m, k).contiguous()
+    s = s.expand(*lead, m, m).contiguous()
+    x_hat = torch.empty(*lead, k, dtype=torch.complex64, device=dev)
+    no_eff = torch.empty(*lead, k, dtype=torch.float32, device=dev)
+    check(lib().sb_mimo_linalg(mode, ptr(y), ptr(h), ptr(s), ptr(x_hat), ptr(no_eff), y.numel() // m, m, k,
+                               current_stream()), "sb_mimo_linalg")
+    return x_hat, no_eff
+
+
+def zf_equalizer(y, h, s, precision=None):
+    r"""ZF equaliser for ``y = H x + n`` with ``E[n n^H] = S`` (equalization.py:235-343): ``x_hat = G y`` with
+    ``G = matrix_pinv(H) = (H^H H)^-1 H^H`` and ``no_eff = Re diag(G S G^H)``; ``sb_mimo_linalg`` mode 4.
+
+    y [..., M], h [..., M, K], s [..., M, M] -> x_hat [..., K] complex, no_eff [..., K] real."""
+    return _dense_equalizer("zf_equalizer", 4, y, h, s, precision)
+
+
+def mf_equalizer(y, h, s, precision=None):
+    r"""Matched-filter equaliser (equalization.py:345-466): ``x_hat = G y`` with ``G = diag(H^H H)^-1 H^H`` and
+    ``no_eff = |diag((I - G H)(I - G H)^H + G S G^H)|``; ``sb_mimo_linalg`` mode 5.
+
+    y [..., M], h [..., M, K], s [..., M, M] -> x_hat [..., K] complex, no_eff [..., K] real."""
+    return _dense_equalizer("mf_equalizer", 5, y, h, s, precision)

@@ -5,7 +5,7 @@ from .modulator import OFDMModulator
 from .demodulator import OFDMDemodulator
 from .channel_estimation import (BaseChannelEstimator, BaseChannelInterpolator, LSChannelEstimator,
                                  NearestNeighborInterpolator, LinearInterpolator)
-from .equalization import OFDMEqualizer, LMMSEEqualizer
+from .equalization import OFDMEqualizer, LMMSEEqualizer, ZFEqualizer, MFEqualizer
 from .precoding import RZFPrecoder, PrecodedChannel, RZFPrecodedChannel, CBFPrecodedChannel, EyePrecodedChannel
 from .detection import (LinearDetector, MaximumLikelihoodDetector, MaximumLikelihoodDetectorWithPrior, KBestDetector,
                         EPDetector, MMSEPICDetector)

@@ -1,5 +1,6 @@
 """OFDM MIMO detection (mirror of /root/reference/src/sionna/phy/ofdm/detection.py:20-1173): ``LinearDetector``
-= fused LMMSE equalisation (``sb_ofdm_lmmse``) + demapping with the per-symbol effective noise variance (``sb_demap``);
+= fused LMMSE / ZF / MF equalisation (``sb_ofdm_lmmse``, ``sb_ofdm_equalize``) + demapping with the per-symbol
+effective noise variance (``sb_demap``, or ``sb_symbol_demap`` for symbol outputs);
 ``MaximumLikelihoodDetector`` / ``MaximumLikelihoodDetectorWithPrior`` = fused covariance assembly + ML detection
 (``sb_ofdm_ml``); ``KBestDetector``, ``EPDetector`` and ``MMSEPICDetector`` = the same assembly + K-Best, EP or
 MMSE-PIC detection (``sb_ofdm_kbest``, ``sb_ofdm_ep``, ``sb_ofdm_mmse_pic``)."""
@@ -7,18 +8,22 @@ import torch
 
 from ..._lib import lib, check, ptr, current_stream
 from ..block import Block
-from ..mapping import Constellation, Demapper
+from ..mapping import Constellation, Demapper, SymbolDemapper
 from ..mimo.detection import (llrs_to_symbol_logits, ml_check_limits, detector_workspace, detector_out,
                               KBestDetector as _MimoKBest, EPDetector as _MimoEP, MMSEPICDetector as _MimoPIC,
                               iterative_check_limits, EP_MAX_POINTS, PIC_MAX_POINTS)
-from .equalization import LMMSEEqualizer, OFDMEqualizer
+from .equalization import LMMSEEqualizer, ZFEqualizer, MFEqualizer, OFDMEqualizer
 
 
 class LinearDetector(Block):
     """LinearDetector(equalizer, output, demapping_method, resource_grid, stream_management, constellation_type=None, num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None)
 
-    ``call(y, h_hat, err_var, no)`` -> LLRs ``[batch, num_tx, num_streams, num_data_symbols*num_bits_per_symbol]``
-    (``output="bit"``); ``equalizer="lmmse"`` (detection.py:740-847; PUSCH default ``("lmmse","bit","maxlog")``)."""
+    OFDM equaliser followed by a demapper (detection.py:740-847; PUSCH default ``("lmmse","bit","maxlog")``):
+    ``equalizer`` ``"lmmse"`` / ``"zf"`` / ``"mf"`` runs the fused ``LMMSEEqualizer`` / ``ZFEqualizer`` /
+    ``MFEqualizer``, a callable ``(y, h, s) -> (x_hat, no_eff)`` runs through ``OFDMEqualizer``'s unfused route.
+    ``call(y, h_hat, err_var, no)`` -> LLRs / hard bits ``[batch, num_tx, num_streams,
+    num_data_symbols*num_bits_per_symbol]`` (``output="bit"``), logits ``[batch, num_tx, num_streams, num_data_symbols,
+    num_points]`` or int32 indices ``[batch, num_tx, num_streams, num_data_symbols]`` (``output="symbol"``)."""
 
     def __init__(self, equalizer, output, demapping_method, resource_grid, stream_management, constellation_type=None,
                  num_bits_per_symbol=None, constellation=None, hard_out=False, precision=None, **kwargs):
@@ -27,16 +32,22 @@ class LinearDetector(Block):
         assert not isinstance(equalizer, str) or equalizer in ["lmmse", "zf", "mf"], "Unknown equalizer."
         assert output in ("bit", "symbol"), "Unknown output"
         assert demapping_method in ("app", "maxlog"), "Unknown demapping method"
-        if equalizer != "lmmse":
-            raise NotImplementedError(f"equalizer={equalizer!r}: only 'lmmse' has a fused OFDM kernel here.")
-        if output != "bit":
-            raise NotImplementedError("output='symbol' (SymbolDemapper) is not provided; use output='bit'.")
         self._constellation = Constellation.check_or_create(constellation_type=constellation_type,
                                                             num_bits_per_symbol=num_bits_per_symbol,
                                                             constellation=constellation, precision=precision)
-        self._equalizer = LMMSEEqualizer(resource_grid, stream_management, precision=precision)
-        self._demapper = Demapper(demapping_method, constellation=self._constellation, hard_out=hard_out,
-                                  precision=precision)
+        if equalizer == "lmmse":
+            self._equalizer = LMMSEEqualizer(resource_grid, stream_management, precision=precision)
+        elif equalizer == "zf":
+            self._equalizer = ZFEqualizer(resource_grid, stream_management, precision=precision)
+        elif equalizer == "mf":
+            self._equalizer = MFEqualizer(resource_grid, stream_management, precision=precision)
+        else:
+            self._equalizer = OFDMEqualizer(equalizer, resource_grid, stream_management, precision=precision)
+        if output == "bit":
+            self._demapper = Demapper(demapping_method, constellation=self._constellation, hard_out=hard_out,
+                                      precision=precision)
+        else:
+            self._demapper = SymbolDemapper(constellation=self._constellation, hard_out=hard_out, precision=precision)
 
     def call(self, y, h_hat, err_var, no):
         x_hat, no_eff = self._equalizer(y, h_hat, err_var, no)

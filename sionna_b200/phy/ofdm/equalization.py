@@ -1,6 +1,7 @@
-"""OFDM MIMO equalisation (mirror of /root/reference/src/sionna/phy/ofdm/equalization.py:17-344).
+"""OFDM MIMO equalisation (mirror of /root/reference/src/sionna/phy/ofdm/equalization.py:17-462).
 
-``LMMSEEqualizer`` runs ``sb_ofdm_lmmse``: per resource element the receive vector, the desired / interfering channel
+``LMMSEEqualizer`` runs ``sb_ofdm_lmmse`` (``whiten_interference=False``: ``sb_ofdm_equalize``), ``ZFEqualizer`` and
+``MFEqualizer`` run ``sb_ofdm_equalize``: per resource element the receive vector, the desired / interfering channel
 columns (``StreamManagement``), the noise and the channel-estimation error variances are read once, the covariance
 ``S = H_u H_u^H + diag(no) + diag(sum err_var)`` is assembled on chip, the LMMSE equaliser is applied and the soft symbols
 of the data-carrying REs are written directly in the ``[batch, num_tx, num_streams, num_data_symbols]`` output layout. A
@@ -38,14 +39,19 @@ def _strides_for(t, full_shape):
     return t, [0 if s == 1 and f != 1 else int(v) for s, f, v in zip(shp, full_shape, st)]
 
 
+# equalisers with a fused kernel: name -> sb_ofdm_equalize's equaliser code ("lmmse" runs sb_ofdm_lmmse)
+FUSED_EQUALIZERS = {"lmmse": 0, "lmmse-no-whitening": 1, "zf": 2, "mf": 3}
+
+
 class OFDMEqualizer(Block):
     """OFDMEqualizer(equalizer, resource_grid, stream_management): wraps a MIMO equaliser ``(y, h, s) -> (x_hat, no_eff)``
     for OFDM (equalization.py:17-275). ``call(y, h_hat, err_var, no)`` returns ``x_hat`` / ``no_eff``
-    ``[batch, num_tx, num_streams, num_data_symbols]``."""
+    ``[batch, num_tx, num_streams, num_data_symbols]``. A callable runs on the unfused route (explicit S tensor); a name
+    of ``FUSED_EQUALIZERS`` runs its fused kernel."""
 
     def __init__(self, equalizer, resource_grid, stream_management, precision=None, **kwargs):
         super().__init__(precision=precision, **kwargs)
-        assert callable(equalizer) or equalizer == "lmmse"
+        assert callable(equalizer) or equalizer in FUSED_EQUALIZERS
         assert isinstance(resource_grid, ResourceGrid)
         self._equalizer = equalizer
         self._resource_grid = resource_grid
@@ -62,14 +68,18 @@ class OFDMEqualizer(Block):
     def call(self, y, h_hat, err_var, no):
         if self.precision != "single":
             raise NotImplementedError("OFDM equalisation runs complex64 kernels only.")
-        if self._equalizer != "lmmse":
+        if callable(self._equalizer):
             return self._unfused(*self._kernel_inputs(y, h_hat, err_var, no))
         sm = self._stream_management
         ptrs, sizes, _alive, nd = self._cabi_args(y, h_hat, err_var, no)
         shp = (sizes[0], sm.num_tx, sm.num_streams_per_tx, nd)
         x_hat = torch.zeros(shp, dtype=torch.complex64, device=self.device)
         no_eff = torch.zeros(shp, dtype=torch.float32, device=self.device)
-        check(lib().sb_ofdm_lmmse(*ptrs, ptr(x_hat), ptr(no_eff), *sizes, current_stream()), "sb_ofdm_lmmse")
+        if self._equalizer == "lmmse":
+            check(lib().sb_ofdm_lmmse(*ptrs, ptr(x_hat), ptr(no_eff), *sizes, current_stream()), "sb_ofdm_lmmse")
+            return x_hat, no_eff
+        check(lib().sb_ofdm_equalize(FUSED_EQUALIZERS[self._equalizer], *ptrs, ptr(x_hat), ptr(no_eff), *sizes,
+                                     current_stream()), "sb_ofdm_equalize")
         return x_hat, no_eff
 
     def _cabi_args(self, y, h_hat, err_var, no):
@@ -146,9 +156,25 @@ class OFDMEqualizer(Block):
 
 class LMMSEEqualizer(OFDMEqualizer):
     """LMMSEEqualizer(resource_grid, stream_management, whiten_interference=True): LMMSE equalisation for OFDM MIMO
-    (equalization.py:277-344); fused kernel ``sb_ofdm_lmmse``."""
+    (equalization.py:277-344); fused kernel ``sb_ofdm_lmmse``, or ``sb_ofdm_equalize`` with
+    ``whiten_interference=False`` (``G = H^H (H H^H + S)^-1`` without whitening first)."""
 
     def __init__(self, resource_grid, stream_management, whiten_interference=True, precision=None, **kwargs):
-        if not whiten_interference:
-            raise NotImplementedError("LMMSEEqualizer: only whiten_interference=True is provided.")
-        super().__init__("lmmse", resource_grid, stream_management, precision=precision, **kwargs)
+        super().__init__("lmmse" if whiten_interference else "lmmse-no-whitening", resource_grid, stream_management,
+                         precision=precision, **kwargs)
+
+
+class ZFEqualizer(OFDMEqualizer):
+    """ZFEqualizer(resource_grid, stream_management): ZF equalisation for OFDM MIMO (equalization.py:346-403,
+    ``mimo.zf_equalizer`` per resource element); fused kernel ``sb_ofdm_equalize``."""
+
+    def __init__(self, resource_grid, stream_management, precision=None, **kwargs):
+        super().__init__("zf", resource_grid, stream_management, precision=precision, **kwargs)
+
+
+class MFEqualizer(OFDMEqualizer):
+    """MFEqualizer(resource_grid, stream_management): matched-filter equalisation for OFDM MIMO
+    (equalization.py:405-462, ``mimo.mf_equalizer`` per resource element); fused kernel ``sb_ofdm_equalize``."""
+
+    def __init__(self, resource_grid, stream_management, precision=None, **kwargs):
+        super().__init__("mf", resource_grid, stream_management, precision=precision, **kwargs)
