@@ -328,6 +328,31 @@ int sb_cir_apply(const float* d_a, const float* d_e, int64_t e_link_stride, cons
  * correlation matrix (for separate rx / tx matrices: kron(L_rx, conj(L_tx))): out[b, :, c] = L in[b, :, c]. */
 int sb_spatial_corr(const float* d_in, const float* d_l, float* d_out, int64_t batch, int32_t n, int64_t cols,
                     void* stream);
+/* Flat-fading MIMO channel (csrc/flat_fading.cu), complex64, M = num_rx_ant, K = num_tx_ant, num channel uses:
+ * GenerateFlatFadingChannel / ApplyFlatFadingChannel / FlatFadingChannel and the KroneckerModel / PerColumnModel
+ * products (channel/flat_fading_channel.py:11-246, channel/spatial_correlation.py:42-195) in one launch.
+ *   h0: d_h_in [*, M, K] (h_in_stride 0: one matrix for every use, 1: one per use) or, d_h_in NULL, drawn from
+ *       (seed_h, offset_h) with sb_awgn's counter convention over the flat [num, M, K] index (element i: Philox block
+ *       i / 2, words (x, y) for even i, (z, w) for odd i), so the draw equals complex_normal([num, M, K]) bit for bit.
+ *   h = L_rx h0 L_tx^H (tx factor applied first). d_l_tx [*, K, K] and d_l_rx [*, M, M] are lower-triangular factors
+ *       (sb_chol_lower), either may be NULL, each with a stride of 0 (shared) or 1 (one set per use). per_column = 1
+ *       takes d_l_rx as [*, K, M, M] and column k of h as L_rx[k] h0[:, k] (no tx factor).
+ *   d_h_out [num, M, K]: h, written only if not NULL. d_x [*, K] (x_stride 0 or 1) and d_y [num, M]: y = h x, summed
+ *       over k in order. d_no (needs d_x; NULL: no noise): y[i] += sqrt(d_no[i / no_inner]) n_i with n the unit
+ *       complex noise of sb_awgn(seed_n, offset_n) over the flat [num, M] index, bit for bit.
+ * No intermediate goes through global memory. Limits: M <= 128 with an rx factor, K <= 128 with a tx factor and
+ * M K <= 16384 with either; without factors any M and K. Beyond them SB_EUNSUPPORTED with a message; malformed
+ * arguments (strides outside {0, 1}, per_column without d_l_rx or with d_l_tx, neither d_h_out nor d_x, d_x without
+ * d_y, d_no without d_x) return SB_EINVAL. All checks run before any device access; num = 0 then returns SB_OK. */
+int sb_flat_fading(const float* d_h_in, int64_t h_in_stride, uint64_t seed_h, uint64_t offset_h, const float* d_l_tx,
+                   int64_t l_tx_stride, const float* d_l_rx, int64_t l_rx_stride, int32_t per_column, float* d_h_out,
+                   const float* d_x, int64_t x_stride, const float* d_no, int64_t no_inner, uint64_t seed_n,
+                   uint64_t offset_n, float* d_y, int64_t num, int32_t num_rx_ant, int32_t num_tx_ant, void* stream);
+/* Lower Cholesky factors L (L L^H = R) of count n x n complex matrices, d_r and d_l [count, n, n] (the strictly upper
+ * triangle of L is 0), in fp32 by sb_dense::chol_lower, one thread per matrix in shared-memory scratch (n = 128: one
+ * thread per CTA). Only the lower triangle of R is read. A non-positive pivot makes the rest of that matrix's factor
+ * NaN; other matrices are unaffected and nothing synchronises. n <= 128 (SB_EUNSUPPORTED beyond). */
+int sb_chol_lower(const float* d_r, float* d_l, int64_t count, int32_t n, void* stream);
 /* PUSCHPrecoder.call (nr/pusch_precoder.py:75-95): d_x [batch, num_tx, num_layers, num_re] complex, d_w [num_tx,
  * num_ports, num_layers] complex -> d_y [batch, num_tx, num_ports, num_re], y = W x per resource element. */
 int sb_pusch_precode(const float* d_x, const float* d_w, float* d_y, int64_t batch, int32_t num_tx, int32_t num_layers,

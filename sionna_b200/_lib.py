@@ -66,6 +66,8 @@ SIGNATURES = {
     "sb_cir_link_scale": (i32, [vp, vp, i64, vp, i64, i32, i32, i32, i32, i32, i32, f32, vp]),
     "sb_cir_apply": (i32, [vp, vp, i64, vp, vp, i64, i32, i32, i32, i32, i32, i32, i32, vp]),
     "sb_spatial_corr": (i32, [vp, vp, vp, i64, i32, i64, vp]),
+    "sb_flat_fading": (i32, [vp, i64, u64, u64, vp, i64, vp, i64, i32, vp, vp, i64, vp, i64, u64, u64, vp, i64, i32, i32, vp]),
+    "sb_chol_lower": (i32, [vp, vp, i64, i32, vp]),
     "sb_pusch_precode": (i32, [vp, vp, vp, i64, i32, i32, i32, i64, vp]),
     "sb_pusch_ls_combine": (i32, [vp, vp, i64, i32, i32, i32, i32, vp]),
     "sb_lmmse_equalize": (i32, [vp, vp, vp, vp, vp, i64, i32, i32, vp]),

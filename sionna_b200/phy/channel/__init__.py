@@ -7,3 +7,6 @@ from .antenna import AntennaElement, PanelArray, Antenna, AntennaArray
 from .time_channel import (time_lag_discrete_time_channel, cir_to_time_channel, time_to_ofdm_channel, ApplyTimeChannel, GenerateOFDMChannel,
                            OFDMChannel, GenerateTimeChannel, TimeChannel)
 from .rayleigh_block_fading import RayleighBlockFading
+from .spatial_correlation import SpatialCorrelation, KroneckerModel, PerColumnModel
+from .flat_fading_channel import GenerateFlatFadingChannel, ApplyFlatFadingChannel, FlatFadingChannel
+from .utils import exp_corr_mat, one_ring_corr_mat
