@@ -571,6 +571,49 @@ int sb_ofdm_frontend(const float* d_y, const float* d_no, const int64_t* h_no_st
                      int32_t num_terms, int32_t num_data, int32_t bits_per_dim, int32_t method, int32_t hard_out,
                      void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Convolutional codes, rate 1/conv_n (csrc/conv.cu)
+ * replaces ConvEncoder.call                     fec/conv/encoding.py:204-291
+ *          ViterbiDecoder.call / _update_fwd   fec/conv/decoding.py:236-453
+ *          BCJRDecoder.call / _update_fwd/_bwd  fec/conv/decoding.py:694-943
+ * Trellis: constraint length K, ns = 2^(K-1) states, the newest register bit is the state's MSB. The decoders take the
+ * reference's Trellis tables (fec/conv/utils.py:148-190) as host arrays [ns, 2] int32: h_from_nodes,
+ * h_op_by_tonode, h_ip_by_tonode; their order is the order in which the Viterbi decoder breaks ties. Tables that are
+ * not those of a rate-1/conv_n shift register return SB_EINVAL. Limits: 2 <= ns <= 256 (K <= 9), conv_n <= 8; beyond
+ * them SB_EUNSUPPORTED with a message. Any k >= 1 and any batch; codeword bits num_syms * conv_n < 2^31. All checks run
+ * before any device access.
+ * ---------------------------------------------------------------------------------------------- */
+/* ConvEncoder: d_u [batch, k] bits (0 / 1 as float), d_x [batch, T * conv_n] with T = k + (terminate ? K - 1 : 0),
+ * the conv_n bits of step t adjacent. h_gen_poly [conv_n]: polynomial j as an integer whose MSB (bit K - 1) is the
+ * first character of the reference's bit string. rsc = 1: polynomial 0 is the feedback polynomial (its MSB must be
+ * 1) and the termination inputs are the feedback bits (encoding.py:262-285). */
+int sb_conv_encode(const float* d_u, float* d_x, int64_t batch, int32_t k, const int32_t* h_gen_poly, int32_t conv_n,
+                   int32_t constraint_length, int32_t rsc, int32_t terminate, void* stream);
+/* ViterbiDecoder: d_llr [batch, num_syms * conv_n] logits (Sionna's sign). method 0 "soft_llr" (branch metric
+ * sum_j llr_j (1 - 2 b_j) in j order), 1 "hard" (Manhattan distance of int_mod_2 of the input). Path metrics start at
+ * 0 for state 0 and 2^20 elsewhere and are never renormalised; ties go to the first predecessor. The traceback starts
+ * from state 0 (terminate = 1) or the first state with the least metric. return_info_bits = 1: d_out [batch, k] input
+ * bits of the first k steps (1 <= k <= num_syms); 0: d_out [batch, num_syms * conv_n] the re-encoded survivor.
+ * d_workspace: sb_viterbi_workspace_bytes(batch, num_syms, ns) bytes (may be 0 and NULL; SB_ENOMEM if short). */
+int sb_viterbi_decode(const float* d_llr, float* d_out, int64_t batch, int32_t num_syms, int32_t k, int32_t method,
+                      int32_t terminate, int32_t return_info_bits, const int32_t* h_from_nodes,
+                      const int32_t* h_op_by_tonode, const int32_t* h_ip_by_tonode, int32_t ns, int32_t conv_n,
+                      void* d_workspace, size_t workspace_bytes, void* stream);
+/* Device bytes of one decision bit per state and step when they do not fit in shared memory, else 0. */
+size_t sb_viterbi_workspace_bytes(int64_t batch, int32_t num_syms, int32_t ns);
+/* BCJRDecoder: d_llr_ch [batch, num_syms * conv_n] and optional d_llr_a [batch, num_syms] (NULL: 0) logits. algorithm
+ * 0 "map", 1 "log", 2 "maxlog". "map" and "log" are the same function and both run in the log domain with the exact
+ * max* (the reference's probability-domain "map" overflows fp32 once |0.5 sum llr| > 88). The backward recursion starts
+ * uniform unless terminate = 1. d_out [batch, num_out] (1 <= num_out <= num_syms): the APP LLRs of the first num_out
+ * steps' input bits (a turbo decoder takes all num_syms), or llr > 0 as 0 / 1 with hard_out = 1.
+ * d_workspace: sb_bcjr_workspace_bytes(batch, num_syms, ns) bytes (may be 0 and NULL; SB_ENOMEM if short). */
+int sb_bcjr_decode(const float* d_llr_ch, const float* d_llr_a, float* d_out, int64_t batch, int32_t num_syms,
+                   int32_t num_out, int32_t algorithm, int32_t terminate, int32_t hard_out, const int32_t* h_from_nodes,
+                   const int32_t* h_op_by_tonode, const int32_t* h_ip_by_tonode, int32_t ns, int32_t conv_n,
+                   void* d_workspace, size_t workspace_bytes, void* stream);
+/* Device bytes of the forward metrics (ns floats per step) when they do not fit in shared memory, else 0. */
+size_t sb_bcjr_workspace_bytes(int64_t batch, int32_t num_syms, int32_t ns);
+
 #ifdef __cplusplus
 }
 #endif

@@ -87,6 +87,11 @@ SIGNATURES = {
     "sb_ofdm_mmse_pic": (i32, [vp] * 13 + [i64] + [i32] * 12 + [vp]),
     "sb_mimo_precode": (i32, [vp, vp, i64, vp, vp, vp, i64, i32, i32, i32, vp]),
     "sb_ofdm_precode": (i32, [vp] * 11 + [i64] + [i32] * 9 + [vp]),
+    "sb_conv_encode": (i32, [vp, vp, i64, i32, vp, i32, i32, i32, i32, vp]),
+    "sb_viterbi_decode": (i32, [vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp, sz, vp]),
+    "sb_viterbi_workspace_bytes": (sz, [i64, i32, i32]),
+    "sb_bcjr_decode": (i32, [vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp, sz, vp]),
+    "sb_bcjr_workspace_bytes": (sz, [i64, i32, i32]),
 }
 
 

@@ -6,7 +6,8 @@ the boundary is a plain C-ABI loaded with ctypes).
 Every source is compiled on its own (in parallel) and linked into one shared library. The LDPC / mapping sources are
 built with -fmad=false: their arithmetic is specified operation by operation (explicit __f*_rn / fmaf calls) so that the
 CPU oracle reproduces it bit for bit, and the compiler must not contract a*b+c on its own. The flat-fading source is
-built the same way so that its random draws and noise equal sb_awgn's (phy_kernels.cu) bit for bit. The OFDM / MIMO / channel
+built the same way so that its random draws and noise equal sb_awgn's (phy_kernels.cu) bit for bit, and the convolutional
+decoders so that their Viterbi path metrics equal the float32 oracle's bit for bit. The OFDM / MIMO / channel
 sources are tolerance-checked floating-point kernels (FFT butterflies, complex MACs, Cholesky): they are built with the
 default -fmad=true, which halves their instruction count.
 """
@@ -19,7 +20,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "..", "libsionna_b200.so")
 OBJ_DIR = os.path.join(HERE, "..", "..", "build", "obj")
 EXACT = ["common.cu", "ldpc_bp.cu", "ldpc_bp_qc.cu", "ldpc_bp_flat.cu", "ldpc_enc.cu", "phy_kernels.cu",
-         "flat_fading.cu"]                                                                        # -fmad=false
+         "flat_fading.cu", "conv.cu"]                                                                        # -fmad=false
 FAST = ["ofdm_mimo.cu", "channel.cu", "frontend.cu", "mimo_ml.cu", "mimo_kbest.cu",
         "mimo_iterative.cu", "precoding.cu"]                                                     # -fmad=true
 SOURCES = EXACT + FAST

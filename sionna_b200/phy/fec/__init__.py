@@ -1,5 +1,7 @@
-"""Forward error correction (mirror of sionna.phy.fec): LDPC codes, CRC, scrambling and test utilities."""
+"""Forward error correction (mirror of sionna.phy.fec): LDPC and convolutional codes, CRC, scrambling and test
+utilities."""
 from . import ldpc
+from . import conv
 from . import utils
 from . import crc
 from . import scrambling

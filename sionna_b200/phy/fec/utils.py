@@ -77,3 +77,20 @@ def load_parity_check_examples(pcm_id, verbose=False):
     if verbose:
         print(f"\nn: {n}, k: {k}, coderate: {coderate:.3f}")
     return pcm, k, n, coderate
+
+
+def bin2int(arr):
+    """Integer of a binary sequence, most significant bit first (fec/utils.py:532-549): ``[1, 0, 1]`` -> 5; None for
+    an empty sequence."""
+    if len(arr) == 0:
+        return None
+    return int("".join(str(int(x)) for x in arr), 2)
+
+
+def int2bin(num, length):
+    """The ``length`` least significant bits of ``num``, most significant first (fec/utils.py:576-611):
+    ``int2bin(5, 4)`` -> ``[0, 1, 0, 1]``, ``int2bin(12, 3)`` -> ``[1, 0, 0]``."""
+    assert num >= 0, "Input integer should be non-negative"
+    assert length >= 0, "length should be non-negative"
+    bits = format(num, f"0{length}b")
+    return [int(x) for x in bits[-length:]] if length else []
