@@ -244,14 +244,16 @@ int sb_ofdm_modulate(const float* d_x, float* d_out, int64_t rows, int32_t num_s
 int sb_ofdm_demodulate(const float* d_x, float* d_out, int64_t rows, int32_t num_symbols, int32_t fft_size,
                        const int32_t* d_cp, const int32_t* d_in_off, int32_t in_len, int32_t l_min, int32_t shift,
                        void* stream);
-/* out[b, r, j] = in[b, (in_rows == 1 ? 0 : r), idx[r, j]] (0 where idx < 0); words = 1 (fp32) or 2 (complex64).
+/* out[b, r, j] = in[b, (in_rows == 1 ? 0 : r), idx[r, j]] (0 where idx < 0); words = 1 (fp32), 2 (complex64 / fp64)
+ * or 4 (complex128): a bit copy. cols_out == 0 is a no-op and the pointers may then be null.
  * Replaces the tf.gather re-indexing of RemoveNulledSubcarriers (ofdm/resource_grid.py:551), ResourceGridDemapper
  * (:466-520) and NearestNeighborInterpolator (ofdm/channel_estimation.py:409-435). */
 int sb_gather_rows(const float* d_in, const int32_t* d_idx, float* d_out, int64_t batch, int32_t rows, int32_t cols_out,
                    int32_t in_rows, int32_t cols_in, int32_t words, void* stream);
 /* ResourceGridMapper.call (ofdm/resource_grid.py:394-412): d_x [batch, num_streams, num_data], d_pilots [num_streams,
  * num_pilots], d_map [num_streams, grid_size] (>= 0 data index, -1 empty, <= -2 pilot index -(v+2)) -> d_out
- * [batch, num_streams, grid_size]. */
+ * [batch, num_streams, grid_size]. d_x may be null when num_data == 0 (every RE a pilot or nulled), d_pilots when
+ * num_pilots == 0. */
 int sb_rg_map(const float* d_x, const float* d_pilots, const int32_t* d_map, float* d_out, int64_t batch,
               int32_t num_streams, int32_t grid_size, int32_t num_data, int32_t num_pilots, void* stream);
 /* Pilot gather (ofdm/channel_estimation.py:138-150) + LSChannelEstimator.estimate_at_pilot_locations (:257-285):

@@ -124,9 +124,9 @@ def ls_estimate(y_eff, mask, pilots, no, dtype=None):
     return h, np.broadcast_to(err, h.shape)
 
 
-def nn_interp(x, mask, pilots, dtype=None):
+def nn_interp_loop(x, mask, pilots, dtype=None):
     """x [..., tx, st, P] -> [..., tx, st, S, F]: nearest non-zero pilot in Manhattan distance (:384-402), in ``dtype``
-    (None: the type of x)."""
+    (None: the type of x). One RE at a time, as the reference states it; `nn_interp` is the same, vectorised."""
     tx, st, s_, f_ = mask.shape
     if dtype is not None:
         x = np.asarray(x).astype(dtype)
@@ -148,10 +148,11 @@ def _lerp(x, x0, x1, y0, y1):
     return (x - x0) * slope + y0
 
 
-def lin_interp(x, mask, pilots, time_avg=False, dtype=np.complex128):
+def lin_interp_loop(x, mask, pilots, time_avg=False, dtype=np.complex128):
     """x [..., tx, st, P] -> [..., tx, st, S, F] (channel_estimation.py:522-734): per pilot-carrying symbol, linear
     inter/extrapolation over frequency from the two bracketing (or nearest two) non-zero pilots, then the same over time.
-    Evaluated in ``dtype`` (positions and slopes in its real type)."""
+    Evaluated in ``dtype`` (positions and slopes in its real type). One RE at a time; `lin_interp` is the same,
+    vectorised."""
     tx, st, s_, f_ = mask.shape
     rdt = _real(dtype)
     x = np.asarray(x).astype(dtype)
@@ -188,6 +189,68 @@ def lin_interp(x, mask, pilots, time_avg=False, dtype=np.complex128):
                     k1 = min(max(k1, 1), len(syms) - 1)
                     k0 = k1 - 1
                     out[..., i, j, a, :] = _lerp(rdt(a), rdt(syms[k0]), rdt(syms[k1]), hf[syms[k0]], hf[syms[k1]])
+    return out
+
+
+def nn_interp(x, mask, pilots, dtype=None):
+    """x [..., tx, st, P] -> [..., tx, st, S, F]: `nn_interp_loop` with the distances of one OFDM symbol's REs to all
+    non-zero pilots at once. A zero pilot's distance S + F exceeds every real one, so it is never the first minimum
+    and leaving it out changes nothing: the same result bit for bit."""
+    tx, st, s_, f_ = mask.shape
+    if dtype is not None:
+        x = np.asarray(x).astype(dtype)
+    out = np.zeros(x.shape[:-1] + (s_, f_), x.dtype)
+    cols = np.arange(f_)[:, None]
+    for i in range(tx):
+        for j in range(st):
+            i_p, j_p = np.where(mask[i, j])
+            nz = np.nonzero(np.abs(pilots[i, j]) > 0)[0]
+            for a in range(s_):
+                d = np.abs(a - i_p[nz])[None, :] + np.abs(cols - j_p[nz][None, :])    # [F, non-zero pilots]
+                out[..., i, j, a, :] = x[..., i, j, :][..., nz[np.argmin(d, axis=1)]]
+    return out
+
+
+def lin_interp(x, mask, pilots, time_avg=False, dtype=np.complex128):
+    """x [..., tx, st, P] -> [..., tx, st, S, F]: `lin_interp_loop` with the brackets of a whole row (frequency) or
+    column (time) found by one searchsorted, and the same element-wise operations (the same result bit for bit)."""
+    tx, st, s_, f_ = mask.shape
+    rdt = _real(dtype)
+    x = np.asarray(x).astype(dtype)
+    out = np.zeros(x.shape[:-1] + (s_, f_), dtype)
+    c = np.arange(f_)
+    for i in range(tx):
+        for j in range(st):
+            pil = pilots[i, j]
+            pos = np.argwhere(mask[i, j])                            # row-major pilot positions <-> pilot index
+            nz = np.abs(pil) > 0
+            hf = {}
+            for a in range(s_):
+                idx = np.nonzero((pos[:, 0] == a) & nz)[0]
+                if not len(idx):
+                    continue
+                xs = pos[idx, 1]
+                if len(idx) == 1:
+                    k0 = k1 = np.zeros(f_, int)
+                else:
+                    k1 = np.clip(np.searchsorted(xs, c, side="left"), 1, len(idx) - 1)
+                    k0 = k1 - 1
+                hf[a] = _lerp(c.astype(rdt), xs[k0].astype(rdt), xs[k1].astype(rdt), x[..., i, j, idx[k0]],
+                              x[..., i, j, idx[k1]])
+            syms = sorted(hf)
+            if time_avg:
+                avg = sum(hf[a] for a in syms) / len(syms)
+                hf = {a: avg for a in syms}
+            if len(syms) == 1:
+                out[..., i, j, :, :] = hf[syms[0]][..., None, :]
+                continue
+            t = np.arange(s_)
+            k1 = np.clip(np.searchsorted(syms, t, side="left"), 1, len(syms) - 1)
+            k0 = k1 - 1
+            rows = np.stack([hf[a] for a in syms], axis=-2)           # [..., num pilot symbols, F]
+            sy = np.asarray(syms)
+            out[..., i, j, :, :] = _lerp(t.astype(rdt)[:, None], sy[k0].astype(rdt)[:, None], sy[k1].astype(rdt)[:, None],
+                                         rows[..., k0, :], rows[..., k1, :])
     return out
 
 

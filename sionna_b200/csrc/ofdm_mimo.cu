@@ -1242,7 +1242,8 @@ extern "C" int sb_ofdm_demodulate(const float* d_x, float* d_out, int64_t rows, 
 
 extern "C" int sb_gather_rows(const float* d_in, const int32_t* d_idx, float* d_out, int64_t batch, int32_t rows,
                               int32_t cols_out, int32_t in_rows, int32_t cols_in, int32_t words, void* stream) {
-    if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
+    // empty batch, or no columns to gather (the data REs of an all-pilot grid): nothing to do, pointers may be null
+    if (batch == 0 || cols_out == 0) return SB_OK;
     SB_CHECK_ARG(d_in && d_idx && d_out && batch >= 0 && rows > 0 && cols_out > 0 && cols_in > 0 &&
                      (in_rows == 1 || in_rows == rows) && (words == 1 || words == 2 || words == 4),
                  "sb_gather_rows: bad arguments");
@@ -1262,7 +1263,9 @@ extern "C" int sb_gather_rows(const float* d_in, const int32_t* d_idx, float* d_
 extern "C" int sb_rg_map(const float* d_x, const float* d_pilots, const int32_t* d_map, float* d_out, int64_t batch,
                          int32_t num_streams, int32_t grid_size, int32_t num_data, int32_t num_pilots, void* stream) {
     if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(d_x && d_map && d_out && batch >= 0 && num_streams > 0 && grid_size > 0, "sb_rg_map: bad arguments");
+    // d_x is never read without data REs (an all-pilot grid), nor d_pilots without pilots: either may then be null
+    SB_CHECK_ARG((d_x || num_data == 0) && (d_pilots || num_pilots == 0) && d_map && d_out && batch >= 0 &&
+                     num_streams > 0 && grid_size > 0 && num_data >= 0 && num_pilots >= 0, "sb_rg_map: bad arguments");
     long long total = batch * num_streams * (long long)grid_size;
     if (total == 0) return SB_OK;
     const RowLaunch rl = row_launch(batch * num_streams, grid_size);

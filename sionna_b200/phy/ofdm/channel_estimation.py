@@ -40,14 +40,17 @@ class NearestNeighborInterpolator(BaseChannelInterpolator):
         assert np.max(np.sum(np.abs(pilots) == 0, -1)) < pilots.shape[-1], \
             "Each pilot sequence must have at least one nonzero entry"
         s_, f_ = mask_shape[-2:]
-        ii, jj = np.meshgrid(np.arange(s_), np.arange(f_), indexing="ij")
-        gather_ind = np.zeros((mask.shape[0], s_ * f_), np.int32)
+        cols = np.arange(f_)[:, None]
+        gather_ind = np.zeros((mask.shape[0], s_, f_), np.int32)
         for a in range(mask.shape[0]):
             i_p, j_p = np.where(mask[a])
-            d = np.abs(ii.reshape(-1, 1) - i_p[None, :]) + np.abs(jj.reshape(-1, 1) - j_p[None, :])
-            d[:, np.abs(pilots[a]) == 0] = s_ + f_
-            gather_ind[a] = np.argmin(d, axis=1)
-        self._gather_ind = gather_ind
+            # zero pilots are never the nearest (the reference gives them a distance beyond any RE's), so only the
+            # non-zero ones are candidates; one OFDM symbol at a time keeps the distance matrix at F x (non-zero pilots)
+            nz = np.nonzero(np.abs(pilots[a]) > 0)[0]
+            for s in range(s_):
+                d = np.abs(s - i_p[nz])[None, :] + np.abs(cols - j_p[nz][None, :])
+                gather_ind[a, s] = nz[np.argmin(d, axis=1)]
+        self._gather_ind = gather_ind.reshape(mask.shape[0], s_ * f_)
         self._shape = mask_shape
         self._dev = None
 
@@ -218,7 +221,7 @@ class LSChannelEstimator(BaseChannelEstimator):
         if self.precision != "single":
             raise NotImplementedError("LSChannelEstimator runs complex64 kernels only.")
         pp = self._pilot_pattern
-        y_eff = self._remove_nulled_scs(y)                                       # [B, rx, ant, S, F]
+        y_eff = self._remove_nulled_scs(y).to(torch.complex64)                  # [B, rx, ant, S, F]
         lead = list(y_eff.shape[:3])
         y_flat = y_eff.reshape(-1, y_eff.shape[-2] * y_eff.shape[-1]).contiguous()
         no_b = _broadcast_inner(no, lead, y_flat.device, torch.float32)          # element b' uses no[b' // inner]

@@ -201,6 +201,8 @@ class ResourceGridMapper(Block):
 class RemoveNulledSubcarriers(Block):
     """Drops guard and DC subcarriers: ``[..., fft_size] -> [..., num_effective_subcarriers]`` (resource_grid.py:522-553)."""
 
+    _native_double = True                   # a bit copy: float64 / complex128 pass through unrounded
+
     def __init__(self, resource_grid, precision=None, **kwargs):
         self._sc_ind = np.asarray(resource_grid.effective_subcarrier_ind, np.int32)
         self._fft_size = resource_grid.fft_size
@@ -221,6 +223,8 @@ class ResourceGridDemapper(Block):
     """ResourceGridDemapper(resource_grid, stream_management): extracts the data REs of every stream from
     ``[batch, num_rx, num_streams_per_rx, num_ofdm_symbols, fft_size(, data_dim)]`` ->
     ``[batch, num_tx, num_streams_per_tx, num_data_symbols(, data_dim)]`` (resource_grid.py:414-520)."""
+
+    _native_double = True                   # a bit copy: float64 / complex128 pass through unrounded
 
     def __init__(self, resource_grid, stream_management, precision=None, **kwargs):
         super().__init__(precision=precision, **kwargs)

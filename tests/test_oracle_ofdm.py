@@ -191,3 +191,50 @@ def test_ls_and_interpolation_in_complex64_equal_complex128_to_fp32_rounding(int
     assert np.abs(r32 - r64).max() <= 8 * eps * np.abs(r64).max()
     assert np.abs(q32 - q64).max() <= 8 * eps * np.abs(q64).max()
     assert np.abs(r32 - r64).max() > 0                                                   # really single precision
+
+
+def _small_patterns(rng):
+    """(mask, pilots) pairs that reach every bracketing rule: Kronecker combs, a pilot symbol with one non-zero pilot,
+    zero pilots between non-zero ones, pilots on the first / last symbol and subcarrier, per-stream masks that differ,
+    a stream whose pilots sit on one symbol only, S = 1 and F = 1."""
+    out = []
+    mask = F.kronecker_mask(2, 1, 14, 12, [2, 11])
+    pil = np.zeros((2, 1, 2, 12), complex)
+    pil[0, 0, :, 0::2], pil[1, 0, :, 1::2] = 1.0, -1j
+    out.append((mask, pil.reshape(2, 1, -1)))
+    mask = np.zeros((1, 3, 9, 10), bool)
+    mask[0, 0, [0, 4], :] = True                                             # 20 pilots each
+    mask[0, 1, 8, :] = True
+    mask[0, 1, 3, :] = True
+    mask[0, 2, :, [0, 9]] = True
+    mask[0, 2, 1, 5] = mask[0, 2, 7, 5] = True
+    pil = (rng.uniform(0.3, 2.0, (1, 3, 20)) * np.exp(2j * np.pi * rng.uniform(size=(1, 3, 20))))
+    pil[0, 0, 1:9] = 0                                                       # symbol 0: pilots on subcarriers 0 and 9 only
+    pil[0, 0, 12:] = 0                                                       # symbol 4: one pilot, at subcarrier 1
+    pil[0, 0, 10] = 0
+    pil[0, 1, 10:] = 0                                                       # stream 1: symbol 3 only
+    out.append((mask, pil))
+    out.append((np.ones((1, 1, 1, 7), bool), rng.normal(size=(1, 1, 7)) + 1j))        # S = 1
+    m1 = np.zeros((1, 2, 6, 1), bool)
+    m1[0, 0, [1, 4], 0] = True
+    m1[0, 1, [0, 5], 0] = True
+    out.append((m1, np.array([[[1.0, 2.0], [0.5j, 0.0]]])))                            # F = 1
+    return out
+
+
+@pytest.mark.parametrize("dtype", [np.complex128, np.complex64])
+def test_vectorised_interpolators_equal_loop_forms(dtype):
+    """oracle.ofdm.nn_interp / lin_interp (vectorised, used at thousands of subcarriers) return exactly what the RE-by-RE
+    restatements nn_interp_loop / lin_interp_loop return, on every small pattern and in both precisions."""
+    rng = np.random.default_rng(11)
+    for mask, pil in _small_patterns(rng):
+        p = pil.shape[-1]
+        x = rng.normal(size=(2, 3) + pil.shape) + 1j * rng.normal(size=(2, 3) + pil.shape)
+        for ta in (False, True):
+            want = F.lin_interp_loop(x, mask, pil, ta, dtype=dtype)
+            got = F.lin_interp(x, mask, pil, ta, dtype=dtype)
+            assert got.dtype == want.dtype and np.array_equal(got, want), (mask.shape, ta)
+        rdt = np.float32 if dtype == np.complex64 else None
+        assert np.array_equal(F.nn_interp(x, mask, pil, dtype=dtype), F.nn_interp_loop(x, mask, pil, dtype=dtype))
+        ev = rng.uniform(size=x.shape[:-1] + (p,))
+        assert np.array_equal(F.nn_interp(ev, mask, pil, dtype=rdt), F.nn_interp_loop(ev, mask, pil, dtype=rdt))
