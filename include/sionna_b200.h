@@ -616,6 +616,34 @@ int sb_bcjr_decode(const float* d_llr_ch, const float* d_llr_a, float* d_out, in
 /* Device bytes of the forward metrics (ns floats per step) when they do not fit in shared memory, else 0. */
 size_t sb_bcjr_workspace_bytes(int64_t batch, int32_t num_syms, int32_t ns);
 
+/* ------------------------------------------------------------------------------------------------
+ * Turbo codes: two rate-1/2 RSC component codes joined by an interleaver (csrc/conv.cu)
+ * replaces TurboDecoder.call / _convenc_cws      fec/turbo/decoding.py:271-312, 357-435
+ *          BCJRDecoder (the component decoder)   fec/conv/decoding.py:694-943
+ * The encoder composes sb_gather_rows and sb_conv_encode; only the decoder has a kernel of its own.
+ * ---------------------------------------------------------------------------------------------- */
+typedef struct sb_turbo_perm sb_turbo_perm;
+/* The interleaver pi (Turbo3GPPInterleaver / RandomInterleaver, fec/interleaving.py:197-745): h_perm [k], decoder 2
+ * sees u[pi(i)] at step i. Returns SB_EINVAL unless h_perm is a permutation of 0 ... k - 1; checked on the host
+ * before any device access. The table is uploaded on first use on each device. */
+int sb_turbo_perm_create(sb_turbo_perm** out, const int32_t* h_perm, int32_t k);
+void sb_turbo_perm_destroy(sb_turbo_perm* p);
+/* TurboDecoder: d_llr [batch, 2, 2 T] logits (Sionna's sign) of the two component codewords, T = k + (terminate ?
+ * K - 1 : 0) steps of conv_n = 2 bits each (systematic, parity), punctured positions 0; decoder 2's systematic LLRs
+ * are decoder 1's through pi. Trellis tables and algorithm as sb_bcjr_decode; both component codes share them. Runs
+ * num_iter iterations of decoder 1 then decoder 2 in one launch, exchanging extrinsic LLRs clipped to +-20 (prior 0 on
+ * the termination steps). d_out [batch, k]: decoder 2's APP LLRs deinterleaved, or llr > 0 as 0 / 1 with hard_out = 1;
+ * num_iter = 0 gives zeros. Limits: ns <= 256; conv_n other than 2 is SB_EUNSUPPORTED. A missing handle or one of
+ * another length is SB_EINVAL. d_workspace: sb_turbo_workspace_bytes(batch, k, terminate, ns) bytes (may be 0 and
+ * NULL; SB_ENOMEM if short). All checks run before any device access. */
+int sb_turbo_decode(const float* d_llr, const sb_turbo_perm* perm, float* d_out, int64_t batch, int32_t k,
+                    int32_t num_iter, int32_t algorithm, int32_t terminate, int32_t hard_out,
+                    const int32_t* h_from_nodes, const int32_t* h_op_by_tonode, const int32_t* h_ip_by_tonode,
+                    int32_t ns, int32_t conv_n, void* d_workspace, size_t workspace_bytes, void* stream);
+/* Device bytes of the forward metrics (ns floats per step) and the extrinsic LLRs (k floats per codeword), each when it
+ * does not fit in shared memory; 0 when both do. */
+size_t sb_turbo_workspace_bytes(int64_t batch, int32_t k, int32_t terminate, int32_t ns);
+
 #ifdef __cplusplus
 }
 #endif

@@ -92,6 +92,10 @@ SIGNATURES = {
     "sb_viterbi_workspace_bytes": (sz, [i64, i32, i32]),
     "sb_bcjr_decode": (i32, [vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp, sz, vp]),
     "sb_bcjr_workspace_bytes": (sz, [i64, i32, i32]),
+    "sb_turbo_perm_create": (i32, [C.POINTER(vp), vp, i32]),
+    "sb_turbo_perm_destroy": (None, [vp]),
+    "sb_turbo_decode": (i32, [vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp, sz, vp]),
+    "sb_turbo_workspace_bytes": (sz, [i64, i32, i32, i32]),
 }
 
 

@@ -1,5 +1,6 @@
 // conv.cu -- rate-1/n convolutional codes: encoder, Viterbi decoder and BCJR decoder (fec/conv/encoding.py:11-292,
-// fec/conv/decoding.py:19-943), DESIGN §3.11.
+// fec/conv/decoding.py:19-943), DESIGN §3.11; the turbo decoder on the same BCJR passes (fec/turbo/decoding.py:15-435),
+// DESIGN §3.12.
 //
 // Trellis. K = constraint length, ns = 2^(K-1) states, conv_n output bits per step. The newest register bit is the
 // state's MSB, so the two predecessors of state s are ((s << 1) & (ns - 1)) | b, b = 0, 1, and the two successors of
@@ -22,6 +23,7 @@
 #include "sb_common.h"
 #include <math.h>
 #include <stdint.h>
+#include <vector>
 
 namespace {
 
@@ -113,11 +115,17 @@ __device__ __forceinline__ float branch_metric(const float* __restrict__ y, int 
     return acc;
 }
 
-// Fill the warp's table for steps [t0, t0 + nt) of its G codewords: tab[(g * ch + tt) * tw + o]; with a prior (tw =
-// 2^conv_n + 1) entry 2^conv_n holds 0.5 llr_a. Lanes of codewords beyond the batch read the last codeword.
-template <int MODE>
-__device__ void fill_table(float* tab, const float* __restrict__ llr, const float* __restrict__ llr_a, long long cw0,
-                           long long batch, int G, int T, int conv_n, int t0, int nt, int ch, int tw, int lane) {
+// Fill the warp's table for steps [t0, t0 + nt) of its G codewords: tab[(g * ch + tt) * tw + o]; codeword cw's step t
+// reads llr[(cw * row_steps + t) * conv_n ...]. With a prior (tw = 2^conv_n + 1) entry 2^conv_n holds prior(g, cw, t),
+// half the a-priori LLR of codeword g's step t. Lanes of codewords beyond the batch read the last codeword.
+struct NoPrior {
+    __device__ float operator()(int, long long, int) const { return 0.f; }
+};
+
+template <int MODE, class Prior>
+__device__ void fill_table(float* tab, const float* __restrict__ llr, long long row_steps,
+                                           const Prior& prior, long long cw0, long long batch, int G, int conv_n,
+                                           int t0, int nt, int ch, int tw, int lane) {
     const int no = 1 << conv_n;
     const int total = G * nt * tw;
     for (int e = lane; e < total; e += 32) {
@@ -127,8 +135,8 @@ __device__ void fill_table(float* tab, const float* __restrict__ llr, const floa
         const long long cw = min(cw0 + g, batch - 1);
         const int t = t0 + tt;
         float v;
-        if (o < no) v = branch_metric<MODE>(llr + (cw * T + t) * conv_n, o, conv_n);
-        else v = llr_a ? __fmul_rn(0.5f, __ldg(llr_a + cw * T + t)) : 0.f;
+        if (o < no) v = branch_metric<MODE>(llr + (cw * row_steps + t) * conv_n, o, conv_n);
+        else v = prior(g, cw, t);
         tab[(g * ch + tt) * tw + o] = v;
     }
 }
@@ -180,7 +188,7 @@ __global__ void __launch_bounds__(kWarps * 32) viterbi_kernel(
     for (int t0 = 0; t0 < T; t0 += ch) {
         const int nt = min(ch, T - t0);
         __syncwarp();
-        fill_table<MODE>(tab, llr, nullptr, cw0, batch, G, T, conv_n, t0, nt, ch, tw, lane);
+        fill_table<MODE>(tab, llr, T, NoPrior{}, cw0, batch, G, conv_n, t0, nt, ch, tw, lane);
         __syncwarp();
         for (int tt = 0; tt < nt; ++tt) {
             const float* bm = tab + (g * ch + tt) * tw;
@@ -249,25 +257,16 @@ __device__ __forceinline__ float max_star(float a, float b) {
 }
 
 // alpha_t (before step t) is stored per step, ns floats in state order: G * T * ns per warp (shared or workspace). The
-// backward pass forms beta and the APP LLR of step t from alpha_t, gamma_t and beta_{t+1}.
-template <int L, int R, bool MAXLOG>
-__global__ void __launch_bounds__(kWarps * 32) bcjr_kernel(
-    const float* __restrict__ llr, const float* __restrict__ llr_a, float* __restrict__ out, float* __restrict__ ws_alpha,
-    long long batch, int T, int conv_n, int num_out, int terminate, int hard_out, int ch, int tw, int on_chip,
-    const __grid_constant__ ConvTrellis tr) {
+// backward pass forms beta and the APP LLR of step t from alpha_t, gamma_t and beta_{t+1}. Both passes are shared by
+// the BCJR and turbo kernels: `prior` supplies the a-priori LLR of a step (see fill_table) and `store(t, v)` receives the
+// APP LLR v (Sionna's sign) of step t < num_out of the lane group's own codeword, on its lane 0, if it is in the batch.
+// Codeword cw's channel LLRs are llr[(cw * row_steps + t) * conv_n ...]; alpha points at the group's own T * ns floats.
+template <int L, int R, bool MAXLOG, class Prior>
+__device__ __forceinline__ void bcjr_forward(float* tab, float* alpha, const float* __restrict__ llr, long long row_steps,
+                                             const Prior& prior, long long cw0, long long batch, int T, int conv_n,
+                                             int ch, int tw, int l, int g, int lane, const ConvTrellis& tr) {
     constexpr int NS = L * R, G = 32 / L;
-    extern __shared__ float smem[];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int g = lane / L, l = lane % L;
-    const long long cw0 = ((long long)blockIdx.x * kWarps + warp) * G;
-    if (cw0 >= batch) return;
     const int no = 1 << conv_n;
-    const size_t table_floats = (size_t)G * ch * tw;
-    float* tab = smem + warp * table_floats;
-    float* alpha = (on_chip ? smem + kWarps * table_floats + (size_t)warp * G * T * NS : ws_alpha + cw0 * T * NS) +
-                   (size_t)g * T * NS;
-
-    // forward, blocked states l R + r
     uint32_t trw[R];
     float a[R];
 #pragma unroll
@@ -278,7 +277,7 @@ __global__ void __launch_bounds__(kWarps * 32) bcjr_kernel(
     for (int t0 = 0; t0 < T; t0 += ch) {
         const int nt = min(ch, T - t0);
         __syncwarp();
-        fill_table<kHalf>(tab, llr, llr_a, cw0, batch, G, T, conv_n, t0, nt, ch, tw, lane);
+        fill_table<kHalf>(tab, llr, row_steps, prior, cw0, batch, G, conv_n, t0, nt, ch, tw, lane);
         __syncwarp();
         for (int tt = 0; tt < nt; ++tt) {
             const float* bm = tab + (g * ch + tt) * tw;
@@ -304,8 +303,15 @@ __global__ void __launch_bounds__(kWarps * 32) bcjr_kernel(
         }
     }
     __syncwarp();
+}
 
-    // backward, interleaved states r L + l
+template <int L, int R, bool MAXLOG, class Prior, class Store>
+__device__ __forceinline__ void bcjr_backward(float* tab, const float* alpha, const float* __restrict__ llr,
+                                              long long row_steps, const Prior& prior, long long cw0, long long batch,
+                                              int T, int conv_n, int num_out, int terminate, int ch, int tw, int l,
+                                              int g, int lane, const ConvTrellis& tr, const Store& store) {
+    constexpr int NS = L * R, G = 32 / L;
+    const int no = 1 << conv_n;
     uint32_t frw[R];
     float b[R];
 #pragma unroll
@@ -317,7 +323,7 @@ __global__ void __launch_bounds__(kWarps * 32) bcjr_kernel(
     for (int t1 = T; t1 > 0; t1 -= ch) {
         const int t0 = max(0, t1 - ch), nt = t1 - t0;
         __syncwarp();
-        fill_table<kHalf>(tab, llr, llr_a, cw0, batch, G, T, conv_n, t0, nt, ch, tw, lane);
+        fill_table<kHalf>(tab, llr, row_steps, prior, cw0, batch, G, conv_n, t0, nt, ch, tw, lane);
         __syncwarp();
         for (int tt = nt - 1; tt >= 0; --tt) {
             const int t = t0 + tt;
@@ -343,14 +349,95 @@ __global__ void __launch_bounds__(kWarps * 32) bcjr_kernel(
                 num = max_star<MAXLOG>(num, __shfl_xor_sync(kFull, num, off, L));
                 den = max_star<MAXLOG>(den, __shfl_xor_sync(kFull, den, off, L));
             }
-            if (l == 0 && cw < batch && t < num_out) {
-                const float v = __fsub_rn(den, num);                // Sionna's sign: log p(1) / p(0)
-                out[cw * num_out + t] = hard_out ? (v > 0.f ? 1.f : 0.f) : v;
-            }
+            if (l == 0 && cw < batch && t < num_out) store(t, __fsub_rn(den, num));   // Sionna's sign: log p(1) / p(0)
             const float b0 = __shfl_sync(kFull, nb[0], 0, L);
 #pragma unroll
             for (int r = 0; r < R; ++r) b[r] = __fsub_rn(nb[r], b0);
         }
+    }
+}
+
+template <int L, int R, bool MAXLOG>
+__global__ void __launch_bounds__(kWarps * 32) bcjr_kernel(
+    const float* __restrict__ llr, const float* __restrict__ llr_a, float* __restrict__ out, float* __restrict__ ws_alpha,
+    long long batch, int T, int conv_n, int num_out, int terminate, int hard_out, int ch, int tw, int on_chip,
+    const __grid_constant__ ConvTrellis tr) {
+    constexpr int NS = L * R, G = 32 / L;
+    extern __shared__ float smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int g = lane / L, l = lane % L;
+    const long long cw0 = ((long long)blockIdx.x * kWarps + warp) * G;
+    if (cw0 >= batch) return;
+    const size_t table_floats = (size_t)G * ch * tw;
+    float* tab = smem + warp * table_floats;
+    float* alpha = (on_chip ? smem + kWarps * table_floats + (size_t)warp * G * T * NS : ws_alpha + cw0 * T * NS) +
+                   (size_t)g * T * NS;
+    const auto prior = [&](int, long long cw, int t) { return llr_a ? __fmul_rn(0.5f, __ldg(llr_a + cw * T + t)) : 0.f; };
+    const long long cw = cw0 + g;
+    const auto store = [&](int t, float v) { out[cw * num_out + t] = hard_out ? (v > 0.f ? 1.f : 0.f) : v; };
+    bcjr_forward<L, R, MAXLOG>(tab, alpha, llr, T, prior, cw0, batch, T, conv_n, ch, tw, l, g, lane, tr);
+    bcjr_backward<L, R, MAXLOG>(tab, alpha, llr, T, prior, cw0, batch, T, conv_n, num_out, terminate, ch, tw, l, g,
+                                lane, tr, store);
+}
+
+// ---- turbo ----------------------------------------------------------------------------------------------------------
+// All num_iter iterations of both rate-1/2 component decoders in one launch (fec/turbo/decoding.py:357-435). llr holds
+// the two component codewords of each turbo codeword side by side, [batch, 2, 2 T]; decoder 2's systematic LLRs are
+// decoder 1's gathered through pi. The warp owns its G codewords throughout, so __syncwarp is the only barrier.
+// Extrinsic buffer: k floats per codeword, always in decoder 1's (natural) order. Decoder 1 reads its prior at step t
+// from position t and writes its extrinsic there; decoder 2 reads its prior at step t from position pi(t) and writes
+// its extrinsic there, i.e. deinterleaved. Each position is read by exactly one step of a half-iteration (pi is a
+// permutation): in that step's chunk fill of the forward pass, again in the backward pass's chunk fill, and by the
+// storing lane in the same step just before it overwrites it. The fill of a backward chunk precedes (__syncwarp) every
+// store of that chunk, and later chunks hold other steps, so no value is overwritten before its last read.
+// Extrinsic out of decoder 1: clip((APP - L_sys) - L_a); of decoder 2: clip((APP - L_a) - L_sys), clip to +-20, the
+// reference's operation order (:407-423). The termination steps' prior is 0. The last half-iteration scatters
+// decoder 2's APP through pi into out: out[pi(t)] = APP_2(t).
+template <int L, int R, bool MAXLOG>
+__global__ void __launch_bounds__(kWarps * 32) turbo_kernel(
+    const float* __restrict__ llr, const int32_t* __restrict__ perm, float* __restrict__ out, float* ws_alpha,
+    float* ws_ext, long long batch, int k, int T, int num_iter, int terminate, int hard_out, int ch, int tw,
+    int alpha_on_chip, int ext_on_chip, const __grid_constant__ ConvTrellis tr) {
+    constexpr int NS = L * R, G = 32 / L, conv_n = 2;
+    constexpr float kClip = 20.f;
+    extern __shared__ float smem[];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int g = lane / L, l = lane % L;
+    const long long cw0 = ((long long)blockIdx.x * kWarps + warp) * G;
+    if (cw0 >= batch) return;
+    const size_t table_floats = (size_t)G * ch * tw;
+    float* tab = smem + warp * table_floats;
+    float* chip = smem + kWarps * table_floats;
+    float* alpha = (alpha_on_chip ? chip + (size_t)warp * G * T * NS : ws_alpha + cw0 * T * NS) + (size_t)g * T * NS;
+    if (alpha_on_chip) chip += (size_t)kWarps * G * T * NS;
+    // written during the kernel: plain loads, not the read-only path
+    float* ext = ext_on_chip ? chip + (size_t)warp * G * k : ws_ext + cw0 * k;
+    float* my_ext = ext + (size_t)g * k;
+    for (int i = l; i < k; i += L) my_ext[i] = 0.f;
+    const long long row_steps = 2LL * T;
+    const long long cw = cw0 + g;
+    // half-iteration h: decoder d = h & 1 reads its prior at step t from position t (d = 0) or pi(t) (d = 1)
+    for (int h = 0; h < 2 * num_iter; ++h) {
+        const int d = h & 1;
+        const bool last = h + 1 == 2 * num_iter;
+        const float* llr_d = llr + d * 2 * T;
+        const auto pos = [&](int t) { return d ? __ldg(perm + t) : t; };
+        const auto prior = [&](int gg, long long, int t) {
+            return t < k ? __fmul_rn(0.5f, ext[(size_t)gg * k + pos(t)]) : 0.f;
+        };
+        const auto store = [&](int t, float v) {
+            const int p = pos(t);
+            if (last) {
+                out[cw * k + p] = hard_out ? (v > 0.f ? 1.f : 0.f) : v;
+                return;
+            }
+            const float ls = __ldg(llr_d + (cw * row_steps + t) * conv_n), la = my_ext[p];
+            const float e = d ? __fsub_rn(__fsub_rn(v, la), ls) : __fsub_rn(__fsub_rn(v, ls), la);
+            my_ext[p] = fminf(fmaxf(e, -kClip), kClip);
+        };
+        bcjr_forward<L, R, MAXLOG>(tab, alpha, llr_d, row_steps, prior, cw0, batch, T, conv_n, ch, tw, l, g, lane, tr);
+        bcjr_backward<L, R, MAXLOG>(tab, alpha, llr_d, row_steps, prior, cw0, batch, T, conv_n, k, terminate, ch, tw, l,
+                                    g, lane, tr, store);
     }
 }
 
@@ -546,6 +633,136 @@ extern "C" int sb_bcjr_decode(const float* d_llr_ch, const float* d_llr_a, float
         kern<<<grid, kWarps * 32, smem, (cudaStream_t)stream>>>(d_llr_ch, d_llr_a, d_out, (float*)d_workspace, batch,
                                                                  num_syms, conv_n, num_out, terminate, hard_out, p.ch,
                                                                  p.tw, p.on_chip, tr);
+        SB_LAUNCH_CHECK();
+        return SB_OK;
+    });
+}
+
+// ---- turbo decoder (host) -------------------------------------------------------------------------------------------
+// The interleaver pi of a turbo code, checked on the host at creation; uploaded on first use per device, as
+// sb_ldpc5g_encoder does, so that the kernel only ever reads validated indices.
+struct sb_turbo_perm {
+    int k = 0;
+    std::vector<int32_t> h;
+    int device = -1;
+    int32_t* d = nullptr;
+};
+
+namespace {
+
+// Extrinsic buffer: k floats per codeword, in shared memory when kWarps of them fit the on-chip budget.
+struct TurboPlan {
+    WarpPlan w;
+    size_t ext_bytes;   // per warp
+    bool ext_on_chip;
+};
+
+TurboPlan turbo_plan(int ns, int k, int T) {
+    TurboPlan p;
+    p.w = warp_plan(ns, 2, T, true, bcjr_step_bytes(ns));
+    p.ext_bytes = (size_t)p.w.G * k * sizeof(float);
+    p.ext_on_chip = kWarps * p.ext_bytes <= kOnChipBytes;
+    return p;
+}
+
+int turbo_syms(int k, int terminate, int ns) { return k + (terminate ? 31 - __builtin_clz((unsigned)ns) : 0); }
+
+int ensure_uploaded(sb_turbo_perm* p) {
+    int dev = 0;
+    SB_CUDA(cudaGetDevice(&dev));
+    if (p->d && p->device == dev) return SB_OK;
+    if (p->d) cudaFree(p->d);
+    p->d = nullptr;
+    SB_CUDA(cudaMalloc((void**)&p->d, p->h.size() * sizeof(int32_t)));
+    SB_CUDA(cudaMemcpy(p->d, p->h.data(), p->h.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    p->device = dev;
+    return SB_OK;
+}
+
+}  // namespace
+
+extern "C" int sb_turbo_perm_create(sb_turbo_perm** out, const int32_t* h_perm, int32_t k) {
+    const char* who = "sb_turbo_perm_create";
+    SB_CHECK_ARG(out && h_perm && k >= 1, "%s: bad arguments (out and h_perm given, k >= 1)", who);
+    std::vector<char> seen(k, 0);
+    for (int i = 0; i < k; ++i) {
+        const int32_t v = h_perm[i];
+        SB_CHECK_ARG(v >= 0 && v < k, "%s: h_perm[%d] = %d is outside 0 ... %d", who, i, v, k - 1);
+        SB_CHECK_ARG(!seen[v], "%s: h_perm is not a permutation (%d appears twice)", who, v);
+        seen[v] = 1;
+    }
+    auto* p = new sb_turbo_perm();
+    p->k = k;
+    p->h.assign(h_perm, h_perm + k);
+    *out = p;
+    return SB_OK;
+}
+
+extern "C" void sb_turbo_perm_destroy(sb_turbo_perm* p) {
+    if (!p) return;
+    if (p->d) cudaFree(p->d);
+    delete p;
+}
+
+extern "C" size_t sb_turbo_workspace_bytes(int64_t batch, int32_t k, int32_t terminate, int32_t ns) {
+    if (batch < 0 || k < 1 || ns < 2 || ns > kMaxStates || (ns & (ns - 1)) || (terminate != 0 && terminate != 1))
+        return 0;
+    const int T = turbo_syms(k, terminate, ns);
+    const TurboPlan p = turbo_plan(ns, k, T);
+    const long long per_cta = kWarps * p.w.G;
+    const long long rows = (batch + per_cta - 1) / per_cta * per_cta;
+    return (p.w.on_chip ? 0 : (size_t)rows * T * bcjr_step_bytes(ns)) +
+           (p.ext_on_chip ? 0 : (size_t)rows * k * sizeof(float));
+}
+
+extern "C" int sb_turbo_decode(const float* d_llr, const sb_turbo_perm* perm, float* d_out, int64_t batch, int32_t k,
+                               int32_t num_iter, int32_t algorithm, int32_t terminate, int32_t hard_out,
+                               const int32_t* h_from_nodes, const int32_t* h_op_by_tonode,
+                               const int32_t* h_ip_by_tonode, int32_t ns, int32_t conv_n, void* d_workspace,
+                               size_t workspace_bytes_given, void* stream) {
+    const char* who = "sb_turbo_decode";
+    ConvTrellis tr;
+    int rc = pack_trellis(who, ns, conv_n, h_from_nodes, h_op_by_tonode, h_ip_by_tonode, &tr);
+    if (rc) return rc;
+    if (conv_n != 2) {
+        sb_set_error("%s: the component codes have %d output bits per step, turbo decoding needs rate 1/2", who, conv_n);
+        return SB_EUNSUPPORTED;
+    }
+    SB_CHECK_ARG(batch >= 0 && k >= 1 && num_iter >= 0 && algorithm >= 0 && algorithm <= 2 &&
+                 (terminate == 0 || terminate == 1) && (hard_out == 0 || hard_out == 1),
+                 "%s: bad arguments (batch >= 0, k >= 1, num_iter >= 0, algorithm in {0, 1, 2}, terminate and "
+                 "hard_out in {0, 1})", who);
+    SB_CHECK_ARG(perm && perm->k == k, "%s: the interleaver handle is missing or not of length k = %d", who, k);
+    const int T = turbo_syms(k, terminate, ns);
+    rc = check_shape(who, batch, 2 * T, conv_n);
+    if (rc) return rc;
+    if (batch == 0) return SB_OK;
+    SB_CHECK_ARG(d_llr && d_out, "%s: null pointer", who);
+    const TurboPlan p = turbo_plan(ns, k, T);
+    const size_t need = sb_turbo_workspace_bytes(batch, k, terminate, ns);
+    rc = check_workspace(who, "sb_turbo_workspace_bytes", d_workspace, workspace_bytes_given, need);
+    if (rc) return rc;
+    if (num_iter == 0) {                                    // the reference returns zeros (its llr_2i starts at 0)
+        SB_CUDA(cudaMemsetAsync(d_out, 0, (size_t)batch * k * sizeof(float), (cudaStream_t)stream));
+        return SB_OK;
+    }
+    auto* ph = const_cast<sb_turbo_perm*>(perm);
+    rc = ensure_uploaded(ph);
+    if (rc) return rc;
+    const long long per_cta = kWarps * p.w.G;
+    const long long rows = (batch + per_cta - 1) / per_cta * per_cta;
+    float* ws_alpha = (float*)d_workspace;
+    float* ws_ext = (float*)d_workspace + (p.w.on_chip ? 0 : (size_t)rows * T * ns);
+    const size_t smem = kWarps * (p.w.table_bytes + (p.w.on_chip ? p.w.state_bytes : 0) +
+                                  (p.ext_on_chip ? p.ext_bytes : 0));
+    const unsigned grid = (unsigned)(rows / per_cta);
+    return dispatch_states(ns, [&](auto LC, auto RC) {
+        constexpr int L = decltype(LC)::value, RR = decltype(RC)::value;
+        auto kern = algorithm == 2 ? turbo_kernel<L, RR, true> : turbo_kernel<L, RR, false>;
+        if (smem > 48 * 1024) SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        kern<<<grid, kWarps * 32, smem, (cudaStream_t)stream>>>(d_llr, ph->d, d_out, ws_alpha, ws_ext, batch, k, T,
+                                                                 num_iter, terminate, hard_out, p.w.ch, p.w.tw,
+                                                                 p.w.on_chip, p.ext_on_chip, tr);
         SB_LAUNCH_CHECK();
         return SB_OK;
     });

@@ -1,7 +1,9 @@
-"""Forward error correction (mirror of sionna.phy.fec): LDPC and convolutional codes, CRC, scrambling and test
-utilities."""
+"""Forward error correction (mirror of sionna.phy.fec): LDPC, convolutional and turbo codes, interleavers, CRC,
+scrambling and test utilities."""
 from . import ldpc
 from . import conv
+from . import interleaving
+from . import turbo
 from . import utils
 from . import crc
 from . import scrambling
