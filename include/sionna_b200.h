@@ -644,6 +644,29 @@ int sb_turbo_decode(const float* d_llr, const sb_turbo_perm* perm, float* d_out,
  * does not fit in shared memory; 0 when both do. */
 size_t sb_turbo_workspace_bytes(int64_t batch, int32_t k, int32_t terminate, int32_t ns);
 
+/* ------------------------------------------------------------------------------------------------
+ * Binary linear block codes (csrc/linear_codes.cu)
+ * replaces LinearEncoder.call                    fec/linear/encoding.py:122-140
+ *          OSDecoder.call / _find_mrb / _find_min_dist   fec/linear/decoding.py:237-478
+ * ---------------------------------------------------------------------------------------------- */
+/* c = u G mod 2. d_u [batch, k] and d_c [batch, n] of one dtype: 0 float32, 1 float64, 2 int32, 3 int64; an input
+ * element contributes bit (long long)u & 1. d_gen_rows: G as k bit-packed rows of ceil(n / 32) words, bit b of word w
+ * = column 32 w + b. Any 1 <= k <= n. batch = 0 is SB_OK with NULL pointers. */
+int sb_gf2_encode(const void* d_u, void* d_c, int32_t dtype, int64_t batch, int32_t k, int32_t n,
+                  const uint32_t* d_gen_rows, void* stream);
+typedef struct sb_osd_code sb_osd_code;
+/* h_gm [k, n] (uint8, 0 / 1): the generator matrix, checked on the host to be binary (SB_EINVAL) and of full rank
+ * (SB_EINVAL); n > 1024 is SB_EUNSUPPORTED. Uploaded on first use on each device. */
+int sb_osd_code_create(sb_osd_code** out, const uint8_t* h_gm, int32_t k, int32_t n);
+void sb_osd_code_destroy(sb_osd_code* p);
+/* Ordered statistics decoding of order t (t > k acts as t = k, i.e. exact ML): d_llr [batch, n] logits
+ * log p(1) / p(0), clipped to +-100; d_out [batch, n] the hard decisions (0.0 / 1.0) of the best candidate by the
+ * discrepancy sum over mismatched positions of |llr| (equal to the reference's metric's order). Ties keep the first
+ * candidate in (order, itertools.combinations rank over the most reliable basis in reliability order). More than
+ * 2^62 candidates, or tables that exceed shared memory, is SB_EUNSUPPORTED. All checks run before any device
+ * access; batch = 0 is SB_OK with NULL pointers. */
+int sb_osd_decode(const sb_osd_code* code, const float* d_llr, float* d_out, int64_t batch, int32_t t, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

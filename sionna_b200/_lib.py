@@ -96,6 +96,10 @@ SIGNATURES = {
     "sb_turbo_perm_destroy": (None, [vp]),
     "sb_turbo_decode": (i32, [vp, vp, vp, i64, i32, i32, i32, i32, i32, vp, vp, vp, i32, i32, vp, sz, vp]),
     "sb_turbo_workspace_bytes": (sz, [i64, i32, i32, i32]),
+    "sb_gf2_encode": (i32, [vp, vp, i32, i64, i32, i32, vp, vp]),
+    "sb_osd_code_create": (i32, [C.POINTER(vp), vp, i32, i32]),
+    "sb_osd_code_destroy": (None, [vp]),
+    "sb_osd_decode": (i32, [vp, vp, vp, i64, i32, vp]),
 }
 
 

@@ -20,7 +20,7 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 LIB = os.path.join(HERE, "..", "libsionna_b200.so")
 OBJ_DIR = os.path.join(HERE, "..", "..", "build", "obj")
 EXACT = ["common.cu", "ldpc_bp.cu", "ldpc_bp_qc.cu", "ldpc_bp_flat.cu", "ldpc_enc.cu", "phy_kernels.cu",
-         "flat_fading.cu", "conv.cu"]                                                                        # -fmad=false
+         "flat_fading.cu", "conv.cu", "linear_codes.cu"]                                         # -fmad=false
 FAST = ["ofdm_mimo.cu", "channel.cu", "frontend.cu", "mimo_ml.cu", "mimo_kbest.cu",
         "mimo_iterative.cu", "precoding.cu"]                                                     # -fmad=true
 SOURCES = EXACT + FAST

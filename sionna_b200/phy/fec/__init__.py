@@ -1,6 +1,7 @@
-"""Forward error correction (mirror of sionna.phy.fec): LDPC, convolutional and turbo codes, interleavers, CRC,
-scrambling and test utilities."""
+"""Forward error correction (mirror of sionna.phy.fec): LDPC, convolutional, turbo and generic linear block codes,
+interleavers, CRC, scrambling and test utilities."""
 from . import ldpc
+from . import linear
 from . import conv
 from . import interleaving
 from . import turbo
