@@ -13,8 +13,9 @@
  *   - every function returns 0 on success or a negative SB_E* code; `sb_last_error()` returns a
  *     thread-local human-readable message for the last failure on the calling thread.
  *   - outputs and workspaces are allocated by the caller; no function synchronises the stream or
- *     allocates device memory, except `*_create` (device copies of index tables owned by the handle,
- *     released by `*_destroy`).
+ *     allocates device memory, except that the first call using a handle on a device copies the
+ *     handle's tables there (one copy per device, kept until `*_destroy` frees them all). That is the
+ *     library's only device allocation and only synchronous copy.
  *   - all pointers named `d_*` are device pointers, `h_*` host pointers.
  *   - real tensors are fp32, complex tensors interleaved (re, im) fp32 ("single" precision).
  */
@@ -66,6 +67,7 @@ enum { SB_VN_SUM = 0, SB_VN_IDENTITY = 1 };
  *       NULL = identity (n_out must equal num_vn).
  *   h_schedule [n_sub * n_active] or NULL: CN indices updated in each sub-iteration
  *       (`cn_schedule`, decoding.py:253-271, 464-497). NULL = flooding.
+ * The graph's tables are copied to a device by the first decode there.
  */
 int sb_ldpc_graph_create(sb_ldpc_graph** out, int32_t num_cn, int32_t num_vn, int32_t num_edges,
                          const int32_t* h_cn_of_edge, const int32_t* h_vn_of_edge,
@@ -88,8 +90,9 @@ void sb_ldpc_graph_destroy(sb_ldpc_graph* g);
 /* Optional: declare the graph quasi-cyclic (lifted base graph, fec/ldpc/encoding.py:322-352): n_entries base entries
  * (h_base_row, h_base_col, h_shift) with lifting size Z, meaning CN r*Z+i is connected to VN c*Z+(i+s) mod Z. Entries
  * beyond the (possibly pruned) graph are ignored. The description is verified against the edge list given at
- * creation (SB_EINVAL on mismatch, handle unchanged). Qualifying decodes (flooding, "sum" VN rule, no input state,
- * graph fits in shared memory) then run the index-free QC kernel; results are identical either way. */
+ * creation (SB_EINVAL on mismatch, handle unchanged); a new description drops the device copies of the previous one.
+ * Qualifying decodes (flooding, "sum" VN rule, no input state, graph fits in shared memory) then run the index-free
+ * QC kernel; results are identical either way. */
 int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entries, const int32_t* h_base_row,
                          const int32_t* h_base_col, const int32_t* h_shift);
 int sb_ldpc_graph_is_qc(const sb_ldpc_graph* g);
@@ -97,9 +100,11 @@ int sb_ldpc_graph_is_qc(const sb_ldpc_graph* g);
  * (n even); both must equal the CPU oracle bit for bit. */
 int sb_debug_phi(const float* d_x, float* d_scalar, float* d_packed, int64_t n, void* stream);
 /* 1 if one codeword's messages + channel LLRs fit in one SM's shared memory (the on-chip path),
- * 0 if the decoder will keep messages in an L2-resident global workspace. */
+ * 0 if the decoder will keep messages in an L2-resident global workspace. Judged for the current device once the graph
+ * has decoded there, else for an H100. */
 int sb_ldpc_graph_on_chip(const sb_ldpc_graph* g);
-/* Bytes of device workspace `sb_ldpc_decode` needs for this graph (0 on the on-chip path). */
+/* Bytes of device workspace `sb_ldpc_decode` needs for this graph (0 on the on-chip path), on the same device as
+ * sb_ldpc_graph_on_chip. */
 size_t sb_ldpc_workspace_bytes(const sb_ldpc_graph* g);
 /* Test hook (no device needed): copies the host-side plan into caller arrays; any pointer may be NULL.
  * dims[10] = {C, N, E, Lc, Lv, n_in, n_out, n_sub, n_active, flooding}; cn_order[C], vn_order[N], slot_of_edge[E],
@@ -163,7 +168,7 @@ typedef struct sb_ldpc5g_encoder sb_ldpc5g_encoder;
  * parity-check matrix H = [[A B 0],[C1 C2 I]] (encoding.py:411-434): A [g_rows x k_ldpc], B^-1 [g_rows x g_rows],
  * C1 [(n_ldpc-k_ldpc-g_rows) x k_ldpc], C2 [same rows x g_rows]; h_tx_vn[n]: index into the n_ldpc-bit codeword
  * [s | p_a | p_b] transmitted at output position j (filler removal, 2Z puncturing, truncation, interleaver of
- * encoding.py:645-661 folded into one gather). */
+ * encoding.py:645-661 folded into one gather). The tables are copied to a device by the first encode there. */
 int sb_ldpc5g_encoder_create(sb_ldpc5g_encoder** out, int32_t k, int32_t n, int32_t k_ldpc, int32_t n_ldpc,
                              int32_t g_rows, const int32_t* h_a_ptr, const int32_t* h_a_idx,
                              const int32_t* h_binv_ptr, const int32_t* h_binv_idx, const int32_t* h_c1_ptr,
@@ -625,7 +630,7 @@ size_t sb_bcjr_workspace_bytes(int64_t batch, int32_t num_syms, int32_t ns);
 typedef struct sb_turbo_perm sb_turbo_perm;
 /* The interleaver pi (Turbo3GPPInterleaver / RandomInterleaver, fec/interleaving.py:197-745): h_perm [k], decoder 2
  * sees u[pi(i)] at step i. Returns SB_EINVAL unless h_perm is a permutation of 0 ... k - 1; checked on the host
- * before any device access. The table is uploaded on first use on each device. */
+ * before any device access. The table is copied to a device by the first decode there. */
 int sb_turbo_perm_create(sb_turbo_perm** out, const int32_t* h_perm, int32_t k);
 void sb_turbo_perm_destroy(sb_turbo_perm* p);
 /* TurboDecoder: d_llr [batch, 2, 2 T] logits (Sionna's sign) of the two component codewords, T = k + (terminate ?
@@ -656,7 +661,7 @@ int sb_gf2_encode(const void* d_u, void* d_c, int32_t dtype, int64_t batch, int3
                   const uint32_t* d_gen_rows, void* stream);
 typedef struct sb_osd_code sb_osd_code;
 /* h_gm [k, n] (uint8, 0 / 1): the generator matrix, checked on the host to be binary (SB_EINVAL) and of full rank
- * (SB_EINVAL); n > 1024 is SB_EUNSUPPORTED. Uploaded on first use on each device. */
+ * (SB_EINVAL); n > 1024 is SB_EUNSUPPORTED. The generator is copied to a device by the first decode there. */
 int sb_osd_code_create(sb_osd_code** out, const uint8_t* h_gm, int32_t k, int32_t n);
 void sb_osd_code_destroy(sb_osd_code* p);
 /* Ordered statistics decoding of order t (t > k acts as t = k, i.e. exact ML): d_llr [batch, n] logits

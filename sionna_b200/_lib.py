@@ -140,6 +140,26 @@ def check(status, what=""):
         raise err(f"{what} failed with status {status}: {msg}")
 
 
+class Handle:
+    """Owns one C-ABI handle of type ``sb_<kind>``: created by ``sb_<kind>_create(&h, *args)`` (or by the constructor
+    named ``create``) and destroyed once, by ``sb_<kind>_destroy``, when the owner is collected."""
+
+    def __init__(self, kind, *args, create=None):
+        name = create or f"sb_{kind}_create"
+        h = C.c_void_p()
+        check(getattr(lib(), name)(C.byref(h), *args), name)
+        self.handle = h
+        self._destroy = getattr(lib(), f"sb_{kind}_destroy")
+
+    def __del__(self):
+        destroy, self._destroy = getattr(self, "_destroy", None), None
+        if destroy is not None:
+            try:
+                destroy(self.handle)
+            except Exception:  # interpreter shutdown
+                pass
+
+
 def ptr(t):
     """Device (or host) pointer of a torch tensor / numpy array as c_void_p; None -> NULL."""
     if t is None:

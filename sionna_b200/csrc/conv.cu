@@ -639,13 +639,12 @@ extern "C" int sb_bcjr_decode(const float* d_llr_ch, const float* d_llr_a, float
 }
 
 // ---- turbo decoder (host) -------------------------------------------------------------------------------------------
-// The interleaver pi of a turbo code, checked on the host at creation; uploaded on first use per device, as
-// sb_ldpc5g_encoder does, so that the kernel only ever reads validated indices.
+// The interleaver pi of a turbo code, checked on the host at creation, so that the kernel only ever reads validated
+// indices.
 struct sb_turbo_perm {
     int k = 0;
     std::vector<int32_t> h;
-    int device = -1;
-    int32_t* d = nullptr;
+    mutable DeviceTables tables;   // device copies of h
 };
 
 namespace {
@@ -667,18 +666,6 @@ TurboPlan turbo_plan(int ns, int k, int T) {
 
 int turbo_syms(int k, int terminate, int ns) { return k + (terminate ? 31 - __builtin_clz((unsigned)ns) : 0); }
 
-int ensure_uploaded(sb_turbo_perm* p) {
-    int dev = 0;
-    SB_CUDA(cudaGetDevice(&dev));
-    if (p->d && p->device == dev) return SB_OK;
-    if (p->d) cudaFree(p->d);
-    p->d = nullptr;
-    SB_CUDA(cudaMalloc((void**)&p->d, p->h.size() * sizeof(int32_t)));
-    SB_CUDA(cudaMemcpy(p->d, p->h.data(), p->h.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
-    p->device = dev;
-    return SB_OK;
-}
-
 }  // namespace
 
 extern "C" int sb_turbo_perm_create(sb_turbo_perm** out, const int32_t* h_perm, int32_t k) {
@@ -694,15 +681,12 @@ extern "C" int sb_turbo_perm_create(sb_turbo_perm** out, const int32_t* h_perm, 
     auto* p = new sb_turbo_perm();
     p->k = k;
     p->h.assign(h_perm, h_perm + k);
+    p->tables.set(p->h);
     *out = p;
     return SB_OK;
 }
 
-extern "C" void sb_turbo_perm_destroy(sb_turbo_perm* p) {
-    if (!p) return;
-    if (p->d) cudaFree(p->d);
-    delete p;
-}
+extern "C" void sb_turbo_perm_destroy(sb_turbo_perm* p) { delete p; }
 
 extern "C" size_t sb_turbo_workspace_bytes(int64_t batch, int32_t k, int32_t terminate, int32_t ns) {
     if (batch < 0 || k < 1 || ns < 2 || ns > kMaxStates || (ns & (ns - 1)) || (terminate != 0 && terminate != 1))
@@ -746,8 +730,8 @@ extern "C" int sb_turbo_decode(const float* d_llr, const sb_turbo_perm* perm, fl
         SB_CUDA(cudaMemsetAsync(d_out, 0, (size_t)batch * k * sizeof(float), (cudaStream_t)stream));
         return SB_OK;
     }
-    auto* ph = const_cast<sb_turbo_perm*>(perm);
-    rc = ensure_uploaded(ph);
+    const DeviceTables::Copy* d = nullptr;
+    rc = perm->tables.get(&d);
     if (rc) return rc;
     const long long per_cta = kWarps * p.w.G;
     const long long rows = (batch + per_cta - 1) / per_cta * per_cta;
@@ -760,8 +744,8 @@ extern "C" int sb_turbo_decode(const float* d_llr, const sb_turbo_perm* perm, fl
         constexpr int L = decltype(LC)::value, RR = decltype(RC)::value;
         auto kern = algorithm == 2 ? turbo_kernel<L, RR, true> : turbo_kernel<L, RR, false>;
         if (smem > 48 * 1024) SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, kWarps * 32, smem, (cudaStream_t)stream>>>(d_llr, ph->d, d_out, ws_alpha, ws_ext, batch, k, T,
-                                                                 num_iter, terminate, hard_out, p.w.ch, p.w.tw,
+        kern<<<grid, kWarps * 32, smem, (cudaStream_t)stream>>>(d_llr, d->at<int32_t>(0), d_out, ws_alpha, ws_ext, batch,
+                                                                 k, T, num_iter, terminate, hard_out, p.w.ch, p.w.tw,
                                                                  p.w.on_chip, p.ext_on_chip, tr);
         SB_LAUNCH_CHECK();
         return SB_OK;

@@ -195,7 +195,7 @@ __global__ void __launch_bounds__(1024, 1) ldpc_bp_kernel(const __grid_constant_
 }  // namespace
 
 // ------------------------------------------------------------------------------------------------------
-// Host side: graph plan (pure host), lazy upload, launch.
+// Host side: graph plan (pure host), launch.
 // ------------------------------------------------------------------------------------------------------
 
 static size_t bp_smem_bytes(const sb_ldpc_graph* g, bool smem_msgs) {
@@ -313,6 +313,9 @@ static int graph_create_impl(sb_ldpc_graph** out, int32_t num_cn, int32_t num_vn
     } else {
         g->flooding = true; g->n_sub = 1; g->n_active = C;
     }
+    g->vn_slot16.assign(g->vn_slot.begin(), g->vn_slot.end());
+    g->tables.set(g->cn_off, g->cn_cnt, g->vn_off, g->vn_cnt, g->in_idx, g->out_pos, g->slot_of_edge, g->sched, g->vn_slot,
+                  g->vn_slot16);
     *out = g;
     return SB_OK;
 }
@@ -334,62 +337,33 @@ extern "C" int sb_ldpc_graph_create_ordered(sb_ldpc_graph** out, int32_t num_cn,
                              n_active, h_cn_view);
 }
 
-static void free_device(sb_ldpc_graph* g) {
-    if (!g->uploaded) return;
-    cudaFree(g->d_cn_off); cudaFree(g->d_cn_cnt); cudaFree(g->d_vn_off); cudaFree(g->d_vn_cnt); cudaFree(g->d_in_idx);
-    cudaFree(g->d_out_pos); cudaFree(g->d_slot_of_edge); cudaFree(g->d_sched); cudaFree(g->d_vn_slot16); cudaFree(g->d_vn_slot32);
-    g->uploaded = false;
-}
-
-extern "C" void sb_ldpc_graph_destroy(sb_ldpc_graph* g) {
-    if (!g) return;
-    free_device(g);
-    sb_qc_free_device(g);
-    delete g;
-}
-
-static int ensure_uploaded(sb_ldpc_graph* g) {
-    int dev = 0;
-    SB_CUDA(cudaGetDevice(&dev));
-    if (g->uploaded && g->device == dev) return SB_OK;
-    free_device(g);
-    int rc;
-    if ((rc = sb_upload(&g->d_cn_off, g->cn_off))) return rc;
-    if ((rc = sb_upload(&g->d_cn_cnt, g->cn_cnt))) return rc;
-    if ((rc = sb_upload(&g->d_vn_off, g->vn_off))) return rc;
-    if ((rc = sb_upload(&g->d_vn_cnt, g->vn_cnt))) return rc;
-    if ((rc = sb_upload(&g->d_in_idx, g->in_idx))) return rc;
-    if ((rc = sb_upload(&g->d_out_pos, g->out_pos))) return rc;
-    if ((rc = sb_upload(&g->d_slot_of_edge, g->slot_of_edge))) return rc;
-    if ((rc = sb_upload(&g->d_sched, g->sched))) return rc;
-    if ((rc = sb_upload(&g->d_vn_slot32, g->vn_slot))) return rc;
-    std::vector<uint16_t> s16(g->vn_slot.size());
-    for (size_t i = 0; i < s16.size(); ++i) s16[i] = (uint16_t)g->vn_slot[i];
-    if ((rc = sb_upload(&g->d_vn_slot16, s16))) return rc;
-    SB_CUDA(cudaDeviceGetAttribute(&g->smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    SB_CUDA(cudaDeviceGetAttribute(&g->num_sms, cudaDevAttrMultiProcessorCount, dev));
-    g->uploaded = true;
-    g->device = dev;
-    return SB_OK;
-}
-
+extern "C" void sb_ldpc_graph_destroy(sb_ldpc_graph* g) { delete g; }
 
 static bool graph_on_chip(const sb_ldpc_graph* g, int smem_optin) {
     return g->E <= 65535 && bp_smem_bytes(g, true) <= (size_t)smem_optin;
 }
 
+// The current device's opt-in shared memory once the graph has been used there, else the H100's.
+static int planning_smem_optin(const sb_ldpc_graph* g) {
+    const DeviceTables::Copy* d = g->tables.find();
+    return d ? d->smem_optin : kSmemOptinH100;
+}
+
 extern "C" int sb_ldpc_graph_on_chip(const sb_ldpc_graph* g) {
     if (!g) return 0;
-    return graph_on_chip(g, g->uploaded ? g->smem_optin : kSmemOptinH100) ? 1 : 0;
+    return graph_on_chip(g, planning_smem_optin(g)) ? 1 : 0;
 }
 
 // upper bound on resident CTAs the launcher will ever use (grid is capped to it)
 static const int kMaxGrid = 132 * 8;
 
-extern "C" size_t sb_ldpc_workspace_bytes(const sb_ldpc_graph* g) {
-    if (!g) return 0;
-    if (graph_on_chip(g, g->uploaded ? g->smem_optin : kSmemOptinH100)) return 0;
+static size_t workspace_bytes(const sb_ldpc_graph* g, int smem_optin) {
+    if (graph_on_chip(g, smem_optin)) return 0;
     return (size_t)kMaxGrid * (g->flooding ? 1 : 2) * (size_t)g->E * sizeof(float);
+}
+
+extern "C" size_t sb_ldpc_workspace_bytes(const sb_ldpc_graph* g) {
+    return g ? workspace_bytes(g, planning_smem_optin(g)) : 0;
 }
 
 static int pick_threads(const sb_ldpc_graph* g) {
@@ -405,7 +379,7 @@ static int pick_threads(const sb_ldpc_graph* g) {
     return best;
 }
 
-static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t batch, int32_t num_iter, int32_t cn_rule,
+static int ldpc_decode_impl(const sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_t num_iter, int32_t cn_rule,
                             int32_t vn_rule, float offset, float llr_max, int32_t hard_out, const float* d_state_in,
                             float* d_state_out, float* d_out, void* d_ws, size_t ws_bytes, void* stream, int32_t early,
                             int32_t* d_iters);
@@ -425,22 +399,22 @@ extern "C" int sb_ldpc_decode_early(const sb_ldpc_graph* gc, const float* d_llr,
                             nullptr, 0, stream, 1, d_num_iter);
 }
 
-static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t batch, int32_t num_iter, int32_t cn_rule,
+static int ldpc_decode_impl(const sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_t num_iter, int32_t cn_rule,
                             int32_t vn_rule, float offset, float llr_max, int32_t hard_out, const float* d_state_in,
                             float* d_state_out, float* d_out, void* d_ws, size_t ws_bytes, void* stream, int32_t early,
                             int32_t* d_iters) {
     if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(gc && d_llr && d_out, "sb_ldpc_decode: null graph/input/output");
+    SB_CHECK_ARG(g && d_llr && d_out, "sb_ldpc_decode: null graph/input/output");
     SB_CHECK_ARG(batch >= 0 && num_iter >= 0, "sb_ldpc_decode: negative batch or num_iter");
     SB_CHECK_ARG(cn_rule >= SB_CN_BOXPLUS_PHI && cn_rule <= SB_CN_IDENTITY, "sb_ldpc_decode: unknown cn_rule %d", cn_rule);
     SB_CHECK_ARG(vn_rule == SB_VN_SUM || vn_rule == SB_VN_IDENTITY, "sb_ldpc_decode: unknown vn_rule %d", vn_rule);
     SB_CHECK_ARG(llr_max >= 0.f, "sb_ldpc_decode: llr_max must be >= 0");
-    auto* g = const_cast<sb_ldpc_graph*>(gc);
-    int rc = ensure_uploaded(g);
+    const DeviceTables::Copy* d = nullptr;
+    int rc = g->tables.get(&d);
     if (rc) return rc;
     {   // quasi-cyclic fast path (ldpc_bp_qc.cu) when the graph carries a QC description and the call qualifies
         bool handled = false;
-        rc = sb_qc_try_decode(g, d_llr, batch, num_iter, cn_rule, vn_rule, offset, llr_max, hard_out, d_state_in,
+        rc = sb_qc_try_decode(g, *d, d_llr, batch, num_iter, cn_rule, vn_rule, offset, llr_max, hard_out, d_state_in,
                               d_state_out, d_out, (cudaStream_t)stream, &handled, early, d_iters);
         if (rc || handled) return rc;
     }
@@ -448,13 +422,13 @@ static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t
         sb_set_error("sb_ldpc_decode_early: early termination needs the quasi-cyclic on-chip path (5G codes, flooding)");
         return SB_EUNSUPPORTED;
     }
-    const bool on_chip = graph_on_chip(g, g->smem_optin);
+    const bool on_chip = graph_on_chip(g, d->smem_optin);
     BpParams p{};
     p.C = g->C; p.N = g->N; p.E = g->E; p.Lc = g->Lc; p.Lv = g->Lv;
-    p.cn_off = g->d_cn_off; p.cn_cnt = g->d_cn_cnt; p.vn_off = g->d_vn_off; p.vn_cnt = g->d_vn_cnt;
-    p.vn_slot = on_chip ? (const void*)g->d_vn_slot16 : (const void*)g->d_vn_slot32;
-    p.in_idx = g->d_in_idx; p.out_pos = g->d_out_pos; p.slot_of_edge = g->d_slot_of_edge;
-    p.sched = g->flooding ? nullptr : g->d_sched;
+    p.cn_off = d->at<int>(0); p.cn_cnt = d->at<int>(1); p.vn_off = d->at<int>(2); p.vn_cnt = d->at<int>(3);
+    p.vn_slot = on_chip ? (const void*)d->at<uint16_t>(9) : (const void*)d->at<uint32_t>(8);
+    p.in_idx = d->at<int>(4); p.out_pos = d->at<int>(5); p.slot_of_edge = d->at<int>(6);
+    p.sched = g->flooding ? nullptr : d->at<int>(7);
     p.n_sub = g->n_sub; p.n_active = g->n_active; p.n_in = g->n_in; p.n_out = g->n_out;
     p.llr = d_llr; p.out = d_out; p.state_in = d_state_in; p.state_out = d_state_out;
     p.B = batch; p.num_iter = num_iter; p.vn_rule = vn_rule; p.hard_out = hard_out;
@@ -465,15 +439,15 @@ static int ldpc_decode_impl(const sb_ldpc_graph* gc, const float* d_llr, int64_t
     p.ws = (float*)d_ws;
     p.use_tma = on_chip && (g->n_in % 4 == 0) && (g->n_in <= g->E) && ((reinterpret_cast<uintptr_t>(d_llr) & 15) == 0);
     if (!on_chip) {
-        size_t need = sb_ldpc_workspace_bytes(g);
+        size_t need = workspace_bytes(g, d->smem_optin);
         if (!d_ws || ws_bytes < need) { sb_set_error("sb_ldpc_decode: workspace %zu < %zu bytes", ws_bytes, need); return SB_ENOMEM; }
     }
     const int threads = pick_threads(g);
     const size_t smem = bp_smem_bytes(g, on_chip);
     cudaStream_t st = (cudaStream_t)stream;
     return sb_dispatch<SB_CN_BOXPLUS_PHI, SB_CN_IDENTITY>(cn_rule, [&](auto R) {
-        return sb_launch_decoder(on_chip ? ldpc_bp_kernel<R, true> : ldpc_bp_kernel<R, false>, p, g, threads, smem,
-                                 kMaxGrid, st, "sb_ldpc_decode");
+        return sb_launch_decoder(on_chip ? ldpc_bp_kernel<R, true> : ldpc_bp_kernel<R, false>, p, d->num_sms, threads,
+                                 smem, kMaxGrid, st, "sb_ldpc_decode");
     });
 }
 

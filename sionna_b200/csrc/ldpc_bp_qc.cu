@@ -822,38 +822,17 @@ size_t qc_smem_bytes(const sb_ldpc_graph* g, int tab_rep, int early = 0) {
            (size_t)g->qc_nnz * 8 + 16 + 16 + (size_t)tab_rep * SB_LOGTAB_N * 8;
 }
 
-int qc_ensure_uploaded(sb_ldpc_graph* g) {
-    if (g->qc_uploaded) return SB_OK;
-    int rc;
-    if ((rc = sb_upload(&g->d_qc_row_info, g->qc_row_info))) return rc;
-    if ((rc = sb_upload(&g->d_qc_col_info, g->qc_col_info))) return rc;
-    if ((rc = sb_upload(&g->d_qc_col_edge, g->qc_col_edge))) return rc;
-    if ((rc = sb_upload(&g->d_qc_in_idx, g->qc_in_idx))) return rc;
-    if ((rc = sb_upload(&g->d_qc_out_pos, g->qc_out_pos))) return rc;
-    if ((rc = sb_upload(&g->d_qc_slot_of_edge, g->qc_slot_of_edge))) return rc;
-    if ((rc = sb_upload(&g->d_qc_row_edge, g->qc_row_edge))) return rc;
-    g->qc_uploaded = true;
-    return SB_OK;
-}
-
 template <int RULE, bool EARLY>
-int launch_qc(const sb_ldpc_graph* g, const QcParams& p, int threads, size_t smem, cudaStream_t stream) {
+int launch_qc(const QcParams& p, int num_sms, int threads, size_t smem, cudaStream_t stream) {
     auto kern = ldpc_bp_qc_kernel<RULE, 16, EARLY>;
     if constexpr (RULE == SB_CN_BOXPLUS_PHI) {
         if (p.tab_rep == 8) kern = ldpc_bp_qc_kernel<RULE, 8, EARLY>;
         if (p.tab_rep == 1) kern = ldpc_bp_qc_kernel<RULE, 1, EARLY>;
     }
-    return sb_launch_decoder(kern, p, g, threads, smem, LLONG_MAX, stream, "sb_ldpc_decode(qc)");
+    return sb_launch_decoder(kern, p, num_sms, threads, smem, LLONG_MAX, stream, "sb_ldpc_decode(qc)");
 }
 
 }  // namespace
-
-void sb_qc_free_device(sb_ldpc_graph* g) {
-    if (!g->qc_uploaded) return;
-    cudaFree(g->d_qc_row_info); cudaFree(g->d_qc_col_info); cudaFree(g->d_qc_col_edge); cudaFree(g->d_qc_in_idx);
-    cudaFree(g->d_qc_out_pos); cudaFree(g->d_qc_slot_of_edge); cudaFree(g->d_qc_row_edge);
-    g->qc_uploaded = false;
-}
 
 // Attach the quasi-cyclic description of the graph: base entries (row, col, shift) of the lifted matrix with lifting
 // size Z; entries outside ceil(C/Z) x ceil(N/Z) are ignored (pruned away). The description is verified against the
@@ -1000,13 +979,14 @@ extern "C" int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entri
         int r = g->h_cn[e] / Z, i = g->h_cn[e] % Z, c = g->h_vn[e] / Z;
         slot[e] = be_of[(size_t)r * n_cols + c] * Z + i;
     }
-    sb_qc_free_device(g);
     g->qc = true; g->qc_Z = Z; g->qc_rows = n_rows; g->qc_cols = n_cols; g->qc_nnz = nnz;
     g->qc_max_row_deg = *std::max_element(rdeg.begin(), rdeg.end());
     g->qc_max_col_deg = *std::max_element(cdeg.begin(), cdeg.end());
     g->qc_row_info.swap(row_info); g->qc_col_info.swap(col_info); g->qc_col_edge.swap(col_edge);
     g->qc_row_cls_end = row_cls_end; g->qc_col_cls_end = col_cls_end;
     g->qc_in_idx.swap(in_nat); g->qc_out_pos.swap(out_nat); g->qc_slot_of_edge.swap(slot); g->qc_row_edge.swap(row_edge);
+    g->qc_tables.set(g->qc_row_info, g->qc_col_info, g->qc_col_edge, g->qc_in_idx, g->qc_out_pos, g->qc_slot_of_edge,
+                     g->qc_row_edge);
     return SB_OK;
 }
 
@@ -1035,33 +1015,35 @@ extern "C" int sb_debug_phi(const float* d_x, float* d_scalar, float* d_packed, 
 
 extern "C" int sb_ldpc_graph_is_qc(const sb_ldpc_graph* g) { return g && g->qc ? 1 : 0; }
 
-int sb_qc_try_decode(sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_t num_iter, int32_t cn_rule,
-                     int32_t vn_rule, float offset, float llr_max, int32_t hard_out, const float* d_state_in,
-                     float* d_state_out, float* d_out, cudaStream_t stream, bool* handled, int32_t early, int32_t* d_iters) {
+int sb_qc_try_decode(const sb_ldpc_graph* g, const DeviceTables::Copy& dev, const float* d_llr, int64_t batch,
+                     int32_t num_iter, int32_t cn_rule, int32_t vn_rule, float offset, float llr_max, int32_t hard_out,
+                     const float* d_state_in, float* d_state_out, float* d_out, cudaStream_t stream, bool* handled,
+                     int32_t early, int32_t* d_iters) {
     *handled = false;
     if (!g->qc || !g->flooding || vn_rule != SB_VN_SUM || d_state_in || cn_rule > SB_CN_OFFSET_MINSUM) return SB_OK;
     // boxplus-phi keeps the log table of phi in shared memory: one copy per bank pair if it fits, else 8 copies or one
     int tab_rep = cn_rule == SB_CN_BOXPLUS_PHI ? 16 : 0;
-    if (tab_rep && qc_smem_bytes(g, tab_rep, early) > (size_t)g->smem_optin) tab_rep = 8;
-    if (tab_rep && qc_smem_bytes(g, tab_rep, early) > (size_t)g->smem_optin) tab_rep = 1;
+    if (tab_rep && qc_smem_bytes(g, tab_rep, early) > (size_t)dev.smem_optin) tab_rep = 8;
+    if (tab_rep && qc_smem_bytes(g, tab_rep, early) > (size_t)dev.smem_optin) tab_rep = 1;
     const size_t smem = qc_smem_bytes(g, tab_rep, early);
-    if (smem > (size_t)g->smem_optin) return SB_OK;
+    if (smem > (size_t)dev.smem_optin) return SB_OK;
     if ((cn_rule == SB_CN_MINSUM || cn_rule == SB_CN_OFFSET_MINSUM) &&
         !(llr_max < 100000.f && (float)(g->qc_max_row_deg - 1) * llr_max < 99000.f))
         return SB_OK;                                      // the generic kernel has the literal 1e5-sentinel path
-    int rc = qc_ensure_uploaded(g);
+    const DeviceTables::Copy* d = nullptr;
+    int rc = g->qc_tables.get(&d);
     if (rc) return rc;
     QcParams p{};
     p.Z = g->qc_Z; p.n_rows = g->qc_rows; p.n_cols = g->qc_cols; p.nnz = g->qc_nnz; p.N = g->N; p.E = g->E;
     p.E_alloc = g->qc_nnz * g->qc_Z; p.n_in = g->n_in; p.n_out = g->n_out;
     for (int k = 0; k < kRowClasses; ++k) p.row_cls_end[k] = g->qc_row_cls_end[k];
     for (int k = 0; k < kColClasses; ++k) p.col_cls_end[k] = g->qc_col_cls_end[k];
-    p.row_info = (const int4*)g->d_qc_row_info; p.col_info = (const int4*)g->d_qc_col_info;
-    p.col_edge = (const int2*)g->d_qc_col_edge; p.in_idx = g->d_qc_in_idx; p.out_pos = g->d_qc_out_pos;
-    p.slot_of_edge = g->d_qc_slot_of_edge;
+    p.row_info = d->at<int4>(0); p.col_info = d->at<int4>(1);
+    p.col_edge = d->at<int2>(2); p.in_idx = d->at<int>(3); p.out_pos = d->at<int>(4);
+    p.slot_of_edge = d->at<int>(5);
     p.llr = d_llr; p.out = d_out; p.state_out = d_state_out; p.B = batch; p.num_iter = num_iter; p.hard_out = hard_out;
     p.offset = offset; p.llr_max = llr_max; p.tab_rep = tab_rep;
-    p.early = early; p.iters_out = d_iters; p.row_edge = (const int2*)g->d_qc_row_edge;
+    p.early = early; p.iters_out = d_iters; p.row_edge = d->at<int2>(6);
     p.use_tma = (g->n_in % 4 == 0) && (g->n_in <= p.E_alloc) && ((reinterpret_cast<uintptr_t>(d_llr) & 15) == 0);
     const int Zb = (g->qc_Z + 31) / 32;                    // 32-lane slices per block row (<= 12 for Z <= 384)
     const int max_warps = kQcThreads / 32;
@@ -1070,7 +1052,8 @@ int sb_qc_try_decode(sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_
     for (int k = 0; k < kRowClasses; ++k) p.row_cls_mod[k] = (k ? g->qc_row_cls_end[k - 1] : 0) % groups;
     for (int k = 0; k < kColClasses; ++k) p.col_cls_mod[k] = (k ? g->qc_col_cls_end[k - 1] : 0) % groups;
     rc = sb_dispatch<SB_CN_BOXPLUS_PHI, SB_CN_OFFSET_MINSUM>(cn_rule, [&](auto R) {
-        return p.early ? launch_qc<R, true>(g, p, threads, smem, stream) : launch_qc<R, false>(g, p, threads, smem, stream);
+        return p.early ? launch_qc<R, true>(p, dev.num_sms, threads, smem, stream)
+                       : launch_qc<R, false>(p, dev.num_sms, threads, smem, stream);
     });
     *handled = (rc == SB_OK);
     return rc;

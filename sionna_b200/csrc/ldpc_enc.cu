@@ -16,11 +16,8 @@
 struct sb_ldpc5g_encoder {
     int k = 0, n = 0, k_ldpc = 0, n_ldpc = 0, g = 0, m_rest = 0;   // g = 4Z rows of A / B^-1, m_rest rows of C1|C2
     std::vector<int> a_ptr, a_idx, b_ptr, b_idx, c1_ptr, c1_idx, c2_ptr, c2_idx, tx_vn;
-    bool uploaded = false;
-    int device = -1;
-    int *d_a_ptr = nullptr, *d_a_idx = nullptr, *d_b_ptr = nullptr, *d_b_idx = nullptr, *d_c1_ptr = nullptr,
-        *d_c1_idx = nullptr, *d_c2_ptr = nullptr, *d_c2_idx = nullptr, *d_tx_vn = nullptr;
     int rows_needed = 0;   // number of p_b rows any transmitted bit depends on
+    mutable DeviceTables tables;   // device copies of the nine tables above, in that order
 };
 
 namespace {
@@ -81,41 +78,6 @@ __global__ void __launch_bounds__(512) ldpc5g_encode_kernel(const __grid_constan
     }
 }
 
-template <typename T>
-int upload_vec(T** dptr, const std::vector<T>& h) {
-    size_t n = h.size() ? h.size() : 1;
-    SB_CUDA(cudaMalloc((void**)dptr, n * sizeof(T)));
-    if (h.size()) SB_CUDA(cudaMemcpy(*dptr, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return SB_OK;
-}
-
-void free_dev(sb_ldpc5g_encoder* e) {
-    if (!e->uploaded) return;
-    cudaFree(e->d_a_ptr); cudaFree(e->d_a_idx); cudaFree(e->d_b_ptr); cudaFree(e->d_b_idx); cudaFree(e->d_c1_ptr);
-    cudaFree(e->d_c1_idx); cudaFree(e->d_c2_ptr); cudaFree(e->d_c2_idx); cudaFree(e->d_tx_vn);
-    e->uploaded = false;
-}
-
-int ensure_uploaded(sb_ldpc5g_encoder* e) {
-    int dev = 0;
-    SB_CUDA(cudaGetDevice(&dev));
-    if (e->uploaded && e->device == dev) return SB_OK;
-    free_dev(e);
-    int rc;
-    if ((rc = upload_vec(&e->d_a_ptr, e->a_ptr))) return rc;
-    if ((rc = upload_vec(&e->d_a_idx, e->a_idx))) return rc;
-    if ((rc = upload_vec(&e->d_b_ptr, e->b_ptr))) return rc;
-    if ((rc = upload_vec(&e->d_b_idx, e->b_idx))) return rc;
-    if ((rc = upload_vec(&e->d_c1_ptr, e->c1_ptr))) return rc;
-    if ((rc = upload_vec(&e->d_c1_idx, e->c1_idx))) return rc;
-    if ((rc = upload_vec(&e->d_c2_ptr, e->c2_ptr))) return rc;
-    if ((rc = upload_vec(&e->d_c2_idx, e->c2_idx))) return rc;
-    if ((rc = upload_vec(&e->d_tx_vn, e->tx_vn))) return rc;
-    e->uploaded = true;
-    e->device = dev;
-    return SB_OK;
-}
-
 bool check_csr(const int32_t* ptr, const int32_t* idx, int rows, int cols) {
     if (!ptr || ptr[0] != 0) return false;
     for (int r = 0; r < rows; ++r) if (ptr[r + 1] < ptr[r]) return false;
@@ -149,34 +111,31 @@ extern "C" int sb_ldpc5g_encoder_create(sb_ldpc5g_encoder** out, int32_t k, int3
         if (tx_vn[j] > max_vn) max_vn = tx_vn[j];
     }
     e->rows_needed = std::max(0, std::min(m_rest, max_vn + 1 - k_ldpc - g_rows));
+    e->tables.set(e->a_ptr, e->a_idx, e->b_ptr, e->b_idx, e->c1_ptr, e->c1_idx, e->c2_ptr, e->c2_idx, e->tx_vn);
     *out = e;
     return SB_OK;
 }
 
-extern "C" void sb_ldpc5g_encoder_destroy(sb_ldpc5g_encoder* e) {
-    if (!e) return;
-    free_dev(e);
-    delete e;
-}
+extern "C" void sb_ldpc5g_encoder_destroy(sb_ldpc5g_encoder* e) { delete e; }
 
-extern "C" int sb_ldpc5g_encode(const sb_ldpc5g_encoder* ec, const float* d_u, int64_t batch, float* d_c, void* stream) {
+extern "C" int sb_ldpc5g_encode(const sb_ldpc5g_encoder* e, const float* d_u, int64_t batch, float* d_c, void* stream) {
     if (batch == 0) return SB_OK;                         // empty batch: nothing to do, pointers may be null
-    SB_CHECK_ARG(ec && d_u && d_c && batch >= 0, "sb_ldpc5g_encode: bad arguments");
-    if (batch == 0) return SB_OK;
-    auto* e = const_cast<sb_ldpc5g_encoder*>(ec);
-    int rc = ensure_uploaded(e);
+    SB_CHECK_ARG(e && d_u && d_c && batch >= 0, "sb_ldpc5g_encode: bad arguments");
+    const DeviceTables::Copy* d = nullptr;
+    int rc = e->tables.get(&d);
     if (rc) return rc;
     EncParams p{};
     p.k = e->k; p.n = e->n; p.k_ldpc = e->k_ldpc; p.n_ldpc = e->n_ldpc; p.g = e->g; p.rows_needed = e->rows_needed;
-    p.a_ptr = e->d_a_ptr; p.a_idx = e->d_a_idx; p.b_ptr = e->d_b_ptr; p.b_idx = e->d_b_idx;
-    p.c1_ptr = e->d_c1_ptr; p.c1_idx = e->d_c1_idx; p.c2_ptr = e->d_c2_ptr; p.c2_idx = e->d_c2_idx; p.tx_vn = e->d_tx_vn;
+    p.a_ptr = d->at<int>(0); p.a_idx = d->at<int>(1); p.b_ptr = d->at<int>(2); p.b_idx = d->at<int>(3);
+    p.c1_ptr = d->at<int>(4); p.c1_idx = d->at<int>(5); p.c2_ptr = d->at<int>(6); p.c2_idx = d->at<int>(7);
+    p.tx_vn = d->at<int>(8);
     p.u = d_u; p.c = d_c; p.B = batch;
     size_t smem = 4 * ((size_t)e->n_ldpc + (size_t)e->g) + 16;
     SB_CUDA(cudaFuncSetAttribute(ldpc5g_encode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, ldpc5g_encode_kernel, 512, smem));
     if (occ < 1) occ = 1;
-    long long grid = std::min<long long>((batch + 31) / 32, (long long)sb_num_sms() * occ);
+    long long grid = std::min<long long>((batch + 31) / 32, (long long)d->num_sms * occ);
     ldpc5g_encode_kernel<<<(unsigned)grid, 512, smem, (cudaStream_t)stream>>>(p);
     SB_LAUNCH_CHECK();
     return SB_OK;

@@ -12,15 +12,10 @@ struct sb_ldpc_graph {
     bool ref_order = false;   // node sums follow the reference's list orders (sb_ldpc_graph_create_ordered)
     std::vector<int> cn_off, cn_cnt, vn_off, vn_cnt, in_idx, out_pos, slot_of_edge, sched, cn_order, vn_order;
     std::vector<uint32_t> vn_slot;
+    std::vector<uint16_t> vn_slot16;   // vn_slot for the on-chip kernel (E <= 65535)
     std::vector<int> h_cn, h_vn;   // the caller's edge list (reference VN order), kept for sb_ldpc_graph_set_qc
-    // device copies (lazy)
-    bool uploaded = false;
-    int device = -1;
-    int *d_cn_off = nullptr, *d_cn_cnt = nullptr, *d_vn_off = nullptr, *d_vn_cnt = nullptr, *d_in_idx = nullptr,
-        *d_out_pos = nullptr, *d_slot_of_edge = nullptr, *d_sched = nullptr;
-    uint16_t* d_vn_slot16 = nullptr;
-    uint32_t* d_vn_slot32 = nullptr;
-    int smem_optin = 0, num_sms = 0;
+    // device copies of cn_off, cn_cnt, vn_off, vn_cnt, in_idx, out_pos, slot_of_edge, sched, vn_slot, vn_slot16
+    mutable DeviceTables tables;
     // ---- quasi-cyclic description (optional, set by sb_ldpc_graph_set_qc; used by ldpc_bp_qc.cu) ----------
     bool qc = false;
     int qc_Z = 0, qc_rows = 0, qc_cols = 0, qc_nnz = 0, qc_max_row_deg = 0, qc_max_col_deg = 0;
@@ -30,40 +25,31 @@ struct sb_ldpc_graph {
     std::vector<int> qc_in_idx, qc_out_pos, qc_slot_of_edge;   // natural VN order / reference edge order
     std::vector<int> qc_row_edge;   // int2 per base entry (processing order): {column * Z, shift} for the syndrome pass
     std::vector<int> qc_row_cls_end, qc_col_cls_end;   // class boundaries in processing order (ldpc_bp_qc.cu)
-    int *d_qc_row_info = nullptr, *d_qc_col_info = nullptr, *d_qc_col_edge = nullptr, *d_qc_in_idx = nullptr,
-        *d_qc_out_pos = nullptr, *d_qc_slot_of_edge = nullptr, *d_qc_row_edge = nullptr;
-    bool qc_uploaded = false;
+    // device copies of qc_row_info, qc_col_info, qc_col_edge, qc_in_idx, qc_out_pos, qc_slot_of_edge, qc_row_edge
+    mutable DeviceTables qc_tables;
 };
 
 // H100 (sm_90) opt-in shared memory per block (227 KB); used for planning when no device is present.
 static const int kSmemOptinH100 = 232448;
 
-// ldpc_bp_qc.cu: runs the QC kernel if the graph / call qualifies; *handled tells the dispatcher.
-int sb_qc_try_decode(sb_ldpc_graph* g, const float* d_llr, int64_t batch, int32_t num_iter, int32_t cn_rule,
-                     int32_t vn_rule, float offset, float llr_max, int32_t hard_out, const float* d_state_in,
-                     float* d_state_out, float* d_out, cudaStream_t stream, bool* handled, int32_t early = 0,
-                     int32_t* d_iters = nullptr);
-void sb_qc_free_device(sb_ldpc_graph* g);
-
-// Device copy of a host table (at least one element, so that an empty table still gets a valid pointer).
-template <typename T>
-int sb_upload(T** d, const std::vector<T>& h) {
-    SB_CUDA(cudaMalloc((void**)d, std::max<size_t>(1, h.size()) * sizeof(T)));
-    if (h.size()) SB_CUDA(cudaMemcpy(*d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
-    return SB_OK;
-}
+// ldpc_bp_qc.cu: runs the QC kernel if the graph / call qualifies; *handled tells the dispatcher. `dev` is the
+// current device's copy of the generic tables.
+int sb_qc_try_decode(const sb_ldpc_graph* g, const DeviceTables::Copy& dev, const float* d_llr, int64_t batch,
+                     int32_t num_iter, int32_t cn_rule, int32_t vn_rule, float offset, float llr_max, int32_t hard_out,
+                     const float* d_state_in, float* d_state_out, float* d_out, cudaStream_t stream, bool* handled,
+                     int32_t early = 0, int32_t* d_iters = nullptr);
 
 #if defined(__CUDACC__)
 // Launch of a persistent decoder kernel: opts in to `smem` bytes of dynamic shared memory, checks that a CTA of
 // `threads` fits on an SM, and runs min(batch, resident CTAs, max_grid) CTAs that stride over the codewords.
 template <class Kernel, class Params>
-int sb_launch_decoder(Kernel kern, const Params& p, const sb_ldpc_graph* g, int threads, size_t smem, long long max_grid,
+int sb_launch_decoder(Kernel kern, const Params& p, int num_sms, int threads, size_t smem, long long max_grid,
                       cudaStream_t stream, const char* who) {
     SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int occ = 0;
     SB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, threads, smem));
     if (occ < 1) { sb_set_error("%s: kernel does not fit (threads %d, smem %zu)", who, threads, smem); return SB_EUNSUPPORTED; }
-    long long grid = std::min<long long>(p.B, std::min<long long>((long long)g->num_sms * occ, max_grid));
+    long long grid = std::min<long long>(p.B, std::min<long long>((long long)num_sms * occ, max_grid));
     kern<<<(unsigned)grid, threads, smem, stream>>>(p);
     SB_LAUNCH_CHECK();
     return SB_OK;

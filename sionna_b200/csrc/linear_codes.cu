@@ -33,8 +33,7 @@
 struct sb_osd_code {
     int k = 0, n = 0, wk = 0;
     std::vector<uint32_t> h;   // column-major: n columns of wk words, bit b of word q = G[32 q + b][column]
-    int device = -1;
-    uint32_t* d = nullptr;
+    mutable DeviceTables tables;   // device copies of h
 };
 
 namespace {
@@ -435,18 +434,6 @@ unsigned long long osd_candidates(int k, int t) {
     return sum;
 }
 
-int osd_upload(sb_osd_code* p) {
-    int dev = 0;
-    SB_CUDA(cudaGetDevice(&dev));
-    if (p->d && p->device == dev) return SB_OK;
-    if (p->d) cudaFree(p->d);
-    p->d = nullptr;
-    SB_CUDA(cudaMalloc((void**)&p->d, p->h.size() * sizeof(uint32_t)));
-    SB_CUDA(cudaMemcpy(p->d, p->h.data(), p->h.size() * sizeof(uint32_t), cudaMemcpyHostToDevice));
-    p->device = dev;
-    return SB_OK;
-}
-
 }  // namespace
 
 extern "C" int sb_gf2_encode(const void* d_u, void* d_c, int32_t dtype, int64_t batch, int32_t k, int32_t n,
@@ -507,15 +494,12 @@ extern "C" int sb_osd_code_create(sb_osd_code** out, const uint8_t* h_gm, int32_
     for (int r = 0; r < k; ++r)
         for (int c = 0; c < n; ++c)
             if (h_gm[(size_t)r * n + c]) p->h[(size_t)c * wk + r / 32] |= 1u << (r & 31);
+    p->tables.set(p->h);
     *out = p;
     return SB_OK;
 }
 
-extern "C" void sb_osd_code_destroy(sb_osd_code* p) {
-    if (!p) return;
-    if (p->d) cudaFree(p->d);
-    delete p;
-}
+extern "C" void sb_osd_code_destroy(sb_osd_code* p) { delete p; }
 
 extern "C" int sb_osd_decode(const sb_osd_code* code, const float* d_llr, float* d_out, int64_t batch, int32_t t,
                              void* stream) {
@@ -537,13 +521,14 @@ extern "C" int sb_osd_decode(const sb_osd_code* code, const float* d_llr, float*
     }
     if (batch == 0) return SB_OK;
     SB_CHECK_ARG(d_llr && d_out, "%s: missing input or output", who);
-    const int rc = osd_upload(const_cast<sb_osd_code*>(code));
+    const DeviceTables::Copy* d = nullptr;
+    const int rc = code->tables.get(&d);
     if (rc) return rc;
     const int grid = sb_grid(batch, 1, 16);
     return sb_dispatch<0, 5>(__builtin_ctz((unsigned)wp), [&](auto LW) {
         auto kern = osd_kernel<(1 << LW)>;
         if (smem > 48 * 1024) SB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        kern<<<grid, kOsdThreads, smem, (cudaStream_t)stream>>>(d_llr, d_out, code->d, batch, k, n, tt);
+        kern<<<grid, kOsdThreads, smem, (cudaStream_t)stream>>>(d_llr, d_out, d->at<uint32_t>(0), batch, k, n, tt);
         SB_LAUNCH_CHECK();
         return SB_OK;
     });

@@ -4,7 +4,10 @@
 #include <stdarg.h>
 #include <stdio.h>
 #include <algorithm>
+#include <memory>
+#include <mutex>
 #include <type_traits>
+#include <vector>
 #include "../../include/sionna_b200.h"
 
 // thread-local error message (defined in common.cu)
@@ -61,6 +64,87 @@ static inline int sb_dispatch(int v, F&& f) {
         return sb_dispatch<LO + 1, HI>(v, f);
     }
 }
+
+// Device copies of a handle's host tables, one per device that has used the handle. The first get() on a device
+// allocates and copies every table there: the library's only device allocation and synchronous copy. A copy never
+// changes once built, and all copies are freed together, by set() or by the destructor (the handle's *_destroy). So a
+// call on one device never frees tables that a kernel on another device may still read, and returning to a device does
+// not upload again. Handles hold the store as a `mutable` member, so that decode and encode calls take them const.
+class DeviceTables {
+  public:
+    struct Copy {
+        int device = -1, smem_optin = 0, num_sms = 0;
+        std::vector<void*> ptr;   // device copy of each table, in the order given to set()
+        template <typename T>
+        const T* at(size_t i) const { return static_cast<const T*>(ptr[i]); }
+    };
+    DeviceTables() = default;
+    DeviceTables(const DeviceTables&) = delete;
+    DeviceTables& operator=(const DeviceTables&) = delete;
+    ~DeviceTables() { set(); }
+
+    // Registers the handle's host tables, which must outlive the registration unchanged, and frees every device copy.
+    template <typename... T>
+    void set(const std::vector<T>&... h) {
+        std::lock_guard<std::mutex> lock(mu_);
+        for (const auto& c : copies_) free_copy(*c);
+        copies_.clear();
+        tables_ = {Table{h.data(), h.size() * sizeof(T)}...};
+    }
+
+    // The copy on the current device, built on first use. If an allocation or copy fails, whatever that attempt
+    // allocated is freed, nothing is recorded and SB_ECUDA is returned; the next call tries again.
+    int get(const Copy** out) {
+        int dev = 0;
+        SB_CUDA(cudaGetDevice(&dev));
+        std::lock_guard<std::mutex> lock(mu_);
+        if ((*out = lookup(dev))) return SB_OK;
+        auto c = std::make_unique<Copy>();
+        c->device = dev;
+        if (int rc = build(*c)) {
+            free_copy(*c);
+            return rc;
+        }
+        copies_.push_back(std::move(c));
+        *out = copies_.back().get();
+        return SB_OK;
+    }
+
+    // The copy on the current device if one has been built, else nullptr.
+    const Copy* find() {
+        int dev = 0;
+        if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
+        std::lock_guard<std::mutex> lock(mu_);
+        return lookup(dev);
+    }
+
+  private:
+    struct Table { const void* data; size_t bytes; };
+
+    const Copy* lookup(int dev) const {
+        for (const auto& c : copies_)
+            if (c->device == dev) return c.get();
+        return nullptr;
+    }
+    int build(Copy& c) const {
+        SB_CUDA(cudaDeviceGetAttribute(&c.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, c.device));
+        SB_CUDA(cudaDeviceGetAttribute(&c.num_sms, cudaDevAttrMultiProcessorCount, c.device));
+        for (const Table& t : tables_) {
+            void* d = nullptr;   // at least one byte, so that an empty table still gets a valid pointer
+            SB_CUDA(cudaMalloc(&d, std::max<size_t>(1, t.bytes)));
+            c.ptr.push_back(d);
+            if (t.bytes) SB_CUDA(cudaMemcpy(d, t.data, t.bytes, cudaMemcpyHostToDevice));
+        }
+        return SB_OK;
+    }
+    static void free_copy(const Copy& c) {
+        for (void* p : c.ptr) cudaFree(p);
+    }
+
+    std::mutex mu_;
+    std::vector<Table> tables_;
+    std::vector<std::unique_ptr<Copy>> copies_;   // one per device; never moved, so get()'s pointer stays valid
+};
 
 // Row-wise element kernels: blockDim = (tx, ty) with tx = row length rounded up to a warp (<= 256) and ty rows per CTA;
 // a CTA walks rows (64-bit row index once per row), threads walk columns with 32-bit arithmetic only.

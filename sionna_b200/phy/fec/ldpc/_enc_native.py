@@ -1,35 +1,22 @@
 """Owns one ``sb_ldpc5g_encoder`` handle (CSR tables of the RU sub-matrices + transmit gather)."""
-import ctypes as C
 import numpy as np
 import torch
 
-from ...._lib import lib, check, ptr, current_stream
+from ...._lib import Handle, lib, check, ptr, current_stream
 from .encoding import _csr_lists
 
 
-class EncoderHandle:
+class EncoderHandle(Handle):
     def __init__(self, enc):
         a, b_inv, c1, c2 = enc._ru_submatrices()
-        self._tabs = [np.ascontiguousarray(t, np.int32) for m in (a, b_inv, c1, c2) for t in _csr_lists(m)]
-        self._tx = np.ascontiguousarray(enc._tx_vn(), np.int32)
-        self._h = C.c_void_p()
+        tabs = [np.ascontiguousarray(t, np.int32) for m in (a, b_inv, c1, c2) for t in _csr_lists(m)]
+        tabs.append(np.ascontiguousarray(enc._tx_vn(), np.int32))
+        super().__init__("ldpc5g_encoder", enc.k, enc.n, enc.k_ldpc, enc.n_ldpc, 4 * enc.z, *(ptr(t) for t in tabs))
         self.k, self.n = enc.k, enc.n
-        t = self._tabs
-        check(lib().sb_ldpc5g_encoder_create(C.byref(self._h), enc.k, enc.n, enc.k_ldpc, enc.n_ldpc, 4 * enc.z,
-                                             ptr(t[0]), ptr(t[1]), ptr(t[2]), ptr(t[3]), ptr(t[4]), ptr(t[5]),
-                                             ptr(t[6]), ptr(t[7]), ptr(self._tx)), "sb_ldpc5g_encoder_create")
 
     def encode(self, u):
         if u.dtype != torch.float32:
             raise NotImplementedError("sb_ldpc5g_encode is an fp32 kernel; precision='double' is not available.")
         c = torch.empty((u.shape[0], self.n), dtype=torch.float32, device=u.device)
-        check(lib().sb_ldpc5g_encode(self._h, ptr(u), u.shape[0], ptr(c), current_stream()), "sb_ldpc5g_encode")
+        check(lib().sb_ldpc5g_encode(self.handle, ptr(u), u.shape[0], ptr(c), current_stream()), "sb_ldpc5g_encode")
         return c
-
-    def __del__(self):
-        try:
-            if self._h:
-                lib().sb_ldpc5g_encoder_destroy(self._h)
-                self._h = C.c_void_p()
-        except Exception:
-            pass

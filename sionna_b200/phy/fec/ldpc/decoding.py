@@ -7,7 +7,6 @@ codeword with the codeword's edge messages resident in shared memory for every i
 (:1431-1475) and output slicing / re-interleaving (:1486-1536) are folded into the kernel's load and store
 index maps, so the decoder moves 4*n bytes in and 4*k (or 4*n) bytes out per codeword and nothing else.
 """
-import ctypes as C
 import os
 import types
 import numpy as np
@@ -16,7 +15,7 @@ import scipy.sparse  # noqa: F401
 import torch
 
 from ...block import Block
-from ...._lib import lib, check, ptr, current_stream
+from ...._lib import Handle, lib, check, ptr, current_stream
 from .encoding import LDPC5GEncoder
 
 _CN_RULES = {"boxplus-phi": 0, "boxplus": 1, "minsum": 2, "min": 2, "offset-minsum": 3, "identity": 4}
@@ -27,12 +26,11 @@ def _i32(a):
     return np.ascontiguousarray(np.asarray(a), dtype=np.int32)
 
 
-class _GraphHandle:
-    """Owns one ``sb_ldpc_graph`` (host plan + lazily uploaded device tables)."""
+class _GraphHandle(Handle):
+    """Owns one ``sb_ldpc_graph`` (host plan + per-device copies of its tables)."""
 
     def __init__(self, num_cn, num_vn, cn_idx, vn_idx, in_map=None, n_in=0, out_vn=None, n_out=0, schedule=None,
                  cn_view=None):
-        self._h = C.c_void_p()
         cn_idx, vn_idx = _i32(cn_idx), _i32(vn_idx)
         in_map = None if in_map is None else _i32(in_map)
         out_vn = None if out_vn is None else _i32(out_vn)
@@ -40,38 +38,31 @@ class _GraphHandle:
         if schedule is not None:
             schedule = _i32(schedule)
             n_sub, n_active = schedule.shape
+        args = (num_cn, num_vn, len(vn_idx), ptr(cn_idx), ptr(vn_idx), ptr(in_map), int(n_in), ptr(out_vn), int(n_out),
+                ptr(schedule), int(n_sub), int(n_active))
         if cn_view is None:
-            check(lib().sb_ldpc_graph_create(C.byref(self._h), num_cn, num_vn, len(vn_idx), ptr(cn_idx), ptr(vn_idx),
-                                             ptr(in_map), int(n_in), ptr(out_vn), int(n_out), ptr(schedule),
-                                             int(n_sub), int(n_active)), "sb_ldpc_graph_create")
+            super().__init__("ldpc_graph", *args)
         else:
             cn_view = _i32(cn_view)
-            check(lib().sb_ldpc_graph_create_ordered(C.byref(self._h), num_cn, num_vn, len(vn_idx), ptr(cn_idx),
-                                                     ptr(vn_idx), ptr(in_map), int(n_in), ptr(out_vn), int(n_out),
-                                                     ptr(schedule), int(n_sub), int(n_active), ptr(cn_view)),
-                  "sb_ldpc_graph_create_ordered")
+            super().__init__("ldpc_graph", *args, ptr(cn_view), create="sb_ldpc_graph_create_ordered")
         self.num_edges = len(vn_idx)
         self.n_in = int(n_in) if in_map is not None else num_vn
         self.n_out = int(n_out) if out_vn is not None else num_vn
         self._ws = None
 
-    @property
-    def handle(self):
-        return self._h
-
     def on_chip(self):
-        return bool(lib().sb_ldpc_graph_on_chip(self._h))
+        return bool(lib().sb_ldpc_graph_on_chip(self.handle))
 
     def set_qc(self, z, base_row, base_col, shift):
         """Declare the lifted-base-graph structure (enables the index-free QC kernel); returns False if rejected."""
         r, c, s = _i32(base_row), _i32(base_col), _i32(shift)
-        return lib().sb_ldpc_graph_set_qc(self._h, int(z), len(r), ptr(r), ptr(c), ptr(s)) == 0
+        return lib().sb_ldpc_graph_set_qc(self.handle, int(z), len(r), ptr(r), ptr(c), ptr(s)) == 0
 
     def is_qc(self):
-        return bool(lib().sb_ldpc_graph_is_qc(self._h))
+        return bool(lib().sb_ldpc_graph_is_qc(self.handle))
 
     def workspace(self, device):
-        need = lib().sb_ldpc_workspace_bytes(self._h)
+        need = lib().sb_ldpc_workspace_bytes(self.handle)
         if need == 0:
             return None, 0
         if self._ws is None or self._ws.numel() < need or self._ws.device != device:
@@ -80,23 +71,15 @@ class _GraphHandle:
 
     def export(self):
         dims = np.zeros(10, np.int32)
-        check(lib().sb_ldpc_graph_export(self._h, ptr(dims), None, None, None, None, None, None), "export")
+        check(lib().sb_ldpc_graph_export(self.handle, ptr(dims), None, None, None, None, None, None), "export")
         c, n, e, lc, lv = (int(x) for x in dims[:5])
         out = {"dims": dims, "cn_order": np.zeros(c, np.int32), "vn_order": np.zeros(n, np.int32),
                "slot_of_edge": np.zeros(e, np.int32), "vn_slot": np.zeros(e, np.int32),
                "cn_off": np.zeros(lc + 1, np.int32), "vn_off": np.zeros(lv + 1, np.int32)}
-        check(lib().sb_ldpc_graph_export(self._h, ptr(dims), ptr(out["cn_order"]), ptr(out["vn_order"]),
+        check(lib().sb_ldpc_graph_export(self.handle, ptr(dims), ptr(out["cn_order"]), ptr(out["vn_order"]),
                                          ptr(out["slot_of_edge"]), ptr(out["vn_slot"]), ptr(out["cn_off"]),
                                          ptr(out["vn_off"])), "export")
         return out
-
-    def __del__(self):
-        try:
-            if self._h:
-                lib().sb_ldpc_graph_destroy(self._h)
-                self._h = C.c_void_p()
-        except Exception:  # interpreter shutdown
-            pass
 
 
 class LDPCBPDecoder(Block):

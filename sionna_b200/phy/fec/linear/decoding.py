@@ -1,6 +1,5 @@
 """Ordered statistics decoding (mirror of fec/linear/decoding.py:14-478) on ``sb_osd_decode``
 (``csrc/linear_codes.cu``, DESIGN §3.13)."""
-import ctypes as C
 import itertools
 
 import numpy as np
@@ -8,23 +7,8 @@ import scipy as sp
 import torch
 
 from ...block import Block
-from ...._lib import lib, check, ptr, current_stream
+from ...._lib import Handle, lib, check, ptr, current_stream
 from ..utils import pcm2gm, make_systematic
-
-
-class _OSDCode:
-    """Owns an ``sb_osd_code`` handle: the host-validated, bit-packed full-rank generator."""
-
-    def __init__(self, gm):
-        gm = np.ascontiguousarray(gm, np.uint8)
-        h = C.c_void_p()
-        check(lib().sb_osd_code_create(C.byref(h), ptr(gm), gm.shape[0], gm.shape[1]), "sb_osd_code_create")
-        self.handle = h
-
-    def __del__(self):
-        if getattr(self, "handle", None):
-            lib().sb_osd_code_destroy(self.handle)
-            self.handle = None
 
 
 class OSDecoder(Block):
@@ -96,7 +80,8 @@ class OSDecoder(Block):
         if num_symbols > 1e11:
             raise ResourceWarning("Due to its high complexity, OSD is not feasible for the selected parameters. "
                                   "Please consider using a smaller value for t.")
-        self._code = _OSDCode(gm_np)
+        gm = np.ascontiguousarray(gm_np, np.uint8)
+        self._code = Handle("osd_code", ptr(gm), *gm.shape)   # the host-validated, bit-packed generator
 
     @property
     def gm(self):

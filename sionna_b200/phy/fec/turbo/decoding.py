@@ -1,39 +1,16 @@
 """Turbo decoder (mirror of fec/turbo/decoding.py:15-435) on ``sb_turbo_decode`` (``csrc/conv.cu``, DESIGN §3.12): one
 ``sb_gather_rows`` depunctures and splits the codeword into the two component codewords, one launch runs every
 iteration of both BCJR component decoders."""
-import ctypes as C
 
 import numpy as np
 import torch
 
 from ...block import Block
-from ...._lib import lib, check, ptr, current_stream
+from ...._lib import Handle, lib, check, ptr, current_stream
 from ..conv.utils import Trellis, _trellis_tables
 from ..interleaving import RandomInterleaver, Turbo3GPPInterleaver
 from .encoding import interleaver_perm, turbo_layout, dev_i32, gather
 from .utils import polynomial_selector, puncture_pattern, TurboTermination
-
-
-class _TurboPerm:
-    """Owns one ``sb_turbo_perm`` handle (the interleaver, checked by the library to be a permutation)."""
-
-    def __init__(self, perm):
-        self._h = C.c_void_p()
-        p = np.ascontiguousarray(perm, np.int32)
-        check(lib().sb_turbo_perm_create(C.byref(self._h), ptr(p), len(p)), "sb_turbo_perm_create")
-
-    @property
-    def handle(self):
-        return self._h
-
-    def __del__(self):
-        h = getattr(self, "_h", None)
-        if h is not None and h.value:
-            try:
-                lib().sb_turbo_perm_destroy(h)
-            except Exception:                               # interpreter shutdown
-                pass
-            self._h = None
 
 
 class TurboDecoder(Block):
@@ -169,7 +146,8 @@ class TurboDecoder(Block):
         perm = interleaver_perm(self.internal_interleaver, k)
         demux[2 * T + 2 * np.arange(k)] = rank[3 * perm]              # decoder 2's systematic LLRs, through pi
         self._demux = dev_i32(demux)
-        self._perm = _TurboPerm(perm)
+        perm = np.ascontiguousarray(perm, np.int32)
+        self._perm = Handle("turbo_perm", ptr(perm), len(perm))   # checked by the library to be a permutation
 
     def call(self, llr_ch, /):
         if llr_ch.shape[-1] != self._n:
@@ -179,7 +157,7 @@ class TurboDecoder(Block):
         k, T = self._k, self._convenc_numsyms
         y = llr_ch.to(device=self.device, dtype=torch.float32).reshape(-1, self._n).contiguous()
         batch = y.shape[0]
-        y2 = gather(y, self._demux, 1, 4 * T, self._n)               # [batch, 1, 2 * 2T]: both component codewords
+        y2 = gather(y, self._demux.to(y.device), 1, 4 * T, self._n)  # [batch, 1, 2 * 2T]: both component codewords
         out = torch.empty((batch, k), dtype=torch.float32, device=y.device)
         nbytes = lib().sb_turbo_workspace_bytes(batch, k, int(self._terminate), self._ns)
         ws = torch.empty(nbytes, dtype=torch.uint8, device=y.device) if nbytes else None
