@@ -96,6 +96,9 @@ void sb_ldpc_graph_destroy(sb_ldpc_graph* g);
 int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entries, const int32_t* h_base_row,
                          const int32_t* h_base_col, const int32_t* h_shift);
 int sb_ldpc_graph_is_qc(const sb_ldpc_graph* g);
+/* 1 if boxplus-phi decodes of this QC graph skip the work that the punctured columns make exact in iterations 0 and 1:
+ * every block row has a punctured column (no channel input) among its first two entries. */
+int sb_ldpc_graph_qc_opening(const sb_ldpc_graph* g);
 /* Test hook: phi(x) of decoding.py:1110-1120 evaluated on the device by the scalar and by the packed-fp32x2 code path
  * (n even); both must equal the CPU oracle bit for bit. */
 int sb_debug_phi(const float* d_x, float* d_scalar, float* d_packed, int64_t n, void* stream);

@@ -26,6 +26,7 @@ SIGNATURES = {
     "sb_ldpc_graph_destroy": (None, [vp]),
     "sb_ldpc_graph_set_qc": (i32, [vp, i32, i32, vp, vp, vp]),
     "sb_ldpc_graph_is_qc": (i32, [vp]),
+    "sb_ldpc_graph_qc_opening": (i32, [vp]),
     "sb_debug_phi": (i32, [vp, vp, vp, i64, vp]),
     "sb_ldpc_graph_on_chip": (i32, [vp]),
     "sb_ldpc_workspace_bytes": (sz, [vp]),

@@ -81,6 +81,8 @@ struct QcParams {
     const int2* row_edge;    // [nnz] per base entry (processing order): {column * Z, shift}  (syndrome pass only)
     int tab_rep;             // copies of the phi log table in shared memory (16, 8 or 1; 0: rule does not use it)
     float offset, llr_max;
+    int open;                // boxplus-phi: run the opening iterations 0 and 1 on the punctured columns (see cn_open_pass)
+    const int* open_tab;     // [n_rows] punctured edge positions of each row (bit l: edge l), then [n_cols] punctured flags
 };
 
 // Message invariant of this kernel: a v2c message is never -0.0f. The initial v2c is canonicalised (llr + 0.0f) and
@@ -447,7 +449,7 @@ __device__ __forceinline__ float vn_qc(uint32_t ce_s, int deg, const VnLane& vl,
 }
 
 // Loop form for any degree. MODE 0: the update; MODE 1: initialisation v2c = llr (decoding.py:571), canonical +0.0 for
-// punctured bits (llr = -0.0).
+// punctured bits (llr = -0.0); MODE 2: `llr` stored on every edge as it is (vn_init's pass-1 words).
 template <int MODE>
 __device__ __forceinline__ float vn_qc_loop(uint32_t ce_s, int deg, const VnLane& vl, float llr, float clip) {
     float acc = 0.f;
@@ -462,7 +464,7 @@ __device__ __forceinline__ float vn_qc_loop(uint32_t ce_s, int deg, const VnLane
         const int2 e = lds_i2(ce_s + 8 * k);
         const uint32_t a = vn_addr(e, vl);
         if (vn_in_row(e, a, vl))
-            sts_f32(a, (MODE == 1) ? __fadd_rn(llr, 0.f) : clipf(__fadd_rn(-lds_f32(a), x_tot), clip));
+            sts_f32(a, (MODE == 1) ? __fadd_rn(llr, 0.f) : (MODE == 2) ? llr : clipf(__fadd_rn(-lds_f32(a), x_tot), clip));
     }
     return x_tot;
 }
@@ -702,12 +704,124 @@ __device__ __forceinline__ void vn_all(const QcParams& p, const WarpCtx& w, cons
 
 // v2c = llr on every edge (decoding.py:571), once per codeword. One class-agnostic loop over the warp's columns in loop
 // form: the unrolled classes are the iterations' code, and a second copy of them for this pass only made the kernel
-// larger (it is bound by instruction fetch).
+// larger (it is bound by instruction fetch). The message is the canonical llr + 0 (+0.0 for punctured bits, whose llr
+// is -0.0). `staged` (the opening iterations, cn_open_pass): the edges get the pass-1 word phi(|v2c|) | sign(v2c)
+// instead, one phi per VN rather than one per edge.
+template <class LT>
 __device__ __forceinline__ void vn_init(const QcParams& p, const WarpCtx& w, const VnLane& vl, const float* llr_s,
-                                        const int4* s_col, uint32_t s_ce) {
+                                        const int4* s_col, uint32_t s_ce, bool staged, const LT& lt) {
     for (int cc = w.grp; cc < p.n_cols; cc += w.G) {
         const int4 ci = s_col[cc];
-        if (w.lane_i < ci.z) vn_qc_loop<1>(s_ce + 8 * ci.x, ci.y, vl, llr_s[ci.w + w.lane_i], 0.f);
+        if (w.lane_i >= ci.z) continue;
+        const float llr = llr_s[ci.w + w.lane_i];
+        if (staged) {
+            float P = 0.f;                                // unused
+            const unsigned st = phi_pass1(__float_as_uint(__fadd_rn(llr, 0.f)), P, lt);
+            vn_qc_loop<2>(s_ce + 8 * ci.x, ci.y, vl, __uint_as_float(st), 0.f);
+        } else {
+            vn_qc_loop<1>(s_ce + 8 * ci.x, ci.y, vl, llr, 0.f);
+        }
+    }
+}
+
+// ---- the opening iterations of boxplus-phi on graphs with punctured columns ----------------------------------------
+// Rate recovery gives a punctured VN the channel LLR -0.0, so its first v2c is +0 and phi(+0) = phi_max ~ 16.97. When
+// every row holds a punctured edge (the host planner decides, open_tab), iteration 0 is mostly an exact no-op:
+//   * CN: for an edge e other than a row's only punctured edge, P - p_e still contains a phi_max, so P - p_e >=
+//     SB_PHI_ZERO and its c2v is +-0 exactly. Only the punctured edge of a row with a single punctured edge needs
+//     phi(P - p_e); the punctured edges of the other rows get +-0.
+//   * VN: a non-punctured VN receives only +-0, so x_tot = (+0 + +-0 + ...) + llr = llr and its new v2c is llr + 0,
+//     its first v2c again (the fused degree-1 update as well). Only the punctured columns change.
+// So vn_init writes the pass-1 words of every edge, iteration 0 sums them into P without evaluating phi (the same
+// values in the same ascending order as pass 1, so P is bit-identical) and writes only the punctured edges, and its VN
+// phase (vn_open) updates only the punctured columns. The other edges still hold their pass-1 words in iteration 1,
+// which evaluates phi(|x|) only at the punctured edges before its usual pass 2 and fused update. Iteration 0 raises no
+// saturation flag: edge 0 or 1 of every row is punctured (host condition), so its first-pair probe sees |x| = 0.
+// Iteration 1 probes like the plain variant, reading the first v2c of a non-punctured edge from the channel LLRs.
+// One out-of-line routine for both iterations and every degree, like cn_phi_qc (the kernel is instruction-fetch bound).
+template <class LT>
+__device__ __noinline__ void cn_phi_open(float* pm, int Z, int deg, unsigned punct, bool second, float clip, LT lt) {
+    float P = 0.f;
+    unsigned u = second ? punct : 0u;                     // iteration 1: the punctured edges hold v2c, stage them
+    for (; u & (u - 1); u &= u - 1) {
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        u &= u - 1;
+        float* q1 = pm + (__ffs(u) - 1) * Z;
+        const uint2 w = phi_pass1_pair(ldw(q0), ldw(q1), P, lt, [](float, float) {});
+        stw(q0, w.x);
+        stw(q1, w.y);
+    }
+    if (u) {
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        stw(q0, phi_pass1(ldw(q0), P, lt));
+    }
+    P = 0.f;
+    unsigned par = 0;
+    for (int l = 0; l < deg; ++l) {                       // P in ascending VN order, as pass 1 sums it
+        const unsigned w = ldw(pm + l * Z);
+        par ^= w;
+        P = __fadd_rn(P, __uint_as_float(w & 0x7fffffffu));
+    }
+    par &= 0x80000000u;
+    if (!second && (punct & (punct - 1))) {               // iteration 0, two or more punctured edges: outputs +-0
+        for (u = punct; u; u &= u - 1) {
+            float* q0 = pm + (__ffs(u) - 1) * Z;
+            stw(q0, (ldw(q0) ^ par) & 0x80000000u);
+        }
+        return;
+    }
+    // pass 2 on every edge (iteration 1) or on the single punctured edge (iteration 0)
+    for (u = second ? 0xffffffffu >> (32 - deg) : punct; u & (u - 1); u &= u - 1) {
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        u &= u - 1;
+        float* q1 = pm + (__ffs(u) - 1) * Z;
+        const uint2 y = phi_pass2_pair(ldw(q0), ldw(q1), P, par, clip, lt);
+        stw(q0, y.x);
+        stw(q1, y.y);
+    }
+    if (u) {
+        float* q0 = pm + (__ffs(u) - 1) * Z;
+        stw(q0, phi_pass2(ldw(q0), P, par, clip, lt));
+    }
+}
+
+// CN phase of iteration 0 (second = false) or 1 of the opening path: the warp's rows as in cn_vote_pass.
+template <class LT>
+__device__ __forceinline__ void cn_open_pass(const QcParams& p, const WarpCtx& w, float* msg, const float* llr_s,
+                                             const int4* s_row, float clip, bool second, int* sat_flag, const LT& lt) {
+    const int Z = p.Z;
+    for (int rr = w.grp; rr < p.n_rows; rr += w.G) {
+        const int4 ri = s_row[rr];
+        if (w.lane_i < ri.z) {
+            const unsigned punct = (unsigned)__ldg(p.open_tab + rr);
+            float* pm = msg + ri.x * Z + w.lane_i;
+            if (second && ri.y >= 2) {                    // the plain variant's probe on |x| of edges 0 and 1
+                auto mag = [&](int l) {
+                    if ((punct >> l) & 1u) return fabsf(pm[l * Z]);
+                    const int2 e = __ldg(p.row_edge + ri.x + l);
+                    int j = w.lane_i + e.y;
+                    j -= (j >= Z) ? Z : 0;
+                    return fabsf(llr_s[e.x + j]);
+                };
+                const float a0 = mag(0), a1 = mag(1);
+                if (__all_sync(__activemask(), a0 >= SB_PHI_HI && a1 >= SB_PHI_HI)) *sat_flag = 1;
+            }
+            cn_phi_open<LT>(pm, Z, ri.y, punct, second, clip, lt);
+            if (second && ri.w >= 0) {
+                float* q = pm + (ri.y - 1) * Z;
+                fused_vn(p, q, *q, ri.w, w.lane_i, llr_s, clip, nullptr);
+            }
+        }
+    }
+}
+
+// VN phase of iteration 0 of the opening path: the punctured columns only, in loop form (once per codeword)
+__device__ __forceinline__ void vn_open(const QcParams& p, const WarpCtx& w, const VnLane& vl, const float* llr_s,
+                                        const int4* s_col, uint32_t s_ce, float clip) {
+    for (int cc = w.grp; cc < p.n_cols; cc += w.G) {
+        const int4 ci = s_col[cc];
+        if (__ldg(p.open_tab + p.n_rows + cc) && w.lane_i < ci.z)
+            vn_qc_loop<0>(s_ce + 8 * ci.x, ci.y, vl, llr_s[ci.w + w.lane_i], clip);
     }
 }
 
@@ -763,6 +877,9 @@ __global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_
     const float clip = p.llr_max;
     const float phi_max = sb_phif(0.f);                   // phi at its lower clipping bound (global-memory table)
     uint32_t tma_phase = 0;
+    // opening iterations 0 and 1 (cn_open_pass); neither is the final one. The early-termination variant keeps the
+    // plain path: its hard decisions come from the VN phase of every column.
+    const bool open = RULE == SB_CN_BOXPLUS_PHI && !EARLY && p.open && p.num_iter >= 3;
 
     for (long long b = blockIdx.x; b < p.B; b += gridDim.x) {
         // ---- channel LLRs in natural VN order, staged in the message array ---------------------------------------
@@ -771,7 +888,7 @@ __global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_
         __syncthreads();
         if (tid == 0) *sat_flag = 0;
         // ---- v2c = llr of the edge's VN (decoding.py:571) ---------------------------------------------------------
-        vn_init(p, w, vl, llr_s, s_col, s_ce);
+        vn_init(p, w, vl, llr_s, s_col, s_ce, open, lt);
         __syncthreads();
         if (p.num_iter == 0) {                           // x_hat = llr_ch (decoding.py:603-608)
             for (int v = tid; v < N; v += T) {
@@ -799,14 +916,16 @@ __global__ void __launch_bounds__(kQcThreads, 1) ldpc_bp_qc_kernel(const __grid_
                 asm volatile("cp.async.bulk.prefetch.L2.global [%0], %1;" ::"l"(p.llr + (size_t)(b + gridDim.x) * p.n_in),
                              "r"((uint32_t)p.n_in * 4u) : "memory");
             if constexpr (RULE == SB_CN_BOXPLUS_PHI) {
-                if (sc) cn_vote_pass(p, w, msg, llr_s, s_row, clip, !final_pass, phi_max, sat_flag, lt, hd);
+                if (open && it < 2) cn_open_pass(p, w, msg, llr_s, s_row, clip, it == 1, sat_flag, lt);
+                else if (sc) cn_vote_pass(p, w, msg, llr_s, s_row, clip, !final_pass, phi_max, sat_flag, lt, hd);
                 else cn_all<RULE>(p, w, msg, llr_s, s_row, clip, !final_pass, sat_flag, lt, hd);
             } else {
                 cn_all<RULE>(p, w, msg, llr_s, s_row, clip, !final_pass, sat_flag, lt, hd);
             }
             __syncthreads();
             // ---- VN phase ---------------------------------------------------------------------------------------
-            vn_all<true>(p, w, vl, llr_s, s_col, s_ce, clip, final_pass, final_pass, b, hd);
+            if (open && it == 0) vn_open(p, w, vl, llr_s, s_col, s_ce, clip);
+            else vn_all<true>(p, w, vl, llr_s, s_col, s_ce, clip, final_pass, final_pass, b, hd);
             __syncthreads();
         }
         if (EARLY && p.iters_out && tid == 0) p.iters_out[b] = limit;
@@ -979,14 +1098,35 @@ extern "C" int sb_ldpc_graph_set_qc(sb_ldpc_graph* g, int32_t Z, int32_t n_entri
         int r = g->h_cn[e] / Z, i = g->h_cn[e] % Z, c = g->h_vn[e] / Z;
         slot[e] = be_of[(size_t)r * n_cols + c] * Z + i;
     }
-    g->qc = true; g->qc_Z = Z; g->qc_rows = n_rows; g->qc_cols = n_cols; g->qc_nnz = nnz;
+    // Opening iterations of boxplus-phi (cn_open_pass): the punctured columns are those whose every VN gets no channel
+    // input (in_idx -1, LLR 0). The path is on when every row has a punctured edge at position 0 or 1 (which keeps the
+    // first-pair probe of iteration 0 silent) and at most 32 edges (one mask word), and no punctured column is fused.
+    std::vector<int> open_tab(n_rows + n_cols, 0);
+    bool open = true;
+    std::vector<char> punct(n_cols, 1);
+    for (int c = 0; c < n_cols; ++c)
+        for (int v = c * Z; v < c * Z + zcol(c); ++v) punct[c] = punct[c] && in_nat[v] == -1;
+    for (int rr = 0; rr < n_rows; ++rr) {
+        const int r = rorder[rr];
+        unsigned m = 0;
+        for (size_t l = 0; l < by_row[r].size() && l < 32; ++l) m |= (unsigned)punct[by_row[r][l].c] << l;
+        open = open && rdeg[r] <= 32 && (m & 3u);
+        open_tab[rr] = (int)m;
+    }
+    for (int cc = 0; cc < n_cols; ++cc) {
+        open_tab[n_rows + cc] = punct[corder[cc]];
+        open = open && !(punct[corder[cc]] && col_fused[corder[cc]]);
+    }
+    g->qc = true;
+    g->qc_open = open;
+    g->qc_open_tab.swap(open_tab); g->qc_Z = Z; g->qc_rows = n_rows; g->qc_cols = n_cols; g->qc_nnz = nnz;
     g->qc_max_row_deg = *std::max_element(rdeg.begin(), rdeg.end());
     g->qc_max_col_deg = *std::max_element(cdeg.begin(), cdeg.end());
     g->qc_row_info.swap(row_info); g->qc_col_info.swap(col_info); g->qc_col_edge.swap(col_edge);
     g->qc_row_cls_end = row_cls_end; g->qc_col_cls_end = col_cls_end;
     g->qc_in_idx.swap(in_nat); g->qc_out_pos.swap(out_nat); g->qc_slot_of_edge.swap(slot); g->qc_row_edge.swap(row_edge);
     g->qc_tables.set(g->qc_row_info, g->qc_col_info, g->qc_col_edge, g->qc_in_idx, g->qc_out_pos, g->qc_slot_of_edge,
-                     g->qc_row_edge);
+                     g->qc_row_edge, g->qc_open_tab);
     return SB_OK;
 }
 
@@ -1014,6 +1154,7 @@ extern "C" int sb_debug_phi(const float* d_x, float* d_scalar, float* d_packed, 
 }
 
 extern "C" int sb_ldpc_graph_is_qc(const sb_ldpc_graph* g) { return g && g->qc ? 1 : 0; }
+extern "C" int sb_ldpc_graph_qc_opening(const sb_ldpc_graph* g) { return g && g->qc && g->qc_open ? 1 : 0; }
 
 int sb_qc_try_decode(const sb_ldpc_graph* g, const DeviceTables::Copy& dev, const float* d_llr, int64_t batch,
                      int32_t num_iter, int32_t cn_rule, int32_t vn_rule, float offset, float llr_max, int32_t hard_out,
@@ -1044,6 +1185,9 @@ int sb_qc_try_decode(const sb_ldpc_graph* g, const DeviceTables::Copy& dev, cons
     p.llr = d_llr; p.out = d_out; p.state_out = d_state_out; p.B = batch; p.num_iter = num_iter; p.hard_out = hard_out;
     p.offset = offset; p.llr_max = llr_max; p.tab_rep = tab_rep;
     p.early = early; p.iters_out = d_iters; p.row_edge = d->at<int2>(6);
+    // the opening path needs c2v = fminf(+0, clip) = +0, i.e. a clipping bound >= 0
+    p.open = cn_rule == SB_CN_BOXPLUS_PHI && g->qc_open && llr_max >= 0.f;
+    p.open_tab = d->at<int>(7);
     p.use_tma = (g->n_in % 4 == 0) && (g->n_in <= p.E_alloc) && ((reinterpret_cast<uintptr_t>(d_llr) & 15) == 0);
     const int Zb = (g->qc_Z + 31) / 32;                    // 32-lane slices per block row (<= 12 for Z <= 384)
     const int max_warps = kQcThreads / 32;

@@ -25,7 +25,10 @@ struct sb_ldpc_graph {
     std::vector<int> qc_in_idx, qc_out_pos, qc_slot_of_edge;   // natural VN order / reference edge order
     std::vector<int> qc_row_edge;   // int2 per base entry (processing order): {column * Z, shift} for the syndrome pass
     std::vector<int> qc_row_cls_end, qc_col_cls_end;   // class boundaries in processing order (ldpc_bp_qc.cu)
-    // device copies of qc_row_info, qc_col_info, qc_col_edge, qc_in_idx, qc_out_pos, qc_slot_of_edge, qc_row_edge
+    bool qc_open = false;           // boxplus-phi runs its opening iterations on the punctured columns (ldpc_bp_qc.cu)
+    std::vector<int> qc_open_tab;   // per row (processing order): punctured edge positions as a bit mask; then per col: punctured
+    // device copies of qc_row_info, qc_col_info, qc_col_edge, qc_in_idx, qc_out_pos, qc_slot_of_edge, qc_row_edge,
+    // qc_open_tab
     mutable DeviceTables qc_tables;
 };
 

@@ -61,6 +61,9 @@ class _GraphHandle(Handle):
     def is_qc(self):
         return bool(lib().sb_ldpc_graph_is_qc(self.handle))
 
+    def qc_opening(self):
+        return bool(lib().sb_ldpc_graph_qc_opening(self.handle))
+
     def workspace(self, device):
         need = lib().sb_ldpc_workspace_bytes(self.handle)
         if need == 0:
