@@ -675,6 +675,40 @@ void sb_osd_code_destroy(sb_osd_code* p);
  * access; batch = 0 is SB_OK with NULL pointers. */
 int sb_osd_decode(const sb_osd_code* code, const float* d_llr, float* d_out, int64_t batch, int32_t t, void* stream);
 
+/* ------------------------------------------------------------------------------------------------
+ * Signal: FIR filters, windows, power spectral density (csrc/signal.cu)
+ * replaces convolve                              signal/utils.py:11-159
+ *          Filter.call (window, normalisation, conjugation)   signal/filter.py:268-285
+ *          Window.call                           signal/window.py:145-163
+ *          empirical_psd (mean of |X|^2)         signal/utils.py:251-311
+ * ---------------------------------------------------------------------------------------------- */
+enum { SB_CONV_WINDOW_NORMALIZE = 1, SB_CONV_NORMALIZE = 2, SB_CONV_CONJUGATE = 4 };
+/* y[r, m] = sum_{k < K} h'[k] x[r, m + offset - k] (x = 0 outside [0, n)), m in [0, out_len): "full" is offset 0,
+ * out_len n + K - 1; "same" offset (K - 1) / 2, out_len n; "valid" offset K - 1, out_len n - K + 1.
+ * d_x [rows, n] and d_h [K] are real or complex (x_complex, h_complex), d_y [rows, out_len] complex if either is; all
+ * of one precision: 0 float32 (complex64), 1 float64 (complex128), computed natively in it. h' is prepared on chip
+ * from the raw taps in Filter.call's order: h' = h w~ with d_w [K] a real window or NULL (w~ = w / sqrt(mean(w^2))
+ * with SB_CONV_WINDOW_NORMALIZE, else w), divided by sqrt(sum |h w~|^2) with SB_CONV_NORMALIZE, then conjugated with
+ * SB_CONV_CONJUGATE (complex h only). Both sums are reduced in one fixed order. Bad shapes (n < 1, K < 1, out_len < 0,
+ * offset outside [0, K - 1], out_len > n + K - 1 - offset), unknown flags or precision, window normalisation without a
+ * window and missing pointers with rows > 0 return SB_EINVAL before any device access; rows = 0 is SB_OK with NULL
+ * pointers. */
+int sb_convolve(const void* d_x, int32_t x_complex, const void* d_h, int32_t h_complex, const void* d_w, void* d_y,
+                int32_t precision, int64_t rows, int32_t n, int32_t k, int32_t offset, int32_t out_len, int32_t flags,
+                void* stream);
+/* y[r, j] = w~[j] x[r, j], d_x / d_y [rows, n] real or complex (x_complex), d_w [n] real, one precision (0 float32,
+ * 1 float64); w~ = w / sqrt(mean(w^2)) with normalize = 1, else w. Malformed arguments return SB_EINVAL before any
+ * device access; rows = 0 is SB_OK with NULL pointers. */
+int sb_scale_last(const void* d_x, int32_t x_complex, const void* d_w, void* d_y, int32_t precision, int64_t rows,
+                  int32_t n, int32_t normalize, void* stream);
+/* d_psd[j] = (1 / rows) sum_r |d_x[r, j]|^2 over complex64 d_x [rows, n]: partial sums over fixed chunks of 1024 rows,
+ * added in chunk order, so the result is bit-identical from run to run and device to device. Needs
+ * sb_power_mean_workspace_bytes(rows, n) bytes of workspace (0 for rows <= 1024; SB_ENOMEM if smaller). rows < 1,
+ * n < 1 or missing pointers return SB_EINVAL before any device access. */
+int sb_power_mean(const float* d_x, float* d_psd, int64_t rows, int32_t n, void* d_workspace, size_t workspace_bytes,
+                  void* stream);
+size_t sb_power_mean_workspace_bytes(int64_t rows, int32_t n);
+
 #ifdef __cplusplus
 }
 #endif

@@ -101,6 +101,10 @@ SIGNATURES = {
     "sb_osd_code_create": (i32, [C.POINTER(vp), vp, i32, i32]),
     "sb_osd_code_destroy": (None, [vp]),
     "sb_osd_decode": (i32, [vp, vp, vp, i64, i32, vp]),
+    "sb_convolve": (i32, [vp, i32, vp, i32, vp, vp, i32, i64, i32, i32, i32, i32, i32, vp]),
+    "sb_scale_last": (i32, [vp, i32, vp, vp, i32, i64, i32, i32, vp]),
+    "sb_power_mean": (i32, [vp, vp, i64, i32, vp, sz, vp]),
+    "sb_power_mean_workspace_bytes": (sz, [i64, i32]),
 }
 
 

@@ -8,8 +8,8 @@ built with -fmad=false: their arithmetic is specified operation by operation (ex
 CPU oracle reproduces it bit for bit, and the compiler must not contract a*b+c on its own. The flat-fading source is
 built the same way so that its random draws and noise equal sb_awgn's (phy_kernels.cu) bit for bit, and the convolutional
 decoders so that their Viterbi path metrics equal the float32 oracle's bit for bit. The OFDM / MIMO / channel
-sources are tolerance-checked floating-point kernels (FFT butterflies, complex MACs, Cholesky): they are built with the
-default -fmad=true, which halves their instruction count.
+and signal sources are tolerance-checked floating-point kernels (FFT butterflies, complex MACs, Cholesky, FIR filters):
+they are built with the default -fmad=true, which halves their instruction count.
 """
 import os
 import subprocess
@@ -22,7 +22,7 @@ OBJ_DIR = os.path.join(HERE, "..", "..", "build", "obj")
 EXACT = ["common.cu", "ldpc_bp.cu", "ldpc_bp_qc.cu", "ldpc_bp_flat.cu", "ldpc_enc.cu", "phy_kernels.cu",
          "flat_fading.cu", "conv.cu", "linear_codes.cu"]                                         # -fmad=false
 FAST = ["ofdm_mimo.cu", "channel.cu", "frontend.cu", "mimo_ml.cu", "mimo_kbest.cu",
-        "mimo_iterative.cu", "precoding.cu"]                                                     # -fmad=true
+        "mimo_iterative.cu", "precoding.cu", "signal.cu"]                                        # -fmad=true
 SOURCES = EXACT + FAST
 HEADERS = ["sb_common.h", "sb_math.h", "sb_math2.cuh", "sb_logtab.h", "rng.cuh", "ldpc_graph.h", "ldpc_rules.cuh",
            "lmmse_diag.cuh", "dense_mimo.cuh", "demap_qam.cuh", "demap_prior.cuh", os.path.join("..", "..", "include", "sionna_b200.h")]

@@ -1,33 +1,7 @@
-"""Signal utilities on the hot path (mirror of /root/reference/src/sionna/phy/signal/utils.py:161-249): normalised DFTs."""
-import numpy as np
-import torch
-
-from ..config import config
-from ..._lib import lib, check, ptr, current_stream
-
-
-def _dft(x, axis, inverse):
-    dev = config.device
-    x = torch.as_tensor(x).to(device=dev, dtype=torch.complex64)
-    x = x.movedim(axis, -1).contiguous()
-    n = x.shape[-1]
-    rows = x.numel() // n
-    zero = torch.zeros(1, dtype=torch.int32, device=dev)
-    out = torch.empty_like(x)
-    if inverse:
-        check(lib().sb_ofdm_modulate(ptr(x), ptr(out), rows, 1, n, ptr(zero), ptr(zero), n, 0, current_stream()),
-              "sb_ofdm_modulate")
-    else:
-        check(lib().sb_ofdm_demodulate(ptr(x), ptr(out), rows, 1, n, ptr(zero), ptr(zero), n, 0, 0, current_stream()),
-              "sb_ofdm_demodulate")
-    return out.movedim(-1, axis)
-
-
-def fft(tensor, axis=-1, precision=None):
-    """Normalised DFT ``X_m = 1/sqrt(N) sum_n x_n exp(-j 2 pi m n / N)`` along ``axis`` (signal/utils.py:161-204)."""
-    return _dft(tensor, axis, False)
-
-
-def ifft(tensor, axis=-1, precision=None):
-    """Normalised IDFT ``x_n = 1/sqrt(N) sum_m X_m exp(j 2 pi m n / N)`` along ``axis`` (signal/utils.py:206-249)."""
-    return _dft(tensor, axis, True)
+"""Signal module (mirror of /root/reference/src/sionna/phy/signal/__init__.py): filters, windows, up/down-sampling,
+convolution, normalised DFTs and the empirical PSD / ACLR, on the kernels of ``csrc/signal.cu`` and the OFDM FFT."""
+from .utils import convolve, empirical_psd, empirical_aclr, fft, ifft
+from .window import Window, HannWindow, HammingWindow, CustomWindow, BlackmanWindow
+from .filter import Filter, RaisedCosineFilter, RootRaisedCosineFilter, CustomFilter, SincFilter
+from .upsampling import Upsampling
+from .downsampling import Downsampling
