@@ -63,8 +63,10 @@ def depuncture(y, k, mu, perm, rate=1 / 3, terminate=False):
 
 
 def decode(y, gen_poly, perm, rate=1 / 3, terminate=False, num_iter=6, algorithm="map", dtype=np.float64,
-           return_llr=True):
-    """APP logits [B, k] (or hard bits) of turbo logits y [B, n], the reference's iteration in `dtype`."""
+           return_llr=True, return_peak_ext=False):
+    """APP logits [B, k] (or hard bits) of turbo logits y [B, n], the reference's iteration in `dtype`. With
+    return_peak_ext also the largest |extrinsic LLR| [B] before the +-20 clip among those passed on to the other
+    decoder (decoder 1's of every iteration, decoder 2's of all but the last), which shows whether the clip bound."""
     mu = len(gen_poly[0]) - 1
     k = len(perm)
     pinv = np.argsort(perm)
@@ -74,12 +76,17 @@ def decode(y, gen_poly, perm, rate=1 / 3, terminate=False, num_iter=6, algorithm
     lch, lch2 = y1[:, 0:2 * k:2], y2[:, 0:2 * k:2]
     l1e = np.zeros((B, k + tz), dtype)
     l2i = np.zeros((B, k), dtype)
-    for _ in range(num_iter):
+    peak = np.zeros(B)
+    for i in range(num_iter):
         l1i = conv.bcjr(y1, gen_poly, True, terminate, algorithm, l1e, dtype)[:, :k]
         ex = ((l1i - lch).astype(dtype) - l1e[:, :k]).astype(dtype)
+        peak = np.maximum(peak, np.abs(ex).max(axis=1))
         l2e = np.concatenate([np.clip(ex[:, perm], -20, 20), np.zeros((B, tz), dtype)], 1).astype(dtype)
         l2i = conv.bcjr(y2, gen_poly, True, terminate, algorithm, l2e, dtype)[:, :k]
         ex = ((l2i - l2e[:, :k]).astype(dtype) - lch2).astype(dtype)
+        if i + 1 < num_iter:
+            peak = np.maximum(peak, np.abs(ex).max(axis=1))
         l1e = np.concatenate([np.clip(ex[:, pinv], -20, 20), np.zeros((B, tz), dtype)], 1).astype(dtype)
     out = l2i[:, pinv]
-    return out if return_llr else (out > 0).astype(np.float64)
+    out = out if return_llr else (out > 0).astype(np.float64)
+    return (out, peak) if return_peak_ext else out
